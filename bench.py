@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — the IndexTTS-2.5 per-segment hot path on B200 (BASELINE.json configs[1]).
+"""bench.py — the IndexTTS-2.5 per-segment hot path on H100 (BASELINE.json configs[1]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--quick]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one utterance through the whole per-segment pipeline of IndexTTS2.infer
@@ -44,11 +44,11 @@ AUDIO_S_PER_TOKEN = 2 * 1.72 * 256 / 22050.0
 def ncu_traffic():
     """DRAM bytes per decode step of the dominant kernel, from the committed ncu capture summary (tests/tools/ncu_metrics.py
     turns the .ncu-rep of `ncu --set full` into this JSON); null when no capture has been committed for this kernel."""
-    p = os.path.join(ROOT, "profiles", "r02_gpt_decode1_ncu.json")
+    p = os.path.join(ROOT, "profiles", "gpt_decode1_ncu.json")
     try:
         d = json.load(open(p))
         return float(d["dram_bytes_per_step"]), (f"dram__bytes_read.sum + dram__bytes_write.sum of one gpt_decode1_kernel launch / "
-                                                 f"{d['steps_per_launch']} steps, ncu --set full, profiles/r02_gpt_decode1_ncu.json")
+                                                 f"{d['steps_per_launch']} steps, ncu --set full, profiles/gpt_decode1_ncu.json")
     except Exception:
         return None, "no committed ncu capture of this kernel"
 
@@ -57,12 +57,12 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet (HBM3, dense bf16)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
 
     def __init__(self, gpu_index):
         self.idx = gpu_index
@@ -167,7 +167,7 @@ WORKLOAD = ("IndexTTS-2.5 infer_v2_5 batch=1 per GPU: 10 s reference (P=861), 32
 
 # -------------------------------------------------------------------------- cpu arm --
 DTYPE = ("bf16 GPT (bf16 weights/activations, fp32 accumulate, fp32 residual stream = the reference's use_bf16 autocast) + "
-         "tail on tcgen05 with fp16 operands (kind::f16: DiT / WaveNet / BigVGAN-resblock GEMMs and the DiT flash attention; "
+         "tail on wgmma with fp16 operands (.f16: DiT / WaveNet / BigVGAN-resblock GEMMs and the DiT flash attention; "
          "fp32 accumulate, fp32 softmax, fp32 residual streams and pointwise math) and tf32 over fp32 storage for the small "
          "rest (codec, length regulator, K=80 input convs, ConvTranspose upsamplers)")
 
@@ -233,7 +233,7 @@ def host_threads():
 def run_reference(args, rank, world):
     """`--impl reference`: the reference's own (CPU, fp32) implementation of the path — the oracle port; the reference
     itself cannot be built offline (DESIGN.md section 6) — on the box's host cores, SAME config, metric and unit as the
-    B200 arm.  Every step is the FULL config-2 utterance (~1 minute of CPU work), so --steps / --warmup are honoured only
+    GPU arm.  Every step is the FULL config-2 utterance (~1 minute of CPU work), so --steps / --warmup are honoured only
     as far as IDX_REF_BUDGET_S allows (default 300 s: "the whole run ends within a few minutes"); the line reports the
     steps that actually ran and says that the request was cut."""
     if rank != 0:
@@ -420,6 +420,15 @@ def job_line(workload, e, cfg, wg, dist, rank, world, local):
     return None
 
 
+def dump_outputs(d, codes, pcm16):
+    """The arrays a caller of the timed path receives, from its last step: 256 speech codes and 225 280 pcm16 samples
+    (0.9 MB as float32), so that two builds can be compared output for output on the same seeded inputs."""
+    os.makedirs(d, exist_ok=True)
+    pcm = pcm16.cpu().numpy() if torch.is_tensor(pcm16) else np.asarray(pcm16)
+    np.save(os.path.join(d, "codes.npy"), np.asarray(codes).astype(np.float64))
+    np.save(os.path.join(d, "pcm16.npy"), pcm.astype(np.float32))
+
+
 # ---------------------------------------------------------------------------- main --
 def main():
     ap = argparse.ArgumentParser()
@@ -431,6 +440,8 @@ def main():
     ap.add_argument("--no-config5", action="store_true", help="skip the config-5 job block of the default run")
     ap.add_argument("--workload", default="config2", choices=["config2", "config3", "config5"],
                     help="config2 (default): the batch-1 headline; config3 / config5: the fixed batch jobs, run once")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (speech codes, pcm16 samples) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -492,7 +503,7 @@ def main():
     g_ms = c_ms = v_ms = 0.0
     gpt_launch_ms, gpt_launches = 0.0, 0
     for _ in range(K):
-        run_utterance(e, mine, prompt_emb_d, host=False)
+        last = run_utterance(e, mine, prompt_emb_d, host=False)
         g, s = stage_breakdown(e)
         g_ms += g["prefill_ms"] + g["decode_ms"]
         gpt_launch_ms += g["decode_ms"]
@@ -504,6 +515,8 @@ def main():
     clocks = sampler.stop()
     t_dev = e.event_elapsed_ms(0, 1) / 1000.0
     launches = e.launches - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last)
     # ---- end to end: host buffers in, pcm16 out, gather on rank 0 ----
     if dist is not None:
         from indextts_b200.sharding import gather_wavs

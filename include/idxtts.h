@@ -1,5 +1,5 @@
 /*
- * idxtts.h — C-ABI of libidxtts.so, the B200 (sm_100a) compute library behind the
+ * idxtts.h — C-ABI of libidxtts.so, the H100 (sm_90a) compute library behind the
  * IndexTTS / IndexTTS2 `.infer()` entry points.
  *
  * Every entry point replaces one "module-level seam" of the reference pipeline
@@ -49,7 +49,7 @@ enum {
   IDX_ERR_CUDA = 1,     /* a CUDA runtime call or kernel failed                    */
   IDX_ERR_ARG = 2,      /* bad argument / shape / missing weight                    */
   IDX_ERR_STATE = 3,    /* call order violated (e.g. generate before finalize)      */
-  IDX_ERR_NOGPU = 4     /* no sm_100 device: there is NO CPU fallback, by design    */
+  IDX_ERR_NOGPU = 4     /* no sm_90 device: there is NO CPU fallback, by design     */
 };
 
 /* ------------------------------------------------------------------ lifecycle -- */
@@ -60,7 +60,7 @@ int idx_create(int device, idx_engine** out);
 void idx_destroy(idx_engine* e);
 /* Last error message of this engine (or of the failed idx_create when e == NULL).   */
 const char* idx_last_error(const idx_engine* e);
-/* Library/ABI version and build flags ("sm_100a;...").                              */
+/* Library/ABI version and build flags ("sm_90a;...").                               */
 const char* idx_version(void);
 /* Number of kernel launches issued by this engine since creation (bench.py reports
  * the delta over the timed region as `gpu_launches`).                               */
@@ -75,7 +75,7 @@ int idx_wait_stream(idx_engine* e, void* cuda_stream);
 int idx_event_record(idx_engine* e, int slot);
 int idx_event_elapsed_ms(idx_engine* e, int slot_a, int slot_b, double* ms);
 
-/* Engine options.  "gemm_backend": 0 = automatic (tcgen05 implicit GEMM wherever the shape
+/* Engine options.  "gemm_backend": 0 = automatic (wgmma implicit GEMM wherever the shape
  * allows — the default), 1 = SIMT fp32 everywhere (strict-fp32 parity runs).  "tail_f16" (with gemm_backend 0): 1 = the
  * DiT / WaveNet / BigVGAN-resblock GEMMs read fp16 operands (kind::f16; activations written as fp16 by the kernel that
  * produces them, fp32 accumulate and fp32 residual streams — the default), 0 = tf32 over fp32 storage (round 1).
@@ -283,7 +283,7 @@ int idx_bigvgan_last_ms(const idx_engine* e, double* ms);
 
 /* Diagnostic (tests): one multi-tap channels-last GEMM — the building block of every Conv1d /
  * ConvTranspose1d / Linear of the vocoder and s2mel paths — through a chosen back end
- * (backend 1 = SIMT fp32, 2 = tcgen05 tf32, 0 = automatic).  wk is K-major [N][taps*K];
+ * (backend 1 = SIMT fp32, 2 = wgmma tf32, 0 = automatic).  wk is K-major [N][taps*K];
  * D[b][m][n] = scale*(act(sum + bias) + res + (accum ? out : 0)) stored at
  * out[b*out_elems_per_batch + out_off + m*ldo + n] where 0 <= flat < out_valid.            */
 int idx_debug_conv_gemm(idx_engine* e, const float* A, int B, int Tin, int K, const float* wk,

@@ -1,4 +1,4 @@
-// bigvgan.cu — BigVGAN-v2 generator (22 kHz, 80 band, 256x) on sm_100a.
+// bigvgan.cu — BigVGAN-v2 generator (22 kHz, 80 band, 256x) on sm_90a.
 //
 // Replaces (SURVEY.md §8a row a12):
 //   BigVGAN.forward / AMPBlock1.forward   indextts/s2mel/modules/bigvgan/bigvgan.py:360-386,132-141
@@ -9,7 +9,7 @@
 //
 // Layout: activations are channels-last fp32 [B][T][C] so that
 //   * every Conv1d is a multi-tap GEMM with M = time, N = C_out, K = C_in (ops.h), zero padding
-//     comes from the row bounds of the A operand (TMA out-of-bounds fill on the tcgen05 path);
+//     comes from the row bounds of the A operand (TMA out-of-bounds fill on the wgmma path);
 //   * ConvTranspose1d(k = 2u, stride u, pad u/2) is the SAME 2-tap GEMM with N = u*C_out: output
 //     phase r of frame q lands at flat offset (q*u + r - pad)*C_out + co, i.e. the GEMM's row q
 //     is a contiguous run of the upsampled signal (shifted by -pad*C_out) — no scatter;

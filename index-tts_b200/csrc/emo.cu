@@ -1,4 +1,4 @@
-// emo.cu — emotion-vector path of UnifiedVoice (SURVEY.md §8a row a7) on sm_100a, fp32/tf32.
+// emo.cu — emotion-vector path of UnifiedVoice (SURVEY.md §8a row a7) on sm_90a, fp32/tf32.
 //
 // Replaces:
 //   merge_emovec / get_emovec / get_emo_conditioning   indextts/gpt/model_v2.py:827-838,588-593
@@ -8,7 +8,7 @@
 //   PerceiverResampler (1 latent, GEGLU FF, RMSNorm)    indextts/gpt/perceiver.py:140-317
 // The reference recomputes this for every text segment with identical inputs (trap P11); callers cache the
 // result per (speaker, emotion, alpha), so it runs once per reference audio.  All GEMMs go through
-// conv_gemm (tcgen05 tf32 where the shape allows); lengths follow the reference's all-valid mask (P10).
+// conv_gemm (wgmma tf32 where the shape allows); lengths follow the reference's all-valid mask (P10).
 #include "ops.h"
 #include <cmath>
 

@@ -81,7 +81,7 @@ __global__ void cvt_to_f32_kernel(const void* src, float* dst, size_t n, int dty
 
 extern "C" {
 
-const char* idx_version(void) { return "idxtts 0.1 (sm_100a; cuda " "12.9" ")"; }
+const char* idx_version(void) { return "idxtts 0.1 (sm_90a; cuda " "12.9" ")"; }
 
 int idx_create(int device, idx_engine** out) {
   idx_engine* e = nullptr;
@@ -91,16 +91,16 @@ int idx_create(int device, idx_engine** out) {
     if (err != cudaSuccess || n == 0) {
       cudaGetLastError();
       throw IdxError(IDX_ERR_NOGPU,
-                     "no CUDA device visible: libidxtts has no CPU fallback (sm_100a only)");
+                     "no CUDA device visible: libidxtts has no CPU fallback (sm_90a only)");
     }
     IDX_CHECK(device >= 0 && device < n, IDX_ERR_ARG, "bad device index");
     IDX_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     IDX_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
+    if (prop.major != 9 || prop.minor != 0)
       throw IdxError(IDX_ERR_NOGPU, std::string("device is sm_") + std::to_string(prop.major) +
                                         std::to_string(prop.minor) +
-                                        ", libidxtts is built for sm_100a only");
+                                        ", libidxtts is built for sm_90a only");
     e = new idx_engine();
     e->device = device;
     e->num_sms = prop.multiProcessorCount;

@@ -1,22 +1,21 @@
-// gemm_tc.cu — tcgen05 implicit-GEMM back end of conv_gemm() for sm_100a.
+// gemm_tc.cu — wgmma implicit-GEMM back end of conv_gemm() for sm_90a.
 //
 //   D[b][m][n] = epi( sum_tap sum_k A[b][m + tap*dil - pad][k] * Wk[n][tap*K + k] )
 //
-// One CTA computes a 128 x BN output tile (M = time rows, N = output channels):
-//   warp 0      TMA producer: per (tap, k-chunk) one 3-D box of the activations [B][T][K]
-//               (32 fp32 x 128 rows, SWIZZLE_128B; rows outside [0,T) and columns >= K are
-//               zero-filled by TMA = Conv1d zero padding / ragged K for free) and one 2-D box of the
-//               K-major weights, into a ring of shared-memory stages (mbarrier full/empty);
-//   warp 1      allocates TMEM, issues tcgen05.mma.kind::tf32 (M=128, N=BN, K=8 per instruction,
-//               4 per stage) from shared-memory descriptors, commits to the stage's empty barrier;
-//               the fp32 accumulator tile lives in TMEM (BN columns x 128 lanes);
-//   warps 2..5  epilogue: tcgen05.ld the accumulator (each warp its 32-lane quarter), apply
-//               bias / activation / layer-scale / residual / accumulate / scale, store with the
-//               generic (out_off, ldo, out_valid) mapping that also serves ConvTranspose1d.
+// One CTA computes a 128 x BN output tile (M = time rows, N = output channels) with 160 threads:
+//   warps 0..3  one warpgroup: issues wgmma (two M = 64 halves, N = BN, K = 8 tf32 / 16 fp16 per instruction, 4 K steps
+//               per stage) from shared-memory descriptors into register accumulators, one commit group per stage, and frees
+//               a stage as soon as the group that read it has retired; then the epilogue: the accumulator tile goes through
+//               shared memory (the operand ring is dead by then) so that each warp applies bias / activation / layer-scale /
+//               residual / accumulate / scale to 32 rows and stores with the generic (out_off, ldo, out_valid) mapping that
+//               also serves ConvTranspose1d;
+//   warp 4      TMA producer: per (tap, k-chunk) one 3-D box of the activations [B][T][K] (128 bytes along K x 128 rows,
+//               SWIZZLE_128B; rows outside [0,T) and columns >= K are zero-filled by TMA = Conv1d zero padding / ragged K
+//               for free) and one box of the K-major weights, into a ring of shared-memory stages (mbarrier full/empty).
 // Two operand formats share the kernel (template EB = operand element bytes):
-//   EB = 4: fp32 in HBM, tensor maps TFLOAT32 (the TMA unit rounds to tf32 on load), tcgen05.mma kind::tf32, K = 8 per MMA;
+//   EB = 4: fp32 in HBM, tensor maps TFLOAT32 (the TMA unit rounds to tf32 on load), wgmma .tf32, K = 8 per MMA;
 //   EB = 2: fp16 in HBM (activations written as fp16 by their producing kernel, weights converted once at init),
-//           kind::f16, K = 16 per MMA: the same 10-bit mantissa as tf32 at half the bytes per operand — the tf32 tiles of
+//           wgmma .f16, K = 16 per MMA: the same 10-bit mantissa as tf32 at half the bytes per operand — the tf32 tiles of
 //           this kernel are bound by L2 -> shared-memory operand traffic (DESIGN.md), so halving the bytes is what counts.
 // A 128-byte swizzle row holds 32 fp32 or 64 fp16 along K; a stage is always A 16 KB + B BN x 128 B.
 #include "ops.h"
@@ -32,6 +31,7 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BKB = 128; // bytes along K per stage row = one SWIZZLE_128B row (32 tf32 or 64 fp16 elements)
+constexpr int GEMM_THREADS = 160;
 
 __device__ __forceinline__ float apply_act_tc(float v, int act) {
   switch (act) {
@@ -57,37 +57,27 @@ struct TcParams {
   const float* res; const float* rowscale; const float* colscale;
   int accum; float scale;
   float* out; long long out_batch_stride, out_off, out_valid; int ldo;
-  int stages;
+  int stages; int ring_bytes;   // ring_bytes = max(stages x stage, accumulator tile), a multiple of 1024
   int epi; __half* out16; const float* aux; int aux_stride;
 };
 
-// UMMA shared-memory descriptor, K-major, SWIZZLE_128B: start address (>>4), LBO (unused for
-// swizzled K-major, set to 1), SBO = 1024 B (8 rows x 128 B), version = 1 (sm_100), layout = 2.
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
+// bytes of the fp32 accumulator tile staged for the epilogue: 128 rows x (BN + 1) (odd pitch: conflict-free row and column reads)
+constexpr int acc_tile_bytes(int BN) { return BM * (BN + 1) * 4; }
 
 template <int BN, int EB>
-__global__ void __launch_bounds__(192, 2)
+__global__ void __launch_bounds__(GEMM_THREADS, 2)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const TcParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  // carve: stages x (A 16 KB | B BN*128 B), then barriers
+  // carve: stages x (A 16 KB | B BN*128 B) (later the accumulator tile), then barriers
   unsigned char* base = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   constexpr int BK = BKB / EB;       // elements along K per stage
   constexpr int A_BYTES = BM * BKB;
   constexpr int B_BYTES = BN * BKB;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  uint64_t* full = (uint64_t*)(base + (size_t)p.stages * STAGE_BYTES);
+  constexpr int TP = BN + 1;         // accumulator tile pitch (floats)
+  uint64_t* full = (uint64_t*)(base + p.ring_bytes);
   uint64_t* empty = full + p.stages;
-  uint64_t* accum_full = empty + p.stages;
-  uint32_t* tmem_slot = (uint32_t*)(accum_full + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM, b = blockIdx.z;
@@ -96,24 +86,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       ptx::mbar_init(&full[s], 1);
-      ptx::mbar_init(&empty[s], 1);
+      ptx::mbar_init(&empty[s], 4);   // lane 0 of each MMA warp, after its wgmma group that read the stage retired
     }
-    ptx::mbar_init(accum_full, 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(tmem_slot, BN < 32 ? 32 : BN);
-  }
-  ptx::tcgen05_fence_before();
   __syncthreads();
-  ptx::tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // everything above overlapped with the previous kernel of the stream (programmatic dependent launch); from here on
   // this grid reads what that kernel wrote
   pdl_wait();
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       ptx::prefetch_tensormap(&tmA);
       ptx::prefetch_tensormap(&tmB);
@@ -129,163 +112,167 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         ptx::tma_load_3d(sb, &tmB, &full[s], tap * p.K + kc * BK, n0, p.w_batched ? b : 0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // instruction descriptor: D=f32 (1<<4), A=B format (tf32 = 2, f16 = 0) at bits 7 and 10, K-major both, N>>3, M>>4
-      constexpr uint32_t FMT = (EB == 4) ? 2u : 0u;
-      const uint32_t idesc = (1u << 4) | (FMT << 7) | (FMT << 10) | ((uint32_t)(BN >> 3) << 17) |
-                             ((uint32_t)(BM >> 4) << 24);
-      for (int it = 0; it < n_iters; ++it) {
-        const int s = it % p.stages;
-        const uint32_t ph = (it / p.stages) & 1u;
-        ptx::mbar_wait(&full[s], ph);
-        ptx::tcgen05_fence_after();
-        const uint32_t sa = ptx::smem_u32(base + (size_t)s * STAGE_BYTES);
-        const uint32_t sb = sa + A_BYTES;
-        const uint64_t da = make_desc(sa), db = make_desc(sb);
+    return;
+  }
+
+  // ---------------- MMA warpgroup (warps 0..3): rows 0..63 in acc0, 64..127 in acc1 ----------------
+  float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
-        for (int k = 0; k < BKB / 32; ++k) {
-          // one MMA consumes 32 bytes of K (8 tf32 / 16 fp16) inside the 128-byte swizzle row: +2 in 16-byte units
-          if (EB == 4) ptx::umma_tf32(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (it > 0 || k > 0) ? 1u : 0u);
-          else ptx::umma_f16(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        ptx::umma_commit(&empty[s]);
-      }
-      ptx::umma_commit(accum_full);
+  for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+  for (int it = 0; it < n_iters; ++it) {
+    const int s = it % p.stages;
+    const uint32_t ph = (it / p.stages) & 1u;
+    ptx::mbar_wait(&full[s], ph);
+    const uint32_t sa = ptx::smem_u32(base + (size_t)s * STAGE_BYTES);
+    const uint32_t sb = sa + A_BYTES;
+    const uint64_t da = ptx::make_desc_sw128(sa), db = ptx::make_desc_sw128(sb);
+    ptx::fence_regs(acc0);
+    ptx::fence_regs(acc1);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BKB / 32; ++k) {
+      // one MMA consumes 32 bytes of K (8 tf32 / 16 fp16) inside the 128-byte swizzle row: +2 in 16-byte units;
+      // the second M half starts 64 rows x 128 B = 8 KB further (+512)
+      ptx::wgmma_ss<BN, EB>(acc0, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
+      ptx::wgmma_ss<BN, EB>(acc1, da + (uint64_t)(512 + 2 * k), db + (uint64_t)(2 * k), 1u);
     }
-  } else {
-    // ---------------- epilogue warps (2..5): TMEM lane quarter = warp % 4 ----------------
-    // Each warp owns 32 accumulator rows.  A 32x32 chunk is read from TMEM (lane = row), transposed
-    // through a private shared-memory tile (the operand ring is dead by now) so that lane = column:
-    // every global load/store of the epilogue is then a coalesced 128-byte row segment.
-    const int q = warp & 3;
-    ptx::mbar_wait(accum_full, 0);
-    ptx::tcgen05_fence_after();
-    float* tile = (float*)base + (size_t)q * 32 * 33;
-    const long long obs = p.out_batch_stride;
-    const int biasN = p.biasN ? p.biasN : p.N;
-    const int mrow0 = m0 + q * 32;
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<1>();           // the group of stage it-1 has retired: its operands may be overwritten
+    ptx::fence_regs(acc0);
+    ptx::fence_regs(acc1);
+    if (it > 0 && lane == 0) ptx::mbar_arrive(&empty[(it - 1) % p.stages]);
+  }
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc0);
+  ptx::fence_regs(acc1);
+
+  // ---------------- epilogue: accumulators -> shared tile [128][BN + 1] -> 32 rows per warp ----------------
+  // every stage has been consumed, so the ring is dead; the named barrier makes sure no warp still reads it
+  ptx::named_bar_sync(1, 128);
+  float* tile = (float*)base;
+  {
+    const int r0 = warp * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      float* t0 = tile + (size_t)r0 * TP + 8 * j + c;
+      t0[0] = acc0[4 * j]; t0[1] = acc0[4 * j + 1];
+      t0[8 * TP] = acc0[4 * j + 2]; t0[8 * TP + 1] = acc0[4 * j + 3];
+      t0[64 * TP] = acc1[4 * j]; t0[64 * TP + 1] = acc1[4 * j + 1];
+      t0[72 * TP] = acc1[4 * j + 2]; t0[72 * TP + 1] = acc1[4 * j + 3];
+    }
+  }
+  ptx::named_bar_sync(1, 128);
+  const int q = warp;                 // this warp's 32 rows of the tile
+  const long long obs = p.out_batch_stride;
+  const int biasN = p.biasN ? p.biasN : p.N;
+  const int mrow0 = m0 + q * 32;
 #pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      if (n0 + c0 >= p.N) break;
-      uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-      ptx::tmem_ld_wait();
-      if (p.epi == EPI_NONE) {
+  for (int c0 = 0; c0 < BN; c0 += 32) {
+    if (n0 + c0 >= p.N) break;
+    const float* trow = tile + (size_t)(q * 32) * TP + c0;   // element (row rr, column j) of the chunk at trow[rr * TP + j]
+    const int n = n0 + c0 + lane;
+    if (p.epi != EPI_NONE) {
+      // fused pair epilogues, thread = accumulator row: both columns of every pair are read by this thread, no shuffle;
+      // each thread writes 16 or 32 fp16 values = whole 32-byte sectors.
+      // (N is a multiple of 32 for these GEMMs: whole 32-column chunks only.)
+      const int row = mrow0 + lane;
+      if (row < p.M) {
+        const int nb = n0 + c0;                                // first column of this chunk
+        float v[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) tile[lane * 33 + j] = __uint_as_float(r[j]);
-      }
-      __syncwarp();
-      const int n = n0 + c0 + lane;
-      if (p.epi != EPI_NONE) {
-        // fused pair epilogues, thread = accumulator row (the TMEM lane it just read): both columns of every pair are in this
-        // thread's registers, no transpose and no shuffle; each thread writes 16 or 32 fp16 values = whole 32-byte sectors.
-        // (N is a multiple of 32 for these GEMMs: whole 32-column chunks only.)
-        const int row = mrow0 + lane;
-        if (row < p.M) {
-          const int nb = n0 + c0;                                // first column of this chunk
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) + (p.bias ? __ldg(p.bias + nb + j) : 0.f);
-          if (p.epi == EPI_ROPE) {
-            const int HD = 64, Hh = p.aux_stride, HW = Hh * HD;
-            const int which = nb / HW, hh = (nb % HW) / HD, d0 = nb % HD;      // q | k | v, head, first dim of the chunk
-            __half* dst = p.out16 + (size_t)which * ((size_t)gridDim.z * Hh * p.M * HD) + (((size_t)b * Hh + hh) * (size_t)p.M + row) * HD + d0;
-            uint32_t o[16];
-            if (which < 2) {
-              const float4* tab = (const float4*)(p.aux + ((size_t)row * (HD / 2) + (d0 >> 1)) * 2);   // (cos, sin) pairs
-              const float sc = (which == 0) ? p.scale : 1.0f;      // 1/8 (x log2 e when the tcgen05 flash kernel consumes q)
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 t4 = __ldg(tab + i);
-                const float a0 = v[4 * i], a1 = v[4 * i + 1], b0 = v[4 * i + 2], b1 = v[4 * i + 3];
-                __half2 h0 = __floats2half2_rn((a0 * t4.x - a1 * t4.y) * sc, (a1 * t4.x + a0 * t4.y) * sc);
-                __half2 h1 = __floats2half2_rn((b0 * t4.z - b1 * t4.w) * sc, (b1 * t4.z + b0 * t4.w) * sc);
-                o[2 * i] = *(uint32_t*)&h0;
-                o[2 * i + 1] = *(uint32_t*)&h1;
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                __half2 h = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-                o[i] = *(uint32_t*)&h;
-              }
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) ((uint4*)dst)[i] = make_uint4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
-          } else {
-            const int NH = p.N >> 1, j0 = nb >> 1;
-            uint32_t o[8];
+        for (int j = 0; j < 32; ++j) v[j] = trow[lane * TP + j] + (p.bias ? __ldg(p.bias + nb + j) : 0.f);
+        if (p.epi == EPI_ROPE) {
+          const int HD = 64, Hh = p.aux_stride, HW = Hh * HD;
+          const int which = nb / HW, hh = (nb % HW) / HD, d0 = nb % HD;      // q | k | v, head, first dim of the chunk
+          __half* dst = p.out16 + (size_t)which * ((size_t)gridDim.z * Hh * p.M * HD) + (((size_t)b * Hh + hh) * (size_t)p.M + row) * HD + d0;
+          uint32_t o[16];
+          if (which < 2) {
+            const float4* tab = (const float4*)(p.aux + ((size_t)row * (HD / 2) + (d0 >> 1)) * 2);   // (cos, sin) pairs
+            const float sc = (which == 0) ? p.scale : 1.0f;      // 1/8 (x log2 e when the wgmma flash kernel consumes q)
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-              float r0, r1;
-              if (p.epi == EPI_SWIGLU) {                          // F.silu(w1 x) * (w3 x)
-                r0 = __fdividef(v[4 * i], 1.f + __expf(-v[4 * i])) * v[4 * i + 1];
-                r1 = __fdividef(v[4 * i + 2], 1.f + __expf(-v[4 * i + 2])) * v[4 * i + 3];
-              } else {                                            // fused_add_tanh_sigmoid_multiply
-                const float* ga = p.aux + (size_t)b * p.aux_stride + j0 + 2 * i;
-                r0 = tanhf(v[4 * i] + __ldg(ga)) * __fdividef(1.f, 1.f + __expf(-(v[4 * i + 1] + __ldg(ga + NH))));
-                r1 = tanhf(v[4 * i + 2] + __ldg(ga + 1)) * __fdividef(1.f, 1.f + __expf(-(v[4 * i + 3] + __ldg(ga + NH + 1))));
-              }
-              __half2 h = __floats2half2_rn(r0, r1);
+              const float4 t4 = __ldg(tab + i);
+              const float a0 = v[4 * i], a1 = v[4 * i + 1], b0 = v[4 * i + 2], b1 = v[4 * i + 3];
+              __half2 h0 = __floats2half2_rn((a0 * t4.x - a1 * t4.y) * sc, (a1 * t4.x + a0 * t4.y) * sc);
+              __half2 h1 = __floats2half2_rn((b0 * t4.z - b1 * t4.w) * sc, (b1 * t4.z + b0 * t4.w) * sc);
+              o[2 * i] = *(uint32_t*)&h0;
+              o[2 * i + 1] = *(uint32_t*)&h1;
+            }
+          } else {
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+              __half2 h = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
               o[i] = *(uint32_t*)&h;
             }
-            uint4* dst = (uint4*)(p.out16 + ((size_t)b * p.M + row) * NH + j0);
-            dst[0] = make_uint4(o[0], o[1], o[2], o[3]);
-            dst[1] = make_uint4(o[4], o[5], o[6], o[7]);
           }
-        }
-      } else if (n < p.N) {
-        const float bv = p.bias ? __ldg(p.bias + (n % biasN)) : 0.f;
-        const float cs = (p.colscale ? __ldg(p.colscale + n) : 1.f);
-        const long long flat0 = p.out_off + (long long)mrow0 * p.ldo + n;     // row rr adds rr*ldo
-        const int rows = min(32, p.M - mrow0);
-        // fast path: the 32-row x 32-col chunk lies wholly inside the valid output range
-        const bool interior = rows == 32 && (p.out_off + (long long)mrow0 * p.ldo + n0 + c0) >= 0 &&
-                              (p.out_off + (long long)(mrow0 + 31) * p.ldo + n0 + c0 + 31) < p.out_valid;
-        float* op = p.out + (long long)b * obs + flat0;
-        const float* rp = p.res ? p.res + (long long)b * obs + flat0 : nullptr;
-        if (interior && p.act == ACT_NONE && !p.rowscale) {
-          const float sc = p.scale;
-          if (!rp && !p.accum) {
-#pragma unroll 8
-            for (int rr = 0; rr < 32; ++rr) op[(long long)rr * p.ldo] = (tile[rr * 33 + lane] + bv) * cs * sc;
-          } else {
-            // res may alias out (in-place residual): fetch the whole 32-row column into registers first so the
-            // 32 L2 round trips overlap instead of serialising behind the stores
-            float addv[32];
 #pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-              float a = 0.f;
-              if (rp) a = rp[(long long)rr * p.ldo];
-              if (p.accum) a += op[(long long)rr * p.ldo];
-              addv[rr] = a;
-            }
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr)
-              op[(long long)rr * p.ldo] = ((tile[rr * 33 + lane] + bv) * cs + addv[rr]) * sc;
-          }
+          for (int i = 0; i < 4; ++i) ((uint4*)dst)[i] = make_uint4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
         } else {
-          for (int rr = 0; rr < rows; ++rr) {
-            const long long flat = flat0 + (long long)rr * p.ldo;
-            if (flat < 0 || flat >= p.out_valid) continue;
-            float v = tile[rr * 33 + lane] + bv;
-            v = apply_act_tc(v, p.act) * cs;
-            if (p.rowscale) v *= __ldg(p.rowscale + (long long)b * p.M + mrow0 + rr);
-            if (rp) v += rp[(long long)rr * p.ldo];
-            if (p.accum) v += op[(long long)rr * p.ldo];
-            op[(long long)rr * p.ldo] = v * p.scale;
+          const int NH = p.N >> 1, j0 = nb >> 1;
+          uint32_t o[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            float r0, r1;
+            if (p.epi == EPI_SWIGLU) {                          // F.silu(w1 x) * (w3 x)
+              r0 = __fdividef(v[4 * i], 1.f + __expf(-v[4 * i])) * v[4 * i + 1];
+              r1 = __fdividef(v[4 * i + 2], 1.f + __expf(-v[4 * i + 2])) * v[4 * i + 3];
+            } else {                                            // fused_add_tanh_sigmoid_multiply
+              const float* ga = p.aux + (size_t)b * p.aux_stride + j0 + 2 * i;
+              r0 = tanhf(v[4 * i] + __ldg(ga)) * __fdividef(1.f, 1.f + __expf(-(v[4 * i + 1] + __ldg(ga + NH))));
+              r1 = tanhf(v[4 * i + 2] + __ldg(ga + 1)) * __fdividef(1.f, 1.f + __expf(-(v[4 * i + 3] + __ldg(ga + NH + 1))));
+            }
+            __half2 h = __floats2half2_rn(r0, r1);
+            o[i] = *(uint32_t*)&h;
           }
+          uint4* dst = (uint4*)(p.out16 + ((size_t)b * p.M + row) * NH + j0);
+          dst[0] = make_uint4(o[0], o[1], o[2], o[3]);
+          dst[1] = make_uint4(o[4], o[5], o[6], o[7]);
         }
       }
-      __syncwarp();
+    } else if (n < p.N) {
+      // thread = column: every global load / store of this epilogue is a coalesced 128-byte row segment
+      const float bv = p.bias ? __ldg(p.bias + (n % biasN)) : 0.f;
+      const float cs = (p.colscale ? __ldg(p.colscale + n) : 1.f);
+      const long long flat0 = p.out_off + (long long)mrow0 * p.ldo + n;     // row rr adds rr*ldo
+      const int rows = min(32, p.M - mrow0);
+      // fast path: the 32-row x 32-col chunk lies wholly inside the valid output range
+      const bool interior = rows == 32 && (p.out_off + (long long)mrow0 * p.ldo + n0 + c0) >= 0 &&
+                            (p.out_off + (long long)(mrow0 + 31) * p.ldo + n0 + c0 + 31) < p.out_valid;
+      float* op = p.out + (long long)b * obs + flat0;
+      const float* rp = p.res ? p.res + (long long)b * obs + flat0 : nullptr;
+      if (interior && p.act == ACT_NONE && !p.rowscale) {
+        const float sc = p.scale;
+        if (!rp && !p.accum) {
+#pragma unroll 8
+          for (int rr = 0; rr < 32; ++rr) op[(long long)rr * p.ldo] = (trow[rr * TP + lane] + bv) * cs * sc;
+        } else {
+          // res may alias out (in-place residual): fetch the whole 32-row column into registers first so the
+          // 32 L2 round trips overlap instead of serialising behind the stores
+          float addv[32];
+#pragma unroll
+          for (int rr = 0; rr < 32; ++rr) {
+            float a = 0.f;
+            if (rp) a = rp[(long long)rr * p.ldo];
+            if (p.accum) a += op[(long long)rr * p.ldo];
+            addv[rr] = a;
+          }
+#pragma unroll
+          for (int rr = 0; rr < 32; ++rr)
+            op[(long long)rr * p.ldo] = ((trow[rr * TP + lane] + bv) * cs + addv[rr]) * sc;
+        }
+      } else {
+        for (int rr = 0; rr < rows; ++rr) {
+          const long long flat = flat0 + (long long)rr * p.ldo;
+          if (flat < 0 || flat >= p.out_valid) continue;
+          float v = trow[rr * TP + lane] + bv;
+          v = apply_act_tc(v, p.act) * cs;
+          if (p.rowscale) v *= __ldg(p.rowscale + (long long)b * p.M + mrow0 + rr);
+          if (rp) v += rp[(long long)rr * p.ldo];
+          if (p.accum) v += op[(long long)rr * p.ldo];
+          op[(long long)rr * p.ldo] = v * p.scale;
+        }
+      }
     }
-    ptx::tcgen05_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tcgen05_fence_after();
-    ptx::tmem_dealloc(tmem_base, BN < 32 ? 32 : BN);
   }
 }
 
@@ -356,43 +343,47 @@ void launch_bn(idx_engine* e, const ConvGemm& g, const CUtensorMap& tmA, const C
   if (stages > 8) stages = 8;
   if (stages > n_iters) stages = n_iters < 2 ? 2 : n_iters;
   p.stages = stages;
-  const size_t smem = (size_t)stages * STAGE + 1024 + (2 * stages + 1) * 8 + 16;
+  p.ring_bytes = ((stages * STAGE > acc_tile_bytes(BN) ? stages * STAGE : acc_tile_bytes(BN)) + 1023) & ~1023;
+  const size_t smem = (size_t)p.ring_bytes + 1024 + 2 * stages * 8;
   const unsigned bit = (BN == 32 ? 1u : (BN == 64 ? 2u : 4u)) << (EB == 2 ? 8 : 0);
   if (!(e->attr_done & bit)) {     // per engine = per device: function attributes live in the device's context
     IDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     e->attr_done |= bit;
   }
   dim3 grid((g.N + BN - 1) / BN, (g.M + BM - 1) / BM, g.B);
-  launch_pdl(e, gemm_tc_kernel<BN, EB>, grid, dim3(192), smem, tmA, tmB, p);
+  launch_pdl(e, gemm_tc_kernel<BN, EB>, grid, dim3(GEMM_THREADS), smem, tmA, tmB, p);
   e->launches++;
 }
 
 
 // ================================================================================================================
-// tcgen05 flash attention for the DiT (full attention, head dim 64, fp16 operands, fp32 softmax and accumulation).
-//   gpt_fast/model.py:293-303 (F.scaled_dot_product_attention over all T keys; q arrives pre-scaled by 1/8 and
+// wgmma flash attention for the DiT (full attention, head dim 64, fp16 operands, fp32 softmax and accumulation).
+//   gpt_fast/model.py:293-303 (F.scaled_dot_product_attention over all T keys; q arrives pre-scaled by log2(e)/8 and
 //   rotated — EPI_ROPE above).
-// One CTA = 128 queries of one (batch, head).  TMEM: S [128 lanes x 128 cols fp32] | O [x 64] | P [x 64: 128 fp16 per
-// row packed two per column] = 256 columns, so two CTAs share an SM and fill each other's bubbles.
-//   warp 0      TMA: Q tile once, then K_j / V_j tiles of 128 keys into a 2-stage ring (SWIZZLE_128B rows of 64 fp16);
-//   warp 1      one thread issues S = Q K_j^T (4 x tcgen05.mma M128 N128 K16, both operands K-major in shared memory) and,
-//               once the softmax warps have stored P_j, O (+)= P_j V_j (8 x M128 N64 K16: A = P from TENSOR MEMORY,
-//               B = V straight from its [key][dim] rows = MN-major operand);
-//   warps 2..5  thread = query row = TMEM lane: online softmax in the log2 domain (two passes over S in TMEM: row max,
-//               then exp2 / row sum / fp16 pack -> tcgen05.st P), rescale of O when the row max moved, final O / l.
-// The legacy mma.sync flash kernel (nn_ops.cu) ran at the mma.sync ceiling of this part (~170 TFLOP/s); here the exp
-// throughput (MUFU) is the bound, as in every Blackwell attention kernel.
+// One CTA = 128 queries of one (batch, head), 288 threads:
+//   warps 0..7  two warpgroups of 64 query rows each.  Per key tile of 128: S = Q K_j^T (4 x wgmma M64 N128 K16, both
+//               operands K-major in shared memory) into registers; online softmax in the log2 domain on the registers
+//               (a row's 128 scores are spread over the 4 lanes of a quad); P_j packed to fp16 in place — the accumulator
+//               layout of S is the register-operand layout of A — and O (+)= P_j V_j (8 x wgmma M64 N64 K16: A = P from
+//               registers, B = V straight from its [key][dim] rows = MN-major operand);
+//   warp 8      TMA: Q tile once, then K_j / V_j tiles of 128 keys into a 2-stage ring (SWIZZLE_128B rows of 64 fp16).
+// The two warpgroups (and the two CTAs an SM holds) fill each other's softmax bubbles on the tensor cores.
 constexpr int FA_Q = 128, FA_K = 128, FA_D = 64;
+constexpr int FA_THREADS = 288;
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+__device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
+  __half2 h = __floats2half2_rn(lo, hi);
+  return *(uint32_t*)&h;
+}
 struct FaParams { int T, H; float* out; __half* out16; };
 
-__global__ void __launch_bounds__(192, 2)
-fa5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-           const FaParams p) {
+__global__ void __launch_bounds__(FA_THREADS, 1)
+fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                const FaParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* base = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   constexpr int TILE = FA_K * FA_D * 2;                  // 16 KB: 128 rows x 128 bytes
@@ -400,29 +391,20 @@ fa5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUte
   unsigned char* sK = base + TILE;                       // [2][TILE]
   unsigned char* sV = base + 3 * TILE;                   // [2][TILE]
   uint64_t* bars = (uint64_t*)(base + 5 * TILE);
-  uint64_t *q_full = bars, *kv_full = bars + 1, *kv_empty = bars + 3, *s_full = bars + 5, *p_full = bars + 6, *o_full = bars + 7;
-  uint32_t* tmem_slot = (uint32_t*)(bars + 8);
+  uint64_t *q_full = bars, *kv_full = bars + 1, *kv_empty = bars + 3;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int bh = blockIdx.y, q0 = blockIdx.x * FA_Q;
   const int T = p.T, ntiles = (T + FA_K - 1) / FA_K;
   if (threadIdx.x == 0) {
     ptx::mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&kv_full[s], 1); ptx::mbar_init(&kv_empty[s], 1); }
-    ptx::mbar_init(s_full, 1);
-    ptx::mbar_init(p_full, 128);
-    ptx::mbar_init(o_full, 1);
+    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&kv_full[s], 1); ptx::mbar_init(&kv_empty[s], 8); }
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, 256);
-  ptx::tcgen05_fence_before();
   __syncthreads();
-  ptx::tcgen05_fence_after();
-  const uint32_t tm = *tmem_slot;
-  const uint32_t tS = tm, tO = tm + 128, tP = tm + 192;
   pdl_wait();
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       ptx::prefetch_tensormap(&tmQ); ptx::prefetch_tensormap(&tmK); ptx::prefetch_tensormap(&tmV);
       ptx::mbar_arrive_expect_tx(q_full, TILE);
@@ -435,137 +417,113 @@ fa5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUte
         ptx::tma_load_3d(sV + s * TILE, &tmV, &kv_full[s], 0, j * FA_K, bh);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // D = f32, A = B = f16; S: N = 128 keys, both K-major; PV: N = 64 dims, B (V) MN-major (bit 16)
-      const uint32_t idesc_s = (1u << 4) | ((uint32_t)(FA_K >> 3) << 17) | ((uint32_t)(FA_Q >> 4) << 24);
-      const uint32_t idesc_o = (1u << 4) | (1u << 16) | ((uint32_t)(FA_D >> 3) << 17) | ((uint32_t)(FA_Q >> 4) << 24);
-      ptx::mbar_wait(q_full, 0);
-      const uint64_t dq = make_desc(ptx::smem_u32(sQ));
-      for (int j = 0; j < ntiles; ++j) {
-        const int s = j & 1;
-        ptx::mbar_wait(&kv_full[s], (j >> 1) & 1u);
-        ptx::tcgen05_fence_after();
-        const uint64_t dk = make_desc(ptx::smem_u32(sK + s * TILE));
-#pragma unroll
-        for (int k = 0; k < FA_D / 16; ++k) ptx::umma_f16(tS, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), idesc_s, k > 0 ? 1u : 0u);
-        ptx::umma_commit(s_full);                       // tracks every MMA issued so far: S_j ready AND O += P_{j-1} V_{j-1} done
-        ptx::mbar_wait(p_full, j & 1u);                 // P_j is in tensor memory, O has been rescaled
-        ptx::tcgen05_fence_after();
-        const uint64_t dv = make_desc(ptx::smem_u32(sV + s * TILE));
-#pragma unroll
-        for (int k = 0; k < FA_K / 16; ++k)             // 16 keys per MMA: 8 packed P columns, 16 V rows = 2048 bytes
-          ptx::umma_f16_ts(tO, tP + (uint32_t)(8 * k), dv + (uint64_t)(128 * k), idesc_o, (j > 0 || k > 0) ? 1u : 0u);
-        ptx::umma_commit(&kv_empty[s]);                 // K_j / V_j consumed
-      }
-      ptx::umma_commit(o_full);
-    }
-  } else {
-    const int qd = warp & 3;                            // TMEM lane quarter of this warp
-    const int row = qd * 32 + lane;                     // query row inside the tile = TMEM lane
-    const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-    float m = -INFINITY, l = 0.f;                       // running row max (log2 domain) and row sum
-    for (int j = 0; j < ntiles; ++j) {
-      ptx::mbar_wait(s_full, j & 1u);
-      ptx::tcgen05_fence_after();
-      const int kbase = j * FA_K;
-      // the whole S row of this thread (128 keys) in registers: four tensor-memory loads in flight, one wait
-      uint32_t r[FA_K];
-#pragma unroll
-      for (int c = 0; c < FA_K; c += 32) ptx::tmem_ld_32x32b_x32(tS + lane_off + (uint32_t)c, r + c);
-      ptx::tmem_ld_wait();
-      // (ncu of the first version: 2200 warp instructions per tile per softmax warp — per element a masked max, an FMA, the
-      // accurate exp2f sequence, two adds — made the kernel issue-bound at the speed of the mma.sync one.  Now the scores
-      // arrive in the log2 domain (q is pre-scaled by log2(e)/8 in EPI_ROPE), exp2 is the bare MUFU, and only the last
-      // key tile pays for masking.)
-      const int nvalid = T - kbase;                     // keys beyond T (zero-filled rows of the last tile) are masked
-      if (nvalid < FA_K) {
-#pragma unroll
-        for (int i = 0; i < FA_K; ++i)
-          if (i >= nvalid) r[i] = 0xff800000u;          // -inf
-      }
-      float mx = __uint_as_float(r[0]);
-#pragma unroll
-      for (int i = 1; i < FA_K; ++i) mx = fmaxf(mx, __uint_as_float(r[i]));
-      const float mn = fmaxf(m, mx);
-      const float corr = ex2_approx(m - mn);            // 0 at the first tile (m = -inf)
-      float rs0 = 0.f, rs1 = 0.f;
-      // p = 2^(s - mn), packed to fp16 pairs in place: r[i] <- (p[2i], p[2i+1])
-#pragma unroll
-      for (int i = 0; i < FA_K / 2; ++i) {
-        const float p0 = ex2_approx(__uint_as_float(r[2 * i]) - mn);
-        const float p1 = ex2_approx(__uint_as_float(r[2 * i + 1]) - mn);
-        rs0 += p0;
-        rs1 += p1;
-        __half2 h = __floats2half2_rn(p0, p1);
-        r[i] = *(uint32_t*)&h;
-      }
-      const float rs = rs0 + rs1;
-      ptx::tmem_st_32x32b_x32(tP + lane_off, r);
-      ptx::tmem_st_32x32b_x32(tP + lane_off + 32u, r + 32);
-      l = l * corr + rs;
-      if (j > 0 && __any_sync(0xffffffffu, corr != 1.f)) {     // warp-uniform: tcgen05.ld / st are warp-collective
-        // the row max moved: O (complete up to tile j-1: s_full tracks that MMA too) is rescaled in tensor memory
-#pragma unroll 1
-        for (int c = 0; c < FA_D; c += 32) {
-          uint32_t r[32];
-          ptx::tmem_ld_32x32b_x32(tO + lane_off + (uint32_t)c, r);
-          ptx::tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * corr);
-          ptx::tmem_st_32x32b_x32(tO + lane_off + (uint32_t)c, r);
-        }
-      }
-      m = mn;
-      ptx::tmem_st_wait();
-      ptx::tcgen05_fence_before();
-      ptx::mbar_arrive(p_full);
-    }
-    // epilogue: O / l -> fp16 (operand of the output projection) and / or fp32, [B][T][H*64]
-    ptx::mbar_wait(o_full, 0);
-    ptx::tcgen05_fence_after();
-    const int t = q0 + row;
-    const float inv = l > 0.f ? 1.f / l : 0.f;
-    const int b = bh / p.H, h = bh % p.H;
-    const size_t o = ((size_t)b * T + t) * (size_t)p.H * FA_D + (size_t)h * FA_D;
-#pragma unroll 1
-    for (int c = 0; c < FA_D; c += 32) {
-      uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(tO + lane_off + (uint32_t)c, r);
-      ptx::tmem_ld_wait();
-      if (t < T) {
-        if (p.out16) {
-          uint32_t hh[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            __half2 h2 = __floats2half2_rn(__uint_as_float(r[2 * i]) * inv, __uint_as_float(r[2 * i + 1]) * inv);
-            hh[i] = *(uint32_t*)&h2;
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) ((uint4*)(p.out16 + o + c))[i] = make_uint4(hh[4 * i], hh[4 * i + 1], hh[4 * i + 2], hh[4 * i + 3]);
-        }
-        if (p.out) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            ((float4*)(p.out + o + c))[i] = make_float4(__uint_as_float(r[4 * i]) * inv, __uint_as_float(r[4 * i + 1]) * inv,
-                                                        __uint_as_float(r[4 * i + 2]) * inv, __uint_as_float(r[4 * i + 3]) * inv);
-        }
-      }
-    }
-    ptx::tcgen05_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tcgen05_fence_after();
-    ptx::tmem_dealloc(tm, 256);
+
+  const int wg = warp >> 2;                             // 64-row half of the query tile
+  const int g = lane >> 2, t4 = lane & 3;
+  // this thread's rows of the tile: rA = 64 wg + 16 (warp % 4) + g and rA + 8
+  const int rA = wg * 64 + (warp & 3) * 16 + g;
+  float S[FA_K / 2], O[FA_D / 2];
+#pragma unroll
+  for (int i = 0; i < FA_D / 2; ++i) O[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running row max (log2 domain), this thread's share of the row sum
+  ptx::mbar_wait(q_full, 0);
+  const uint64_t dq = ptx::make_desc_sw128(ptx::smem_u32(sQ + wg * 64 * 128));
+  for (int j = 0; j < ntiles; ++j) {
+    const int s = j & 1;
+    ptx::mbar_wait(&kv_full[s], (j >> 1) & 1u);
+    const uint64_t dk = ptx::make_desc_sw128(ptx::smem_u32(sK + s * TILE));
+    ptx::fence_regs(S);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < FA_D / 16; ++k) ptx::wgmma_ss<FA_K, 2>(S, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(S);
+    // keys beyond T (zero-filled rows of the last tile) are masked; element 4c + i is key 8c + 2 t4 + (i & 1)
+    const int nvalid = T - j * FA_K;
+    if (nvalid < FA_K) {
+#pragma unroll
+      for (int c = 0; c < FA_K / 8; ++c) {
+        const int key = 8 * c + 2 * t4;
+        if (key >= nvalid) { S[4 * c] = -INFINITY; S[4 * c + 2] = -INFINITY; }
+        if (key + 1 >= nvalid) { S[4 * c + 1] = -INFINITY; S[4 * c + 3] = -INFINITY; }
+      }
+    }
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int c = 0; c < FA_K / 8; ++c) {
+      mx0 = fmaxf(mx0, fmaxf(S[4 * c], S[4 * c + 1]));
+      mx1 = fmaxf(mx1, fmaxf(S[4 * c + 2], S[4 * c + 3]));
+    }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+    const float c0 = ex2_approx(m0 - mn0), c1 = ex2_approx(m1 - mn1);   // 0 at the first tile (m = -inf)
+    // p = 2^(s - mn) packed to fp16 pairs: P[2c] = row rA keys (8c + 2 t4, +1), P[2c + 1] = row rA + 8, same keys
+    uint32_t P[FA_K / 4];
+    float rs0 = 0.f, rs1 = 0.f;
+#pragma unroll
+    for (int c = 0; c < FA_K / 8; ++c) {
+      const float p0 = ex2_approx(S[4 * c] - mn0), p1 = ex2_approx(S[4 * c + 1] - mn0);
+      const float p2 = ex2_approx(S[4 * c + 2] - mn1), p3 = ex2_approx(S[4 * c + 3] - mn1);
+      rs0 += p0 + p1;
+      rs1 += p2 + p3;
+      P[2 * c] = pack_half2(p0, p1);
+      P[2 * c + 1] = pack_half2(p2, p3);
+    }
+    l0 = l0 * c0 + rs0;
+    l1 = l1 * c1 + rs1;
+    m0 = mn0;
+    m1 = mn1;
+#pragma unroll
+    for (int c = 0; c < FA_D / 8; ++c) { O[4 * c] *= c0; O[4 * c + 1] *= c0; O[4 * c + 2] *= c1; O[4 * c + 3] *= c1; }
+    const uint64_t dv = ptx::make_desc_sw128(ptx::smem_u32(sV + s * TILE));
+    ptx::fence_regs(O);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < FA_K / 16; ++k) {               // 16 keys per MMA: A = keys 16k..16k+15 of P, B = 16 V rows = 2048 bytes
+      const uint32_t a[4] = {P[4 * k], P[4 * k + 1], P[4 * k + 2], P[4 * k + 3]};
+      ptx::wgmma_rs_f16_n64_tb(O, a, dv + (uint64_t)(128 * k), 1u);
+    }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(O);
+    __syncwarp();
+    if (lane == 0) ptx::mbar_arrive(&kv_empty[s]);      // K_j / V_j consumed by this warp
+  }
+  // epilogue: O / l -> fp16 (operand of the output projection) and / or fp32, [B][T][H*64]
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float i0 = l0 > 0.f ? 1.f / l0 : 0.f, i1 = l1 > 0.f ? 1.f / l1 : 0.f;
+  const int b = bh / p.H, h = bh % p.H;
+  const int t0 = q0 + rA, t1 = t0 + 8;
+  const size_t o0 = ((size_t)b * T + t0) * (size_t)p.H * FA_D + (size_t)h * FA_D;
+  const size_t o1 = o0 + (size_t)8 * p.H * FA_D;
+#pragma unroll
+  for (int c = 0; c < FA_D / 8; ++c) {
+    const int d = 8 * c + 2 * t4;
+    if (p.out16) {
+      if (t0 < T) *(uint32_t*)(p.out16 + o0 + d) = pack_half2(O[4 * c] * i0, O[4 * c + 1] * i0);
+      if (t1 < T) *(uint32_t*)(p.out16 + o1 + d) = pack_half2(O[4 * c + 2] * i1, O[4 * c + 3] * i1);
+    }
+    if (p.out) {
+      if (t0 < T) *(float2*)(p.out + o0 + d) = make_float2(O[4 * c] * i0, O[4 * c + 1] * i0);
+      if (t1 < T) *(float2*)(p.out + o1 + d) = make_float2(O[4 * c + 2] * i1, O[4 * c + 3] * i1);
+    }
   }
 }
 
 }  // namespace
 
-// tcgen05 flash attention on the rotated / split fp16 tensors Qr | Kr | Vb [B*H][T][64] (see fa5_kernel)
-void flash_attention_tc5(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
-                         int B, int T, int H) {
+// wgmma flash attention on the rotated / split fp16 tensors Qr | Kr | Vb [B*H][T][64] (see fa_wgmma_kernel)
+void flash_attention_wgmma(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
+                           int B, int T, int H) {
   const int BH = B * H;
   cuuint64_t dims[3] = {(cuuint64_t)FA_D, (cuuint64_t)T, (cuuint64_t)BH};
   cuuint64_t str[2] = {(cuuint64_t)FA_D * 2, (cuuint64_t)T * FA_D * 2};
@@ -573,12 +531,12 @@ void flash_attention_tc5(idx_engine* e, const __half* Qr, const __half* Kr, cons
   CUtensorMap tq = make_map(Qr, 3, dims, str, box, true), tk = make_map(Kr, 3, dims, str, box, true), tv = make_map(Vb, 3, dims, str, box, true);
   FaParams p;
   p.T = T; p.H = H; p.out = out; p.out16 = out16;
-  const size_t smem = 5 * (size_t)(FA_K * FA_D * 2) + 1024 + 128;
+  const size_t smem = 5 * (size_t)(FA_K * FA_D * 2) + 1024 + 64;
   if (!(e->attr_done & (1u << 20))) {
-    IDX_CUDA(cudaFuncSetAttribute(fa5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    IDX_CUDA(cudaFuncSetAttribute(fa_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     e->attr_done |= 1u << 20;
   }
-  launch_pdl(e, fa5_kernel, dim3((T + FA_Q - 1) / FA_Q, BH), dim3(192), smem, tq, tk, tv, p);
+  launch_pdl(e, fa_wgmma_kernel, dim3((T + FA_Q - 1) / FA_Q, BH), dim3(FA_THREADS), smem, tq, tk, tv, p);
   e->launches++;
 }
 
@@ -618,7 +576,7 @@ void gemm_tc_launch(idx_engine* e, const ConvGemm& g) {
     // fewer 128-wide tiles than SMs: halve the tile so every SM gets work (2 CTAs/SM are resident anyway)
     static const int bn64 = getenv("IDX_GEMM_BN64") ? atoi(getenv("IDX_GEMM_BN64")) : 1;
     const long long tiles128 = (long long)((g.N + 127) / 128) * ((g.M + BM - 1) / BM) * g.B;
-    if (bn64 && BN == 128 && tiles128 < 148) BN = 64;
+    if (bn64 && BN == 128 && tiles128 < e->num_sms) BN = 64;
   }
   cuuint32_t bbox[3] = {(cuuint32_t)(BKB / EBh), (cuuint32_t)BN, 1};
   CUtensorMap tmB = make_map(half ? (const void*)g.Wk16 : (const void*)g.Wk, 3, bdims, bstr, bbox, half);

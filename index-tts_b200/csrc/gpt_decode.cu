@@ -1,5 +1,5 @@
 // gpt_decode.cu — the autoregressive speech-token path of UnifiedVoice as ONE persistent
-// sm_100a kernel per group of decode steps.
+// sm_90a kernel per group of decode steps.
 //
 // Replaces, for the v2/v2.5 GPT (SURVEY.md §8a rows a2–a6):
 //   GPT2InferenceModel.forward            indextts/gpt/model_v2.py:121-198
@@ -8,7 +8,7 @@
 //   GenerationMixin._sample greedy loop     transformers_generation_utils.py:3123-3297
 //   RepetitionPenaltyLogitsProcessor        (transformers.generation.logits_process)
 //
-// Design (B200-first, batch-1 decode is pure weight streaming — 965.6 MB bf16 per token):
+// Design (batch-1 decode is pure weight streaming — 965.6 MB bf16 per token):
 //   * one CTA per SM (cooperative launch), 8 compute warps + 1 producer warp;
 //   * every CTA owns a fixed slice of output columns of every GEMV phase; its weights for
 //     ALL layers/phases are pre-packed into one contiguous byte stream in consumption order,
@@ -219,7 +219,7 @@ __device__ __forceinline__ void grid_sync(unsigned* ctr, unsigned& target, int G
   ptx::named_bar_sync(1, NCT);
   if (flavor == 2) {
     // flag barrier: one arrival word per CTA (no same-address atomics, which L2 serialises at
-    // ~27 cycles each: 148 arrivals on one counter cost ~2 us), polled by the 32 lanes of warp 0.
+    // ~27 cycles each: one arrival per SM on one counter costs ~2 us), polled by the 32 lanes of warp 0.
     if (threadIdx.x < 32) {
       unsigned* flags = ctr + 32;
       target += 1u;
@@ -386,7 +386,7 @@ __device__ __forceinline__ void ln_block(float (&v)[NPL / 8], const float* w, co
 // positions; a 1-row step aliases row 0), K runs over the segment: warp w owns k-steps
 // [w*KS, (w+1)*KS), so every warp issues KS x (ldmatrix A, ldmatrix B, mma) per chunk and the 8 partial
 // accumulators are summed through shared memory.  A tile of M = 8 weight rows per 20 KB stage is what
-// keeps the prefetch ring deep; tcgen05's minimum M = 64 would need 160 KB stages.
+// keeps the prefetch ring deep; wgmma's minimum M = 64 would need 160 KB stages.
 // EPI: 0 QKV, 1 O-proj(+residual), 2 FC(+gelu), 3 PROJ(+residual), 4 HEAD
 template <int BT, int EPI, int D>
 __device__ __forceinline__ void gemv_phase(const GptParams& p, const Smem<BT>& sm, int layer,

@@ -166,7 +166,7 @@ __device__ __forceinline__ float red_sum(const float* red, int item, int row) {
 }
 
 // Hand-over polls.  Round-2 measurement: the LAST producer's words became visible to the pollers 2-3 us after they were
-// stored when all 256 threads of all 148 CTAs re-read their whole slice in every round — 148 x 4 sector reads per 128-byte
+// stored when all 256 threads of all CTAs re-read their whole slice in every round — CTAs x 4 sector reads per 128-byte
 // line per round queue at the L2 slice that holds the line, in front of the very stores the pollers wait for.  So a warp
 // first spins on ONE word (all lanes the same address = one request per warp per round, the word chosen per (CTA, warp)
 // so the spinners spread over the lines) and only then checks its whole slice.
@@ -354,7 +354,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
     unsigned cons_tile = 0;           // phases consumed
     int cons_row = 0;                 // ring row of the next phase to consume
     // A phase may be issued in instalments (mbarrier.expect_tx for all but the last, which arrives) and one call issues at
-    // most `cap` rows: see gpt_decode8.cuh — bursts of 148 x 60-150 KB bulk copies delay the latency-critical hand-over traffic.
+    // most `cap` rows: see gpt_decode8.cuh — bursts of one 60-150 KB bulk copy per CTA copies delay the latency-critical hand-over traffic.
     // Measured over 256 steps (us / step): whole phases only 445.2; instalments, no cap 433.1; cap 24: 432.8; cap 18: 425.5; cap 12: 436.5.
     constexpr int MINPART = 4;
     const int cap = ((p.dbg >> 8) & 0xff) ? ((p.dbg >> 8) & 0xff) : 18;
@@ -439,7 +439,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
       if ((p.dbg & 8) || tix == cons_tile) issue_fitting(max(cap, sc.rows(pidx) - part));   // the phase consumed next is not (completely) issued: all of it at once; dbg 8 = always
     };
     // The freed rows are refilled a little later — right after this CTA's NEXT hand-over poll has completed: at the release
-    // point all 148 CTAs would start their 60-90 KB bulk copies together, exactly when the epilogue stores and the polls of
+    // point all CTAs would start their 60-90 KB bulk copies together, exactly when the epilogue stores and the polls of
     // the hand-over (the latency-critical traffic) are in flight; the ring holds two to three phases, so the weights issued
     // one poll later still arrive long before they are consumed.
     auto refill = [&]() { if (!(p.dbg & 8)) issue_fitting(); };

@@ -219,7 +219,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
   // smaller than FC + PROJ of one CTA (66-71 rows), and a PROJ requested only after FC had been consumed arrived late.
   // Pacing: one call issues at most `cap` rows.  Round-2 timeline: with every freed row refilled at once, the grid barriers
   // that followed a big release (FC: 3.9 us, PROJ: 3.3 us, QKV: 2.5 us) cost two to three times the barrier after the
-  // attention phase (1.0-1.3 us, no refill in flight) although all CTAs arrived within 0.3 us — 148 CTAs x up to 150 KB of
+  // attention phase (1.0-1.3 us, no refill in flight) although all CTAs arrived within 0.3 us — every CTA x up to 150 KB of
   // bulk copies queue in front of the barrier's atomics and polls.  Smaller instalments at more points of the layer keep
   // the ring ahead of the consumption (~4.4 rows / us) without such bursts.
   constexpr int MINPART = 4;

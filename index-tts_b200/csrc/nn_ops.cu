@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(256) attention_kernel(const float* __restrict_
   }
 }
 
-// ---- unfused tensor-core attention helpers (S = Q K^T and O = P V run on the tcgen05 GEMM) ----
+// ---- unfused tensor-core attention helpers (S = Q K^T and O = P V run on the wgmma GEMM) ----
 __global__ void rope_split_kernel(const float* __restrict__ qkv, const float* __restrict__ rope,
                                   float* __restrict__ Qr, float* __restrict__ Kr, float* __restrict__ Vt,
                                   int T, int Tp, int H) {
@@ -688,7 +688,7 @@ void attention_rope(idx_engine* e, const float* qkv, float* out, int B, int T, i
   }
   IDX_CHECK(out16 == nullptr, IDX_ERR_STATE, "attention_rope: an fp16 output exists only on the fused tensor-core path");
   if (gemm_default_backend(e) == 0 && lens == nullptr && T >= 128) {
-    // tensor-core path: rotate/split -> S = Q K^T (tcgen05) -> row softmax -> O = P V (tcgen05) -> merge
+    // tensor-core path: rotate/split -> S = Q K^T (wgmma) -> row softmax -> O = P V (wgmma) -> merge
     const size_t mark = e->arena.off;
     const int Tp = (T + 3) & ~3;
     const long long BH = (long long)B * H;
@@ -724,15 +724,15 @@ void attention_rope(idx_engine* e, const float* qkv, float* out, int B, int T, i
   attention_kernel<<<grid, 256, smem, e->stream>>>(qkv, out, T, H, rope, lens);
   LAUNCH_CHECK(e);
 }
-static bool fa5_on() {
-  static const bool on = !(getenv("IDX_FA5") && atoi(getenv("IDX_FA5")) == 0);
+static bool fa_wgmma_on() {
+  static const bool on = !(getenv("IDX_FA_WGMMA") && atoi(getenv("IDX_FA_WGMMA")) == 0);
   return on;
 }
-float flash_attention_q_scale() { return fa5_on() ? 0.125f * 1.4426950408889634f : 0.125f; }
+float flash_attention_q_scale() { return fa_wgmma_on() ? 0.125f * 1.4426950408889634f : 0.125f; }
 void flash_attention_split(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
                            int B, int T, int H) {
-  if (fa5_on()) {
-    flash_attention_tc5(e, Qr, Kr, Vb, out, out16, B, T, H);
+  if (fa_wgmma_on()) {
+    flash_attention_wgmma(e, Qr, Kr, Vb, out, out16, B, T, H);
     return;
   }
   launch_pdl(e, flash_attn_tc_kernel, dim3((T + FQ - 1) / FQ, (unsigned)((long long)B * H)), dim3(128), 0, Qr, Kr, Vb, out, T, H, out16);

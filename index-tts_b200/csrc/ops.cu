@@ -1,6 +1,6 @@
 // ops.cu — generic multi-tap GEMM (Conv1d / ConvTranspose1d / Linear on channels-last fp32) and
 // layout helpers.  Two back ends behind conv_gemm():
-//   * tcgen05 implicit GEMM (gemm_tc.cu): TMA-staged operands, TMEM accumulators, kind::tf32;
+//   * wgmma implicit GEMM (gemm_tc.cu): TMA-staged operands, register accumulators, tf32 or fp16;
 //   * a plain SIMT fp32 tile kernel (this file): bring-up / odd-shape path and the reference
 //     the tensor-core path is tested against.  Both are CUDA; neither is a CPU fallback.
 #include "ops.h"
@@ -152,7 +152,7 @@ extern "C" int idx_set_option(idx_engine* e, const char* name, int value) {
   IDX_CHECK(e && name, IDX_ERR_ARG, "null argument");
   const std::string n(name);
   if (n == "gemm_backend") {
-    IDX_CHECK(value >= 0 && value <= 1, IDX_ERR_ARG, "gemm_backend: 0 = auto (tcgen05 tf32 where applicable), 1 = SIMT fp32");
+    IDX_CHECK(value >= 0 && value <= 1, IDX_ERR_ARG, "gemm_backend: 0 = auto (wgmma tf32 where applicable), 1 = SIMT fp32");
     e->gemm_backend = value;       // per engine: another handle (another GPU, another thread) keeps its own
   } else if (n == "tail_f16") {
     IDX_CHECK(value >= 0 && value <= 1, IDX_ERR_ARG, "tail_f16: 1 = fp16 GEMM operands on the tensor-core path (default), 0 = tf32 over fp32 storage");

@@ -22,7 +22,7 @@ struct ConvGemm {
   int lda = 0;                   // row stride of A in elements; 0 → K
   const float* W = nullptr;   // [taps][K][N]  (N contiguous)  — SIMT layout
   const float* Wk = nullptr;  // [N][taps*K]   (K contiguous)  — tensor-core layout (optional)
-  // fp16 operand path (tcgen05 kind::f16): both set -> the tensor-core kernel reads these instead of A / Wk (same shapes,
+  // fp16 operand path (wgmma .f16): both set -> the tensor-core kernel reads these instead of A / Wk (same shapes,
   // strides given in ELEMENTS as for the fp32 operands).  Written by the producing kernel of A / converted once at init.
   const __half* A16 = nullptr;
   const __half* Wk16 = nullptr;
@@ -56,7 +56,7 @@ struct ConvGemm {
 };
 
 void conv_gemm(idx_engine* e, const ConvGemm& g);
-inline int gemm_default_backend(const idx_engine* e) { return e->gemm_backend; }   // 0 auto (tcgen05), 1 SIMT fp32
+inline int gemm_default_backend(const idx_engine* e) { return e->gemm_backend; }   // 0 auto (wgmma), 1 SIMT fp32
 
 // [B][C][T] <-> [B][T][C]
 void transpose_bct_to_btc(idx_engine* e, const float* in, float* out, int B, int C, int T);
@@ -65,7 +65,7 @@ void transpose_btc_to_bct(idx_engine* e, const float* in, float* out, int B, int
 // ------------------------------------------------------------- programmatic dependent launch --
 // The tail is ~4000 short kernels per utterance.  Kernels launched through launch_pdl() carry the programmatic-stream-
 // serialization attribute: their CTAs may be scheduled while the previous kernel of the stream is still draining, so launch
-// latency and the kernel's own prologue (barrier init, TMEM allocation, descriptor prefetch) overlap with it.  Such a kernel
+// latency and the kernel's own prologue (barrier init, descriptor prefetch) overlap with it.  Such a kernel
 // executes pdl_wait() — every thread — before it touches global memory, and pdl_trigger() as soon as it has nothing left that
 // the NEXT kernel could disturb (the next kernel's own pdl_wait still waits for this grid to finish completely).
 #ifdef __CUDACC__
@@ -156,11 +156,11 @@ __half* pack_half_interleaved(idx_engine* e, WeightPool& pool, const PackedW& w,
 // the fused flash attention on already rotated / split fp16 tensors Qr | Kr | Vb [B*H][T][64] (what EPI_ROPE writes)
 void flash_attention_split(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
                            int B, int T, int H);
-// scale EPI_ROPE must apply to q for flash_attention_split: 1/8, times log2(e) when the tcgen05 kernel (exp2 softmax) is on
+// scale EPI_ROPE must apply to q for flash_attention_split: 1/8, times log2(e) when the wgmma kernel (exp2 softmax) is on
 float flash_attention_q_scale();
-// the same on tcgen05 (gemm_tc.cu: S and O in tensor memory, P fed back as a tensor-memory operand)
-void flash_attention_tc5(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
-                         int B, int T, int H);
+// the same on wgmma (gemm_tc.cu: S and O in registers, P fed back as a register operand)
+void flash_attention_wgmma(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
+                           int B, int T, int H);
 // fp32 -> fp16 (round to nearest), n elements
 void to_half(idx_engine* e, const float* x, __half* y, long long n);
 // true when the engine runs the tail with fp16 GEMM operands (tensor-core back end and not disabled by IDX_TAIL_F16=0)

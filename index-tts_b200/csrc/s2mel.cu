@@ -1,5 +1,5 @@
 // s2mel.cu — semantic-codec decode → length regulator → flow-matching CFM (DiT + WaveNet) Euler
-// solver of IndexTTS-2 / 2.5 on sm_100a, fp32 (the reference disables autocast here, P5).
+// solver of IndexTTS-2 / 2.5 on sm_90a, fp32 (the reference disables autocast here, P5).
 //
 // Replaces (SURVEY.md §8a rows a8–a11):
 //   EnhancedCodec.decode               indextts/codec/models.py:205-231
@@ -361,7 +361,7 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
       // wqkv with the RoPE / 1/8 scale / head split in its epilogue: fp16 Qr | Kr | Vb go straight to the flash attention
       ConvGemm g = gemm_of16(s->wqkv[l], b.a16, Bn, T, nullptr);
       g.epi = EPI_ROPE; g.out16 = b.qkv16; g.aux = b.rope; g.aux_stride = nh;
-      g.scale = flash_attention_q_scale();          // 1/sqrt(64), times log2(e) when the tcgen05 flash kernel takes q
+      g.scale = flash_attention_q_scale();          // 1/sqrt(64), times log2(e) when the wgmma flash kernel takes q
       conv_gemm(e, g);
       const size_t one = (size_t)Bn * nh * T * 64;
       flash_attention_split(e, b.qkv16, b.qkv16 + one, b.qkv16 + 2 * one, nullptr, b.att16, Bn, T, nh);

@@ -4,7 +4,7 @@
 constructor, i.e. with its own config/checkpoint loaders (`indextts.infer_v2.IndexTTS2` is NOT covered: its
 `inference_speech` call passes no `campplus_embedding` and consumes the returned conditioning latent,
 infer_v2.py:583-662 — `attach` raises for it) — registers the
-weights of its modules with a B200 engine and rebinds the module-level seams of `infer_generator`
+weights of its modules with the CUDA engine and rebinds the module-level seams of `infer_generator`
 (SURVEY.md §8b) to the C-ABI:
 
     tts.gpt.merge_emovec              → idx_merge_emovec                            (model_v2.py:827-838)
@@ -103,7 +103,7 @@ def _fresh_seed():
 
 def _check_hf_kwargs(num_return_sequences, typical_sampling, hf):
     if typical_sampling:
-        raise NotImplementedError("typical_sampling=True (TypicalLogitsWarper, model_v2.py:798-800) is not built on the B200 path")
+        raise NotImplementedError("typical_sampling=True (TypicalLogitsWarper, model_v2.py:798-800) is not built on the engine path")
     if int(num_return_sequences or 1) != 1:
         raise NotImplementedError("num_return_sequences must be 1 (what infer_v2_5.py:771-791 / infer.py pass)")
     nb = int(hf.get("num_beams", 1) or 1)
@@ -112,13 +112,13 @@ def _check_hf_kwargs(num_return_sequences, typical_sampling, hf):
     if hf.get("do_sample", False):
         tk = int(hf.get("top_k", 0) or 0)
         if tk <= 0 or tk > 128:
-            raise NotImplementedError("do_sample needs 1 <= top_k <= 128 on the B200 path (the reference default is 30, the "
+            raise NotImplementedError("do_sample needs 1 <= top_k <= 128 on the engine path (the reference default is 30, the "
                                       "webui allows up to 100); top_k=0 / larger values are rejected, never silently capped")
     return nb
 
 
 def attach(tts, engine: Engine = None, device: int = 0):
-    """Rebind the compute seams of a reference IndexTTS2 (infer_v2_5) instance to the B200 engine (see module doc)."""
+    """Rebind the compute seams of a reference IndexTTS2 (infer_v2_5) instance to the CUDA engine (see module doc)."""
     if type(tts).__module__.endswith("infer_v2"):
         raise NotImplementedError("attach() covers indextts.infer_v2_5.IndexTTS2; infer_v2.IndexTTS2 (row f3) is not built")
     engine = engine or Engine(device)
@@ -132,7 +132,7 @@ def attach(tts, engine: Engine = None, device: int = 0):
                          typical_mass=.9, **hf):
         # same argument meaning as gpt/model_v2.py:716-825; emo_vec comes from merge_emovec (:833-838)
         if emo_vec is None or campplus_embedding is None:
-            raise ValueError("the B200 path needs emo_vec and campplus_embedding (what infer_v2_5.py:759-791 passes)")
+            raise ValueError("the engine path needs emo_vec and campplus_embedding (what infer_v2_5.py:759-791 passes)")
         nb = _check_hf_kwargs(num_return_sequences, typical_sampling, hf)
         sampling = dict(do_sample=bool(hf.get("do_sample", False)), top_k=int(hf.get("top_k", 0) or 0),
                         top_p=float(hf.get("top_p", 1.0)), temperature=float(hf.get("temperature", 1.0)),
@@ -266,7 +266,7 @@ def attach_v1(tts, engine: Engine = None, device: int = 0):
     def forward(speech_conditioning_latent, text_inputs, text_lengths, mel_codes, wav_lengths, cond_mel_lengths=None, types=None,
                 text_first=True, raw_mels=None, return_attentions=False, return_latent=False, clip_inputs=False):
         if not return_latent:
-            raise NotImplementedError("the B200 path implements the inference use of forward(): return_latent=True (infer.py:~640)")
+            raise NotImplementedError("the engine path implements the inference use of forward(): return_latent=True (infer.py:~640)")
         conds = _conds(speech_conditioning_latent)
         lat = engine.gpt_latents_v1(conds, text_inputs[0, : int(text_lengths[0])].cpu().numpy(), mel_codes[0].cpu().numpy())
         return torch.from_numpy(lat)[None].to(dev)

@@ -2,7 +2,7 @@
 
 The library is the product; this file only marshals pointers.  Tensors may be torch tensors
 (CPU or CUDA) or numpy arrays — the library accepts host or device pointers.  There is no CPU
-fallback: `Engine()` raises RuntimeError when no sm_100 device is visible or the library is
+fallback: `Engine()` raises RuntimeError when no sm_90 device is visible or the library is
 missing.
 """
 import ctypes as C
@@ -404,7 +404,7 @@ class Engine:
                     "idx_gpt_profile")
         return buf
 
-    def gpt_profile_fine(self, num_sms=148):
+    def gpt_profile_fine(self, num_sms=132):
         """[num_sms][64] sub-phase %globaltimer stamps (ns) of every CTA, middle layer of the last decode step."""
         buf = np.zeros((num_sms, 64), dtype=np.int64)
         self._check(self.lib.idx_gpt_profile_fine(self.h, _ptr(buf), buf.size), "idx_gpt_profile_fine")
@@ -583,7 +583,7 @@ class Engine:
     def debug_conv_gemm(self, A, wk, taps=1, dil=1, pad=0, M=None, bias=None, act=0, res=None, accum=False,
                         scale=1.0, out_off=0, ldo=None, out_valid=None, out_rows=None, backend=0, out_init=None,
                         biasN=0):
-        """One channels-last multi-tap GEMM through a chosen back end (1 SIMT, 2 tcgen05)."""
+        """One channels-last multi-tap GEMM through a chosen back end (1 SIMT, 2 wgmma)."""
         A = np.ascontiguousarray(A, dtype=np.float32)
         wk = np.ascontiguousarray(wk, dtype=np.float32)
         B, Tin, K = A.shape

@@ -1,5 +1,5 @@
 """`indextts_b200.infer.IndexTTS` — the v1 / v1.5 entry point (indextts/infer.py:29-32, 520-521) with its compute seams on
-the B200 engine: the reference object is built by the reference's own constructor, `dropin.attach_v1()` rebinds
+the CUDA engine: the reference object is built by the reference's own constructor, `dropin.attach_v1()` rebinds
 `gpt.inference_speech`, the latent pass `gpt(..., return_latent=True)` and `bigvgan(latent, mel_ref)`; `.infer()` /
 `.infer_fast()` stay the reference's code.  See infer_v2_5.py in this package for the import contract."""
 from .dropin import attach_v1

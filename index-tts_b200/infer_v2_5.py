@@ -1,4 +1,4 @@
-"""`indextts_b200.infer_v2_5.IndexTTS2` — the reference's entry-point class with its compute seams on the B200 engine.
+"""`indextts_b200.infer_v2_5.IndexTTS2` — the reference's entry-point class with its compute seams on the CUDA engine.
 
 Same constructor and `.infer()` / `.infer_generator()` signatures as `indextts.infer_v2_5.IndexTTS2`
 (infer_v2_5.py:77-80, 506-509, 570-573): the class builds the REFERENCE object with the reference's own config and
@@ -7,7 +7,7 @@ checkpoint loaders (so every loader quirk stays the reference's), then `dropin.a
 `.infer()` — text front-end, prompt caching, segment loop, timing prints, file output — is the reference's code, unmodified.
 
 The reference package must be importable (`pip install -e` of the index-tts checkout, or IDX_REFERENCE_ROOT pointing at
-it); this module does not vendor it.  There is no PyTorch-compute fallback: without a B200 the constructor raises."""
+it); this module does not vendor it.  There is no PyTorch-compute fallback: without an H100 the constructor raises."""
 import importlib
 import os
 import sys

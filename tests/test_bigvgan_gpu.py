@@ -1,6 +1,6 @@
 """GPU parity of the BigVGAN path (C-ABI) against goldens from the reference module and the CPU
 oracle.  Tolerances: Activation1d <= 1e-5 max-abs (fp32, SURVEY §8c); waveform RMS error <= 1e-3
-(north-star) with the default tcgen05 kind::tf32 convolutions — measured value is printed; max-abs
+(north-star) with the default wgmma tf32 convolutions — measured value is printed; max-abs
 <= 2e-2 guards against localised garbage; with the strict fp32 back end the error is ~1e-6."""
 import os
 

@@ -1,16 +1,60 @@
-"""CPU (build container only: needs /root/reference): `dropin.load_reference_weights` against the REAL reference
-modules.  The reference's own classes are instantiated (random init, small dims) through oracle/refimport.py, a
-recording stand-in replaces the engine, and the test checks that every hyper-parameter the drop-in derives from the
-modules' state dicts equals what the modules were constructed with, and that every tensor name the engine will ask for
-(`gpt.…`, `s2mel.…`, `codec.…`, `bigvgan.…`) is present.  Skipped where the reference tree is absent (GPU box)."""
+"""CPU: `dropin.load_reference_weights`, `attach` and `attach_v1` against what the reference's own modules expose.  The
+reference's classes were instantiated (random init, small dims) by oracle/make_goldens_dropin.py, which stored their
+state-dict names and shapes and the attributes the drop-in reads (tests/golden/dropin_modules.json); the reference's seam
+call sites are in tests/golden/reference_signatures.json (oracle/make_goldens_signatures.py).  Shape-only stand-ins are
+rebuilt from them, a recording stand-in replaces the engine, and the tests check that every hyper-parameter the drop-in
+derives from the modules' state dicts equals what the modules were constructed with, that every tensor name the engine
+will ask for (`gpt.…`, `s2mel.…`, `codec.…`, `bigvgan.…`) is present, and that the reference's calls bind to the
+callables the drop-in installs."""
+import json
+import os
 import types
 
-import pytest
 import torch
 
-from oracle import refimport
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
-pytestmark = pytest.mark.skipif(not refimport.available(), reason="/root/reference not present")
+
+def _golden(name):
+    with open(os.path.join(GOLDEN, name)) as f:
+        return json.load(f)
+
+
+class StandIn(torch.nn.Module):
+    """A module that has only the recorded state-dict entries (zeros of the recorded shapes)."""
+
+    def __init__(self, shapes, **attrs):
+        super().__init__()
+        self._shapes = shapes
+        for k, v in attrs.items():
+            object.__setattr__(self, k, v)
+
+    def state_dict(self, *a, **k):
+        return {n: torch.zeros(s) for n, s in self._shapes.items()}
+
+
+def _gpt(rec):
+    a = rec["attrs"]
+    sd = rec["state_dict"]
+    extra = dict(gpt=types.SimpleNamespace(h=[None] * a["layers"]),
+                 inference_model=types.SimpleNamespace(kv_cache=a["kv_cache"]))
+    if "emo_perceiver_heads" in a:
+        extra["emo_perceiver_encoder"] = types.SimpleNamespace(heads=a["emo_perceiver_heads"],
+                                                               latents=torch.zeros(sd["emo_perceiver_encoder.latents"]))
+    if "emo_input_size" in a:
+        extra["emo_input_size"] = a["emo_input_size"]
+    return StandIn(sd, **{k: a[k] for k in ("model_dim", "heads", "number_mel_codes", "start_mel_token", "stop_mel_token")},
+                   **extra)
+
+
+def _tts_v2_5():
+    g = _golden("dropin_modules.json")
+    gpt = _gpt(g["gpt"])
+    s2 = StandIn(g["s2mel"]["state_dict"])
+    s2.models = {"length_regulator": torch.nn.Module(), "cfm": types.SimpleNamespace(in_channels=80)}
+    codec = StandIn(g["codec"]["state_dict"])
+    bv = StandIn(g["bigvgan"]["state_dict"], h=g["bigvgan"]["attrs"]["h"])
+    return g, types.SimpleNamespace(gpt=gpt, s2mel=s2, semantic_codec=codec, bigvgan=bv)
 
 
 class RecordingEngine:
@@ -41,21 +85,10 @@ class RecordingEngine:
 
 
 def test_config_derivation_from_real_reference_modules():
-    from indextts_b200 import synth
     from indextts_b200.dropin import load_reference_weights
-    from oracle.gpt import make_gpt_weights
-    from oracle.validate_gpt_vs_hf import small_case
 
-    cfg, _, _, _ = small_case()
-    cfg = dict(cfg, n_langs=106)
-    gpt = refimport.gpt_module(cfg, make_gpt_weights(cfg, seed=1, bf16=False))
-    s2 = refimport.s2mel_module(refimport.s2mel_args(hidden=64, heads=1, depth=3, wn_hidden=64, wn_layers=2,
-                                                     content_dim=64, lr_in=96, style_dim=24))
-    codec = refimport.codec_module(codebook_size=64, hidden_size=96, codebook_dim=8, vocos_dim=48,
-                                   vocos_intermediate_dim=64, vocos_num_layers=2)
-    h = synth.small_config()
-    bv = refimport.bigvgan_module(h)
-    tts = types.SimpleNamespace(gpt=gpt, s2mel=s2, semantic_codec=codec, bigvgan=bv)
+    g, tts = _tts_v2_5()
+    cfg, h = g["cfg"], g["h"]
     eng = RecordingEngine()
     load_reference_weights(eng, tts, max_batch=4)
 
@@ -66,7 +99,7 @@ def test_config_derivation_from_real_reference_modules():
     assert k["max_batch"] == 4 and k["weights_bf16"] is True
     emo = eng.calls["emo_init"]
     assert (emo["idim"], emo["odim"], emo["linear_units"], emo["heads"], emo["blocks"]) == (1024, 32, 48, 2, 1)
-    assert emo["model_dim"] == cfg["model_dim"] and emo["p_dim"] == gpt.emo_perceiver_encoder.latents.shape[-1]
+    assert emo["model_dim"] == cfg["model_dim"] and emo["p_dim"] == tts.gpt.emo_perceiver_encoder.latents.shape[-1]
     s = eng.calls["s2mel_init"]
     assert (s["hidden"], s["heads"], s["depth"], s["wn_hidden"], s["wn_layers"], s["wn_kernel"]) == (64, 1, 3, 64, 2, 5)
     assert (s["in_channels"], s["content_dim"], s["style_dim"], s["lr_in"], s["lr_convs"]) == (80, 64, 24, 96, 4)
@@ -89,24 +122,8 @@ def test_config_derivation_from_real_reference_modules():
 
 
 def _reference_call_sites():
-    """(positional count, keyword names) of the calls `infer_generator` makes at the six seams (infer_v2_5.py:749-864),
-    read from the reference source with ast."""
-    import ast
-    import os
-    src = open(os.path.join(refimport.REF, "indextts", "infer_v2_5.py")).read()
-    tree = ast.parse(src)
-    want = {"self.gpt.merge_emovec": "merge_emovec", "self.gpt.inference_speech": "inference_speech",
-            "self.semantic_codec.decode": "codec_decode", "self.s2mel.models['length_regulator']": "length_regulator",
-            "self.s2mel.models['cfm'].inference": "cfm_inference", "self.bigvgan": "bigvgan"}
-    found = {}
-    for node in ast.walk(tree):
-        if isinstance(node, ast.Call):
-            name = ast.unparse(node.func)
-            if name in want:
-                kws = [k.arg for k in node.keywords if k.arg is not None]
-                star = any(k.arg is None for k in node.keywords)
-                found.setdefault(want[name], []).append((len(node.args), kws, star))
-    return found
+    """(positional count, keyword names) of the calls `infer_generator` makes at the six seams (infer_v2_5.py:749-864)."""
+    return _golden("reference_signatures.json")["call_sites_v2_5"]
 
 
 def test_rebound_seams_accept_the_reference_call_sites():
@@ -114,20 +131,10 @@ def test_rebound_seams_accept_the_reference_call_sites():
     arity, same keyword names) — the drop-in claim of INTEGRATION.md, checked against the reference source."""
     import inspect
 
-    from indextts_b200 import synth
     from indextts_b200.dropin import attach
-    from oracle.gpt import make_gpt_weights
-    from oracle.validate_gpt_vs_hf import small_case
 
-    cfg, _, _, _ = small_case()
-    cfg = dict(cfg, n_langs=106)
-    gpt = refimport.gpt_module(cfg, make_gpt_weights(cfg, seed=1, bf16=False))
-    s2 = refimport.s2mel_module(refimport.s2mel_args(hidden=64, heads=1, depth=3, wn_hidden=64, wn_layers=2,
-                                                     content_dim=64, lr_in=96, style_dim=24))
-    codec = refimport.codec_module(codebook_size=64, hidden_size=96, codebook_dim=8, vocos_dim=48,
-                                   vocos_intermediate_dim=64, vocos_num_layers=2)
-    bv = refimport.bigvgan_module(synth.small_config())
-    tts = types.SimpleNamespace(gpt=gpt, s2mel=s2, semantic_codec=codec, bigvgan=bv)
+    _, tts = _tts_v2_5()
+    gpt, bv = tts.gpt, tts.bigvgan
     eng = RecordingEngine()
     attach(tts, engine=eng)
     seams = {"merge_emovec": tts.gpt.merge_emovec, "inference_speech": tts.gpt.inference_speech,
@@ -150,20 +157,14 @@ def test_attach_v1_on_real_reference_v1_modules():
     """v1 / v1.5 drop-in (row a13): `attach_v1` on the reference's own v1 `UnifiedVoice` and `BigVGAN` classes — the derived
     prompt-encoder / vocoder configuration equals what the modules were built with, and the calls `indextts/infer.py` makes
     at the three seams bind to the rebound callables."""
-    import ast
     import inspect
-    import os
 
-    from indextts_b200 import synth
     from indextts_b200.dropin import attach_v1
-    from oracle.make_goldens_v1 import reference_module
-    from oracle.validate_gpt_vs_hf import small_case
 
-    cfg, _, _, _ = small_case()
-    ccfg = synth.small_v1_cond_cfg(cfg["model_dim"])
-    gpt = refimport.gpt_module_v1(cfg, ccfg, synth.make_gpt_v1_weights(cfg, ccfg, seed=3), kv_cache=False)
-    h = synth.small_v1_config()
-    bv = reference_module(h, synth.make_bigvgan_v1_weights(h, seed=5))
+    g = _golden("dropin_modules.json")
+    cfg, ccfg, h = g["cfg"], g["ccfg"], g["h1"]
+    gpt = _gpt(g["gpt_v1"])
+    bv = StandIn(g["bigvgan_v1"]["state_dict"], h=g["bigvgan_v1"]["attrs"]["h"])
     tts = types.SimpleNamespace(gpt=gpt, bigvgan=bv)
 
     class Rec(RecordingEngine):
@@ -185,13 +186,9 @@ def test_attach_v1_on_real_reference_v1_modules():
     assert "bigvgan_v1.speaker_encoder.blocks.0.conv.conv.weight" in eng.weights and "bigvgan_v1.cond_layer.weight" in eng.weights
     assert "gpt.conditioning_encoder.embed.out.0.weight" in eng.weights and "gpt.perceiver_encoder.latents" in eng.weights
     # call sites of indextts/infer.py
-    tree = ast.parse(open(os.path.join(refimport.REF, "indextts", "infer.py")).read())
-    want = {"self.gpt.inference_speech": tts.gpt.inference_speech, "self.gpt": tts.gpt.forward, "self.bigvgan": tts.bigvgan.forward}
-    seen = set()
-    for node in ast.walk(tree):
-        if isinstance(node, ast.Call) and ast.unparse(node.func) in want:
-            name = ast.unparse(node.func)
-            kws = [k.arg for k in node.keywords if k.arg is not None]
-            inspect.signature(want[name]).bind(*([None] * len(node.args)), **{k: None for k in kws})
-            seen.add(name)
-    assert seen == set(want)
+    sites = _golden("reference_signatures.json")["call_sites_v1"]
+    want = {"inference_speech": tts.gpt.inference_speech, "gpt_forward": tts.gpt.forward, "bigvgan": tts.bigvgan.forward}
+    for name, calls in sites.items():
+        for npos, kws, _ in calls:
+            inspect.signature(want[name]).bind(*([None] * npos), **{k: None for k in kws})
+    assert set(sites) == set(want)

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (tf32, TMA + TMEM) implicit-GEMM back end against the SIMT fp32 back end and a
+"""GPU: the wgmma (tf32, TMA + register accumulators) implicit-GEMM back end against the SIMT fp32 back end and a
 float64 numpy reference, over the shapes the vocoder / s2mel paths use (multi-tap, dilation, ragged
 K and N, ConvTranspose output mapping, fused epilogues).  tf32 keeps 10 mantissa bits: the bound is
 |err| <= 2e-3 * (sum_k |a||w|) per output, far looser than what is observed (printed)."""
@@ -51,7 +51,7 @@ def test_tc_matches_simt_and_fp64(engine, B, Tin, K, N, taps, dil, pad):
     print(f"tc max err {err.max():.2e} (ref max {np.abs(ref).max():.2f}, bound {2e-3 * mag.max():.2e}); "
           f"rel rms {np.sqrt((err ** 2).mean()) / np.sqrt((ref ** 2).mean()):.2e}")
     assert np.all(err <= 2e-3 * mag + 1e-5)
-    # fp16 operands (tcgen05 kind::f16, the round-2 tail path): same 10-bit mantissa, same bound; needs K % 8 == 0
+    # fp16 operands (wgmma .f16, the tail path): same 10-bit mantissa, same bound; needs K % 8 == 0
     if K % 8 == 0:
         h = engine.debug_conv_gemm(A, wk, taps, dil, pad, bias=bias, backend=3).reshape(B, Tin, N)
         errh = np.abs(h - ref)

@@ -2,7 +2,7 @@
 C-ABI against goldens minted from the reference modules and the CPU oracle.
 
 Two precisions are checked.  Strict fp32 (engine option gemm_backend=1, SIMT fp32 GEMMs): every stage
-within 1e-4 of the reference goldens.  Default (tcgen05 kind::tf32 GEMMs, 10-bit mantissa operands,
+within 1e-4 of the reference goldens.  Default (wgmma tf32 GEMMs, 10-bit mantissa operands,
 fp32 accumulate — what PyTorch's own conv path uses on Ampere+ with cudnn.allow_tf32): single
 stages / one DiT evaluation <= 1e-2 max-abs on O(1) activations (the TRT backend's own --verify
 bound, SURVEY §8c), CFM solve <= 2e-2 max-abs on mel values of std ~1.4; measured values printed."""

@@ -1,4 +1,4 @@
-"""BASELINE config 4: BigVGAN-only throughput sweep on one B200 (mel frames 128-4096, batch 1-16), device-resident
+"""BASELINE config 4: BigVGAN-only throughput sweep on one H100 (mel frames 128-4096, batch 1-16), device-resident
 mel and wav, CUDA-event time of idx_bigvgan_forward (engine stream).  Prints samples/s and the fraction of the
 measured dense bf16 tensor peak using 1.8037 GFLOP per mel frame (SURVEY section 8d); the GEMMs run in tf32.
     python -m tests.tools.bigvgan_sweep"""

@@ -1,5 +1,5 @@
 """BASELINE config 3: IndexTTS-2.5, 32 utterances of one speaker, 512 speech tokens each (20.45 s of audio each), full
-gpt -> codec -> length regulator -> CFM (25 steps, CFG 0.7, T = 861 + 1761) -> BigVGAN pipeline on ONE B200, synthetic
+gpt -> codec -> length regulator -> CFM (25 steps, CFG 0.7, T = 861 + 1761) -> BigVGAN pipeline on ONE H100, synthetic
 weights and inputs.  GPT decodes 8 utterances per group (4 groups back to back), the tail runs per utterance.
 Prints RTF (= wall / 654 s of audio) and speech-tokens/s (= 16384 / GPT time).
     python -m tests.tools.config3 [n_utt] [n_tokens]"""
