@@ -282,15 +282,49 @@ int idx_v1_vocode(idx_engine* e, const float* latent, int T, const float* mel_re
 int idx_bigvgan_last_ms(const idx_engine* e, double* ms);
 
 /* Diagnostic (tests): one multi-tap channels-last GEMM — the building block of every Conv1d /
- * ConvTranspose1d / Linear of the vocoder and s2mel paths — through a chosen back end
- * (backend 1 = SIMT fp32, 2 = wgmma tf32, 0 = automatic).  wk is K-major [N][taps*K];
- * D[b][m][n] = scale*(act(sum + bias) + res + (accum ? out : 0)) stored at
- * out[b*out_elems_per_batch + out_off + m*ldo + n] where 0 <= flat < out_valid.            */
-int idx_debug_conv_gemm(idx_engine* e, const float* A, int B, int Tin, int K, const float* wk,
-                        int taps, int dil, int pad, int M, int N, const float* bias, int biasN,
-                        int act, const float* res, int accum, float scale, long long out_off,
-                        int ldo, long long out_valid, long long out_elems_per_batch, int backend,
-                        float* out);
+ * ConvTranspose1d / Linear of the vocoder and s2mel paths — through a chosen back end and tile width.
+ *   acc[b][m][n] = sum_tap sum_k A[b][m + tap*dil - pad][k] * wk[b][n][tap*K + k]   (rows outside [0, Tin) read 0)
+ *   epi == 0: D = scale*((act(acc + bias[n % biasN]) * colscale[n] * rowscale[b][m]) + res + (accum ? out : 0)),
+ *             stored at out[b*out_elems_per_batch + out_off + m*ldo + n] where 0 <= flat < out_valid;
+ *   epi 1 (SwiGLU) / 2 (WaveNet gate): wk is the plain [w1; w3] / [a; c] weight, packed by the entry exactly as the
+ *             model packs it (rows interleaved, fp16); out16 [B][M][N/2] fp16;
+ *   epi 3 (RoPE): N = 3*heads*64 (q | k | v), aux = table [M][32][2] (cos, sin); out16 = Qr | Kr | Vb, each
+ *             [B*heads][M][64] fp16, q multiplied by scale (0: the scale the DiT uses for its flash attention).
+ * Every pointer may be host or device memory.  out / out16 carry `guard` extra elements on each side that are copied
+ * to the device and back with the output, so a caller can check that nothing outside the output was written.   */
+typedef struct {
+  const float* A;              /* [B or 1][Tin][lda]                                                   */
+  int32_t B, Tin, K, lda;      /* lda 0 -> K                                                           */
+  int32_t a_bcast;             /* 1: every batch entry reads the one A matrix                          */
+  const float* wk;             /* K-major [B or 1][N][ldw]                                             */
+  int32_t N, taps, dil, pad, ldw;   /* ldw 0 -> taps*K                                                 */
+  int32_t w_batched;           /* 1: one weight matrix per batch entry                                 */
+  int32_t M;
+  const float* bias; int32_t biasN; int32_t act;      /* act: 0 none, 1 GELU (erf), 2 SiLU, 3 Mish, 4 GELU (tanh), 5 ReLU */
+  const float* res;            /* indexed like out; ignored when res_is_out                            */
+  int32_t res_is_out;          /* 1: the residual is the initial content of out (in-place update)      */
+  int32_t accum; float scale;
+  const float* rowscale;       /* [B][M] or null                                                       */
+  const float* colscale;       /* [N] or null                                                          */
+  int64_t out_off; int32_t ldo; int64_t out_valid; int64_t out_elems_per_batch;   /* ldo 0 -> N        */
+  int32_t backend;             /* 1 SIMT fp32, 2 tensor core, 0 automatic                              */
+  int32_t operands;            /* 0 fp32 (tf32 on the tensor cores), 1 fp16 (A and wk rounded on the device) */
+  int32_t tile_n;              /* tensor-core tile width: 0 automatic, 32 / 64 / 128 forced            */
+  int32_t epi;                 /* 0 none, 1 SwiGLU, 2 WaveNet gate, 3 RoPE (fp16 operands only)        */
+  const float* aux;            /* epi 2: g [B][aux_stride] (aux_stride 0: one g for all); epi 3: RoPE table */
+  int32_t aux_stride, heads;
+  int64_t guard;               /* elements before and after out / out16 that belong to the caller (a multiple of 8) */
+  float* out;                  /* [B][out_elems_per_batch], in / out (epi == 0)                        */
+  uint16_t* out16;             /* fp16 output of epi 1..3                                              */
+} idx_debug_gemm;
+int idx_debug_conv_gemm(idx_engine* e, const idx_debug_gemm* g);
+
+/* Diagnostic (tests): one flash attention kernel on already rotated, split fp16 tensors q16 (already scaled: by 1/8
+ * for kernel 1, by log2(e)/8 for kernel 2), k16, v16 [B*H][T][64].  kernel: 0 = the one the DiT uses, 1 = mma.sync
+ * (softmax in e^x), 2 = wgmma (softmax in 2^x).  out [B][T][H*64] f32 and / or out16 (same layout, fp16), each with
+ * `guard` caller elements on both sides (see idx_debug_gemm).                                                     */
+int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16, int B,
+                              int T, int H, int kernel, long long guard, float* out, uint16_t* out16);
 
 /* ---------------------------------------------------------------- s2mel + codec -- */
 

@@ -578,6 +578,7 @@ void gemm_tc_launch(idx_engine* e, const ConvGemm& g) {
     const long long tiles128 = (long long)((g.N + 127) / 128) * ((g.M + BM - 1) / BM) * g.B;
     if (bn64 && BN == 128 && tiles128 < e->num_sms) BN = 64;
   }
+  if (e->force_tile_n) BN = e->force_tile_n;
   cuuint32_t bbox[3] = {(cuuint32_t)(BKB / EBh), (cuuint32_t)BN, 1};
   CUtensorMap tmB = make_map(half ? (const void*)g.Wk16 : (const void*)g.Wk, 3, bdims, bstr, bbox, half);
   if (half) {

@@ -730,8 +730,9 @@ static bool fa_wgmma_on() {
 }
 float flash_attention_q_scale() { return fa_wgmma_on() ? 0.125f * 1.4426950408889634f : 0.125f; }
 void flash_attention_split(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
-                           int B, int T, int H) {
-  if (fa_wgmma_on()) {
+                           int B, int T, int H, int kernel) {
+  IDX_CHECK(kernel >= FA_KERNEL_DEFAULT && kernel <= FA_KERNEL_WGMMA, IDX_ERR_ARG, "flash_attention_split: unknown kernel");
+  if (kernel == FA_KERNEL_WGMMA || (kernel == FA_KERNEL_DEFAULT && fa_wgmma_on())) {
     flash_attention_wgmma(e, Qr, Kr, Vb, out, out16, B, T, H);
     return;
   }

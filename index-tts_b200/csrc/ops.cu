@@ -348,66 +348,161 @@ __global__ void kmajor_to_simt_kernel(const float* wk, float* ws, int N, int KT)
 }
 }  // namespace
 
-// Diagnostic entry (tests): run one multi-tap GEMM through a chosen back end.
-// wk is the K-major weight [N][taps*K]; out is [B][out_rows][ldo]-shaped via (out_off, ldo, out_valid).
-extern "C" int idx_debug_conv_gemm(idx_engine* e, const float* A, int B, int Tin, int K, const float* wk, int taps,
-                                   int dil, int pad, int M, int N, const float* bias, int biasN, int act,
-                                   const float* res, int accum, float scale, long long out_off, int ldo,
-                                   long long out_valid, long long out_elems_per_batch, int backend, float* out) {
+namespace {
+// restores the engine's diagnostic overrides however the debug entry leaves
+struct DebugOverrides {
+  idx_engine* e;
+  ~DebugOverrides() { e->force_backend = 0; e->force_tile_n = 0; }
+};
+}  // namespace
+
+// Diagnostic entry (tests): run one multi-tap GEMM through a chosen back end, operand format and tile width
+// (include/idxtts.h, idx_debug_gemm).  Every operand is staged into the arena; out / out16 travel with their guard bands.
+extern "C" int idx_debug_conv_gemm(idx_engine* e, const idx_debug_gemm* d) {
   IDX_API_BEGIN
-  IDX_CHECK(e && A && wk && out, IDX_ERR_ARG, "null argument");
+  IDX_CHECK(e && d && d->A && d->wk, IDX_ERR_ARG, "null argument");
+  const bool fused = d->epi != EPI_NONE;
+  IDX_CHECK(d->B > 0 && d->Tin > 0 && d->K > 0 && d->N > 0 && d->M > 0 && d->taps > 0, IDX_ERR_ARG, "idx_debug_conv_gemm: bad shape");
+  IDX_CHECK(d->epi >= EPI_NONE && d->epi <= EPI_ROPE, IDX_ERR_ARG, "idx_debug_conv_gemm: unknown epi");
+  IDX_CHECK(fused ? (d->out16 && d->operands == 1) : d->out != nullptr, IDX_ERR_ARG,
+            "idx_debug_conv_gemm: epi 0 writes out; the fused epilogues write out16 and need fp16 operands");
+  IDX_CHECK(d->operands == 0 || (d->operands == 1 && d->backend != 1), IDX_ERR_ARG,
+            "idx_debug_conv_gemm: fp16 operands exist on the tensor-core path only");
+  IDX_CHECK(d->tile_n == 0 || d->tile_n == 32 || d->tile_n == 64 || d->tile_n == 128, IDX_ERR_ARG,
+            "idx_debug_conv_gemm: tile_n is 0, 32, 64 or 128");
+  IDX_CHECK(d->guard >= 0 && d->guard % 8 == 0, IDX_ERR_ARG, "idx_debug_conv_gemm: guard must be a non-negative multiple of 8");
   IDX_CUDA(cudaSetDevice(e->device));
-  const size_t na = (size_t)B * Tin * K, nw = (size_t)N * taps * K, no = (size_t)B * out_elems_per_batch;
-  e->ensure_arena(4 * (2 * na + 3 * nw + 2 * no + (size_t)N) + (1 << 20));
+  const int B = d->B, M = d->M, N = d->N, KT = d->taps * d->K;
+  const int lda = d->lda ? d->lda : d->K, ldw = d->ldw ? d->ldw : KT;
+  IDX_CHECK(lda >= d->K && ldw >= KT, IDX_ERR_ARG, "idx_debug_conv_gemm: lda < K or ldw < taps*K");
+  const size_t na = (size_t)(d->a_bcast ? 1 : B) * d->Tin * lda, nw = (size_t)(d->w_batched ? B : 1) * N * ldw;
+  const size_t no = fused ? 0 : (size_t)B * d->out_elems_per_batch;
+  const size_t no16 = d->epi == EPI_ROPE ? (size_t)B * M * N : (size_t)B * M * (N / 2);
+  const int nbias = d->biasN ? d->biasN : N;
+  size_t naux = 0;
+  if (d->epi == EPI_ROPE) {
+    IDX_CHECK(d->aux && d->heads > 0 && N == 3 * d->heads * 64, IDX_ERR_ARG, "idx_debug_conv_gemm: RoPE needs N = 3*heads*64 and a table");
+    naux = (size_t)M * 64;
+  } else if (d->epi == EPI_WNGATE) {
+    IDX_CHECK(d->aux && d->aux_stride >= 0, IDX_ERR_ARG, "idx_debug_conv_gemm: the WaveNet gate needs g");
+    naux = (size_t)(B - 1) * d->aux_stride + N;
+  }
+  if (d->epi == EPI_SWIGLU || d->epi == EPI_WNGATE)
+    IDX_CHECK(!d->w_batched && ldw == KT, IDX_ERR_ARG, "idx_debug_conv_gemm: pair epilogues take one dense [N][taps*K] weight");
+  const size_t g2 = 2 * (size_t)d->guard;
+  // bytes: A fp32 + fp16, Wk fp32 + SIMT copy + fp16, out + res, out16, bias / aux / scales, alignment slack
+  e->ensure_arena(6 * na + 10 * nw + 4 * (no + g2) + 4 * no + 2 * (no16 + g2) + 4 * (nbias + naux + (size_t)B * M + N) + (16 << 20));
   e->arena.reset();
   float* dA = e->arena.get<float>(na);
   float* dWk = e->arena.get<float>(nw);
-  float* dWs = e->arena.get<float>(nw);
-  float* dOut = e->arena.get<float>(no);
-  float* dRes = res ? e->arena.get<float>(no) : nullptr;
-  float* dBias = bias ? e->arena.get<float>(biasN ? biasN : N) : nullptr;
-  idx_to_device(e, dA, A, na * 4);
-  idx_to_device(e, dWk, wk, nw * 4);
-  idx_to_device(e, dOut, out, no * 4);   // initial contents matter for accum
-  if (res) idx_to_device(e, dRes, res, no * 4);
-  if (bias) idx_to_device(e, dBias, bias, (size_t)(biasN ? biasN : N) * 4);
-  kmajor_to_simt_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, e->stream>>>(dWk, dWs, N, taps * K);
-  IDX_CUDA(cudaGetLastError());
+  idx_to_device(e, dA, d->A, na * 4);
+  idx_to_device(e, dWk, d->wk, nw * 4);
+  auto stage = [&](const float* src, size_t n) -> float* {
+    if (!src) return nullptr;
+    float* p = e->arena.get<float>(n);
+    idx_to_device(e, p, src, n * 4);
+    return p;
+  };
+  float* dOut = nullptr;
+  __half* dOut16 = nullptr;
+  if (fused) {
+    dOut16 = (__half*)e->arena.alloc((no16 + g2) * 2);
+    idx_to_device(e, dOut16, d->out16 - d->guard, (no16 + g2) * 2);
+  } else {
+    dOut = stage(d->out - d->guard, no + g2);   // initial contents matter for accum / an in-place residual
+  }
+  const float* dRes = d->res_is_out ? (dOut ? dOut + d->guard : nullptr) : stage(d->res, no);
+  const float* dBias = stage(d->bias, nbias);
+  const float* dRow = stage(d->rowscale, (size_t)B * M);
+  const float* dCol = stage(d->colscale, N);
+  const float* dAux = stage(d->aux, naux);
+
   ConvGemm g;
-  g.A = dA; g.B = B; g.Tin = Tin; g.K = K; g.W = dWs; g.Wk = dWk; g.taps = taps; g.dil = dil; g.pad = pad;
-  g.M = M; g.N = N; g.bias = dBias; g.biasN = biasN; g.act = act; g.res = dRes; g.accum = accum; g.scale = scale;
-  g.out = dOut; g.out_off = out_off; g.ldo = ldo; g.out_valid = out_valid; g.out_batch_stride = out_elems_per_batch;
-  if (backend == 3) {          // fp16 operands on the tensor cores: convert A and the K-major weights on the device
-    __half* dA16 = (__half*)e->arena.get<float>(na / 2 + 4);
-    __half* dW16 = (__half*)e->arena.get<float>(nw / 2 + 4);
+  g.A = dA; g.B = B; g.Tin = d->Tin; g.K = d->K; g.lda = d->lda; g.a_bcast = d->a_bcast;
+  g.Wk = dWk; g.ldw = d->ldw; g.w_batch_stride = d->w_batched ? (long long)N * ldw : 0;
+  if (!d->w_batched && ldw == KT && !d->operands) {   // the SIMT kernel's [taps][K][N] copy
+    float* dWs = e->arena.get<float>(nw);
+    kmajor_to_simt_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, e->stream>>>(dWk, dWs, N, KT);
+    IDX_CUDA(cudaGetLastError());
+    g.W = dWs;
+  }
+  g.taps = d->taps; g.dil = d->dil; g.pad = d->pad;
+  g.M = M; g.N = N; g.bias = dBias; g.biasN = d->biasN; g.act = d->act; g.res = dRes; g.accum = d->accum;
+  g.rowscale = dRow; g.colscale = dCol; g.scale = d->scale;
+  g.out = dOut ? dOut + d->guard : nullptr;
+  g.out_off = d->out_off; g.ldo = d->ldo; g.out_valid = d->out_valid; g.out_batch_stride = d->out_elems_per_batch;
+  WeightPool pool;
+  if (d->operands == 1) {      // fp16 operands on the tensor cores: round A and the K-major weights on the device
+    __half* dA16 = (__half*)e->arena.alloc(na * 2);
     to_half(e, dA, dA16, (long long)na);
-    to_half(e, dWk, dW16, (long long)nw);
-    g.A16 = dA16; g.Wk16 = dW16;
-    backend = 0;
-  }
-  e->force_backend = backend;
-  try {
-    conv_gemm(e, g);
-    // timing loop (diagnostics): env IDX_GEMM_REPS=n repeats the launch between CUDA events
-    static const int reps = getenv("IDX_GEMM_REPS") ? atoi(getenv("IDX_GEMM_REPS")) : 0;
-    if (reps > 0) {
-      cudaEvent_t a, b2;
-      IDX_CUDA(cudaEventCreate(&a)); IDX_CUDA(cudaEventCreate(&b2));
-      IDX_CUDA(cudaEventRecord(a, e->stream));
-      for (int i = 0; i < reps; ++i) conv_gemm(e, g);
-      IDX_CUDA(cudaEventRecord(b2, e->stream));
-      IDX_CUDA(cudaEventSynchronize(b2));
-      float ms = 0; IDX_CUDA(cudaEventElapsedTime(&ms, a, b2));
-      fprintf(stderr, "[idx_debug_conv_gemm] backend %d B=%d M=%d N=%d K=%d taps=%d: %.2f us/launch, %.1f TFLOP/s\n", backend, B,
-              M, N, K, taps, ms * 1000.0 / reps, 2.0 * B * M * (double)N * K * taps / (ms / reps * 1e-3) / 1e12);
-      cudaEventDestroy(a); cudaEventDestroy(b2);
+    g.A16 = dA16;
+    if (d->epi == EPI_SWIGLU || d->epi == EPI_WNGATE) {
+      PackedW w;
+      w.wk = dWk; w.N = N; w.K = d->K; w.taps = d->taps; w.bias = dBias;
+      float* bias_i = nullptr;
+      g.Wk16 = pack_half_interleaved(e, pool, w, &bias_i);    // the pair layout the model's weights get at init
+      g.bias = bias_i;
+    } else {
+      __half* dW16 = (__half*)e->arena.alloc(nw * 2);
+      to_half(e, dWk, dW16, (long long)nw);
+      g.Wk16 = dW16;
     }
-  } catch (...) {
-    e->force_backend = 0;
-    throw;
+    g.epi = d->epi;
+    g.out16 = dOut16 ? dOut16 + d->guard : nullptr;
+    g.aux = dAux;
+    g.aux_stride = d->epi == EPI_ROPE ? d->heads : d->aux_stride;
+    if (d->epi == EPI_ROPE && d->scale == 0.f) g.scale = flash_attention_q_scale();
   }
-  e->force_backend = 0;
-  idx_from_device(e, out, dOut, no * 4);
+  DebugOverrides restore{e};
+  e->force_backend = d->operands == 1 ? 0 : d->backend;
+  e->force_tile_n = d->tile_n;
+  conv_gemm(e, g);
+  // timing loop (diagnostics): env IDX_GEMM_REPS=n repeats the launch between CUDA events
+  static const int reps = getenv("IDX_GEMM_REPS") ? atoi(getenv("IDX_GEMM_REPS")) : 0;
+  if (reps > 0) {
+    cudaEvent_t a, b2;
+    IDX_CUDA(cudaEventCreate(&a)); IDX_CUDA(cudaEventCreate(&b2));
+    IDX_CUDA(cudaEventRecord(a, e->stream));
+    for (int i = 0; i < reps; ++i) conv_gemm(e, g);
+    IDX_CUDA(cudaEventRecord(b2, e->stream));
+    IDX_CUDA(cudaEventSynchronize(b2));
+    float ms = 0; IDX_CUDA(cudaEventElapsedTime(&ms, a, b2));
+    fprintf(stderr, "[idx_debug_conv_gemm] backend %d operands %d B=%d M=%d N=%d K=%d taps=%d: %.2f us/launch, %.1f TFLOP/s\n",
+            d->backend, d->operands, B, M, N, d->K, d->taps, ms * 1000.0 / reps,
+            2.0 * B * M * (double)N * d->K * d->taps / (ms / reps * 1e-3) / 1e12);
+    cudaEventDestroy(a); cudaEventDestroy(b2);
+  }
+  if (dOut) idx_from_device(e, d->out - d->guard, dOut, (no + g2) * 4);
+  if (dOut16) idx_from_device(e, d->out16 - d->guard, dOut16, (no16 + g2) * 2);
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  pool.release();
+  IDX_API_END(e)
+}
+
+// Diagnostic entry (tests): one flash attention kernel on fp16 q / k / v [B*H][T][64] (include/idxtts.h).
+extern "C" int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16, int B,
+                                         int T, int H, int kernel, long long guard, float* out, uint16_t* out16) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && q16 && k16 && v16 && (out || out16), IDX_ERR_ARG, "null argument");
+  IDX_CHECK(B > 0 && T > 0 && H > 0, IDX_ERR_ARG, "idx_debug_flash_attention: bad shape");
+  IDX_CHECK(guard >= 0 && guard % 8 == 0, IDX_ERR_ARG, "idx_debug_flash_attention: guard must be a non-negative multiple of 8");
+  IDX_CUDA(cudaSetDevice(e->device));
+  const size_t n = (size_t)B * H * T * 64, ng = n + 2 * (size_t)guard;
+  e->ensure_arena(3 * 2 * n + 6 * ng + (16 << 20));
+  e->arena.reset();
+  __half* dq = (__half*)e->arena.alloc(2 * n);
+  __half* dk = (__half*)e->arena.alloc(2 * n);
+  __half* dv = (__half*)e->arena.alloc(2 * n);
+  idx_to_device(e, dq, q16, 2 * n);
+  idx_to_device(e, dk, k16, 2 * n);
+  idx_to_device(e, dv, v16, 2 * n);
+  float* dOut = out ? e->arena.get<float>(ng) : nullptr;
+  __half* dOut16 = out16 ? (__half*)e->arena.alloc(2 * ng) : nullptr;
+  if (dOut) idx_to_device(e, dOut, out - guard, 4 * ng);
+  if (dOut16) idx_to_device(e, dOut16, out16 - guard, 2 * ng);
+  flash_attention_split(e, dq, dk, dv, dOut ? dOut + guard : nullptr, dOut16 ? dOut16 + guard : nullptr, B, T, H, kernel);
+  if (dOut) idx_from_device(e, out - guard, dOut, 4 * ng);
+  if (dOut16) idx_from_device(e, out16 - guard, dOut16, 2 * ng);
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   IDX_API_END(e)
 }

@@ -153,9 +153,11 @@ void pack_half(idx_engine* e, WeightPool& pool, PackedW& w);
 // fp16 K-major copy of w.wk with the two halves of the output rows interleaved (row 2j = row j, row 2j+1 = row N/2 + j): the
 // weight layout of the EPI_SWIGLU / EPI_WNGATE pair epilogues; bias_out (optional) receives the bias interleaved the same way
 __half* pack_half_interleaved(idx_engine* e, WeightPool& pool, const PackedW& w, float** bias_out);
-// the fused flash attention on already rotated / split fp16 tensors Qr | Kr | Vb [B*H][T][64] (what EPI_ROPE writes)
+// the fused flash attention on already rotated / split fp16 tensors Qr | Kr | Vb [B*H][T][64] (what EPI_ROPE writes);
+// kernel: 0 = the default (wgmma unless IDX_FA_WGMMA=0), 1 = mma.sync, 2 = wgmma
+enum { FA_KERNEL_DEFAULT = 0, FA_KERNEL_MMA = 1, FA_KERNEL_WGMMA = 2 };
 void flash_attention_split(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
-                           int B, int T, int H);
+                           int B, int T, int H, int kernel = FA_KERNEL_DEFAULT);
 // scale EPI_ROPE must apply to q for flash_attention_split: 1/8, times log2(e) when the wgmma kernel (exp2 softmax) is on
 float flash_attention_q_scale();
 // the same on wgmma (gemm_tc.cu: S and O in registers, P fed back as a register operand)

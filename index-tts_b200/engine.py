@@ -77,6 +77,46 @@ class VocodeRequest(C.Structure):
                 ("F", C.c_int32), ("wav_out", C.c_void_p), ("pcm16_out", C.c_void_p), ("mel_out", C.c_void_p)]
 
 
+class DebugGemm(C.Structure):
+    """include/idxtts.h idx_debug_gemm."""
+    _fields_ = [("A", C.c_void_p), ("B", C.c_int32), ("Tin", C.c_int32), ("K", C.c_int32), ("lda", C.c_int32),
+                ("a_bcast", C.c_int32), ("wk", C.c_void_p), ("N", C.c_int32), ("taps", C.c_int32), ("dil", C.c_int32),
+                ("pad", C.c_int32), ("ldw", C.c_int32), ("w_batched", C.c_int32), ("M", C.c_int32),
+                ("bias", C.c_void_p), ("biasN", C.c_int32), ("act", C.c_int32), ("res", C.c_void_p),
+                ("res_is_out", C.c_int32), ("accum", C.c_int32), ("scale", C.c_float), ("rowscale", C.c_void_p),
+                ("colscale", C.c_void_p), ("out_off", C.c_int64), ("ldo", C.c_int32), ("out_valid", C.c_int64),
+                ("out_elems_per_batch", C.c_int64), ("backend", C.c_int32), ("operands", C.c_int32),
+                ("tile_n", C.c_int32), ("epi", C.c_int32), ("aux", C.c_void_p), ("aux_stride", C.c_int32),
+                ("heads", C.c_int32), ("guard", C.c_int64), ("out", C.c_void_p), ("out16", C.c_void_p)]
+
+
+# Guard bands of the diagnostic entries: sentinel NaNs (a payload no kernel produces) on both sides of every output,
+# at least one 128-row tile long, so a store to a row or column outside the output lands in them.
+_SENTINEL32 = np.uint32(0x7FC0DEAD)
+_SENTINEL16 = np.uint16(0x7E5A)
+
+
+def _guarded(n, guard, dtype, init=None):
+    bits = np.uint32 if dtype == np.float32 else np.uint16
+    buf = np.empty(n + 2 * guard, dtype=bits)
+    buf[:] = _SENTINEL32 if dtype == np.float32 else _SENTINEL16
+    if init is not None:
+        buf[guard:guard + n] = np.ascontiguousarray(init, dtype=dtype).reshape(-1).view(bits)
+    return buf
+
+
+def _check_guard(buf, guard, n, what):
+    sent = _SENTINEL32 if buf.dtype == np.uint32 else _SENTINEL16
+    head, tail = buf[:guard], buf[guard + n:]
+    if not (np.all(head == sent) and np.all(tail == sent)):
+        raise AssertionError(f"{what} wrote outside its output: {int((head != sent).sum())} elements before, "
+                             f"{int((tail != sent).sum())} after")
+
+
+def _guard_len(row_elems):
+    return max(4096, (128 * int(row_elems) + 7) // 8 * 8)
+
+
 def fold_weight_norm(sd):
     """torch weight_norm (dim=0) folded into a plain `.weight`: w = g * v / ||v|| — what
     remove_weight_norm() / the parametrisation computes on the fly in the reference."""
@@ -150,9 +190,9 @@ def load_library(path: str = None):
     lib.idx_antialias_snake.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.idx_bigvgan_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
-    lib.idx_debug_conv_gemm.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
-                                        C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
-                                        C.c_float, C.c_longlong, C.c_int, C.c_longlong, C.c_longlong, C.c_int, C.c_void_p]
+    lib.idx_debug_conv_gemm.argtypes = [C.c_void_p, C.POINTER(DebugGemm)]
+    lib.idx_debug_flash_attention.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                              C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]
     lib.idx_s2mel_init.argtypes = [C.c_void_p, C.POINTER(S2melConfig)]
     lib.idx_codec_init.argtypes = [C.c_void_p, C.POINTER(CodecConfig)]
     lib.idx_codec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -582,25 +622,91 @@ class Engine:
     # --------------------------------------------------------------- diagnostics --
     def debug_conv_gemm(self, A, wk, taps=1, dil=1, pad=0, M=None, bias=None, act=0, res=None, accum=False,
                         scale=1.0, out_off=0, ldo=None, out_valid=None, out_rows=None, backend=0, out_init=None,
-                        biasN=0):
-        """One channels-last multi-tap GEMM through a chosen back end (1 SIMT, 2 wgmma)."""
+                        biasN=0, K=None, B=None, operands=0, tile_n=0, a_bcast=False, w_batched=False, rowscale=None,
+                        colscale=None, res_is_out=False, pad_cols=0, epi=0, aux=None, aux_stride=0, heads=0):
+        """One channels-last multi-tap GEMM (include/idxtts.h, idx_debug_gemm) through a chosen back end (1 SIMT,
+        2 wgmma, 0 automatic), operand format (0 fp32 / tf32, 1 fp16) and tensor-core tile width (0 automatic).
+        A is [B or 1][Tin][lda] (lda = A.shape[-1], K defaults to it); wk is [N][ldw] or, with w_batched, [B][N][ldw]
+        (ldw = wk.shape[-1], taps*K by default).  pad_cols > 0 stores rows at ldo = N + pad_cols and checks that the
+        extra columns stay untouched.  Returns out [B][out_elems_per_batch] (epi 0, [B][M][N] with pad_cols), the
+        fp16 Qr | Kr | Vb [3][B*heads][M][64] (epi 3) or the fp16 pair result [B][M][N/2] (epi 1, 2).  Raises
+        AssertionError when the kernel wrote outside its output."""
         A = np.ascontiguousarray(A, dtype=np.float32)
         wk = np.ascontiguousarray(wk, dtype=np.float32)
-        B, Tin, K = A.shape
-        N = wk.shape[0]
+        Ab, Tin, lda = A.shape
+        B = Ab if B is None else int(B)
+        K = lda if K is None else int(K)
+        N, ldw = wk.shape[-2], wk.shape[-1]
+        assert (Ab == 1 if a_bcast else Ab == B) and (wk.ndim == 3 and wk.shape[0] == B if w_batched else wk.ndim == 2)
         M = Tin if M is None else M
+        if pad_cols:
+            assert ldo is None and out_valid is None and out_rows is None and out_off == 0
+            ldo = N + pad_cols
         ldo = N if ldo is None else ldo
         out_rows = M if out_rows is None else out_rows
         per = out_rows * ldo if out_valid is None else int(out_valid)
-        out_valid = per
-        out = np.zeros((B, per), dtype=np.float32) if out_init is None else np.ascontiguousarray(out_init, dtype=np.float32).reshape(B, per).copy()
-        b_ = None if bias is None else np.ascontiguousarray(bias, dtype=np.float32)
-        r_ = None if res is None else np.ascontiguousarray(res, dtype=np.float32).reshape(B, per)
-        self._check(self.lib.idx_debug_conv_gemm(self.h, _ptr(A), B, Tin, K, _ptr(wk), taps, dil, pad, M, N, _ptr(b_),
-                                                 biasN, act, _ptr(r_), int(accum), float(scale), int(out_off), ldo,
-                                                 int(out_valid), int(per), int(backend), _ptr(out)),
-                    "idx_debug_conv_gemm")
-        return out
+        f32 = lambda x: None if x is None else np.ascontiguousarray(x, dtype=np.float32)
+        g = DebugGemm(A=_ptr(A), B=B, Tin=Tin, K=K, lda=lda, a_bcast=int(a_bcast), wk=_ptr(wk), N=N, taps=taps, dil=dil,
+                      pad=pad, ldw=ldw, w_batched=int(w_batched), M=M, bias=None, biasN=biasN, act=act, res=None,
+                      res_is_out=int(res_is_out), accum=int(accum), scale=float(scale), out_off=int(out_off), ldo=ldo,
+                      out_valid=per, out_elems_per_batch=per, backend=int(backend), operands=int(operands),
+                      tile_n=int(tile_n), epi=int(epi), aux_stride=int(aux_stride), heads=int(heads))
+        keep = [f32(bias), f32(res), f32(rowscale), f32(colscale), f32(aux)]
+        g.bias, g.res, g.rowscale, g.colscale, g.aux = (_ptr(x) for x in keep)
+        if res is not None:
+            assert keep[1].size == B * per
+        if epi == 0:
+            n = B * per
+            guard = _guard_len(ldo)
+            init = np.zeros(n, np.float32) if out_init is None else out_init
+            if pad_cols and out_init is not None:
+                init = np.zeros((B, M, ldo), np.float32)
+                init[..., :N] = np.asarray(out_init, np.float32).reshape(B, M, N)
+            buf = _guarded(n, guard, np.float32, init)
+            if pad_cols:      # the columns >= N of every row are sentinels as well
+                buf[guard:guard + n].reshape(B, M, ldo)[..., N:] = _SENTINEL32
+            g.out, g.guard = buf.ctypes.data + 4 * guard, guard
+        else:
+            n = B * M * N if epi == 3 else B * M * (N // 2)
+            guard = _guard_len(64 if epi == 3 else N // 2)
+            buf = _guarded(n, guard, np.float16)
+            g.out16, g.guard = buf.ctypes.data + 2 * guard, guard
+        self._check(self.lib.idx_debug_conv_gemm(self.h, C.byref(g)), "idx_debug_conv_gemm")
+        _check_guard(buf, guard, n, "idx_debug_conv_gemm")
+        out = buf[guard:guard + n]
+        if epi == 3:
+            return out.view(np.float16).reshape(3, B * heads, M, 64)
+        if epi:
+            return out.view(np.float16).reshape(B, M, N // 2)
+        if pad_cols:
+            o = out.reshape(B, M, ldo)
+            assert np.all(o[..., N:] == _SENTINEL32), "idx_debug_conv_gemm wrote columns >= N"
+            return o[..., :N].view(np.float32).copy()
+        return out.view(np.float32).reshape(B, per).copy()
+
+    def debug_flash_attention(self, q16, k16, v16, B, H, kernel=0, out=True, out16=True):
+        """One flash attention kernel (include/idxtts.h idx_debug_flash_attention) on fp16 q (already scaled), k, v
+        [B*H][T][64].  Returns (out [B][T][H*64] f32 or None, out16 [B][T][H*64] fp16 or None); raises AssertionError
+        when the kernel wrote outside them."""
+        q16, k16, v16 = (np.ascontiguousarray(x, dtype=np.float16) for x in (q16, k16, v16))
+        BH, T, D = q16.shape
+        assert D == 64 and BH == B * H and k16.shape == q16.shape and v16.shape == q16.shape
+        n, guard = B * T * H * 64, _guard_len(H * 64)
+        b32 = _guarded(n, guard, np.float32) if out else None
+        b16 = _guarded(n, guard, np.float16) if out16 else None
+        self._check(self.lib.idx_debug_flash_attention(
+            self.h, _ptr(q16), _ptr(k16), _ptr(v16), B, T, H, int(kernel), guard,
+            None if b32 is None else b32.ctypes.data + 4 * guard, None if b16 is None else b16.ctypes.data + 2 * guard),
+            "idx_debug_flash_attention")
+        res = []
+        for buf in (b32, b16):
+            if buf is None:
+                res.append(None)
+                continue
+            _check_guard(buf, guard, n, "idx_debug_flash_attention")
+            dt = np.float32 if buf.dtype == np.uint32 else np.float16
+            res.append(buf[guard:guard + n].view(dt).reshape(B, T, H * 64).copy())
+        return tuple(res)
 
     # ------------------------------------------------------------------- emotion --
     def emo_init(self, c: dict):

@@ -1,0 +1,106 @@
+"""float64 references of the tensor-core kernels' operations, computed on exactly the operands the kernels read.
+tests/test_kernel_refs_cpu.py pins each of them against PyTorch / the oracle, so that a failing GPU comparison
+points at the kernel and not at its reference."""
+import math
+
+import numpy as np
+import torch
+
+
+def ref_conv(A, wk, taps, dil, pad, M):
+    """Multi-tap channels-last GEMM (Conv1d with zero padding):
+        out[b][m][n] = sum_tap sum_k A[b][m + tap*dil - pad][k] * wk[b][n][tap*K + k].
+    A [B or 1][Tin][K]; wk [N][taps*K] (shared) or [B][N][taps*K] (per batch entry).  Returns (out, mag), both
+    float64 [B][M][N]; mag = the same sum over |A| |wk|, the scale of any summation error."""
+    A = np.asarray(A, np.float64)
+    W = np.asarray(wk, np.float64)
+    B = max(A.shape[0], W.shape[0] if W.ndim == 3 else 1)
+    if W.ndim == 2:
+        W = W[None]
+    A = np.broadcast_to(A, (B,) + A.shape[1:])
+    W = np.broadcast_to(W, (B,) + W.shape[1:])
+    Tin, K = A.shape[1], A.shape[2]
+    N = W.shape[1]
+    W = W.reshape(B, N, taps, K)
+    out = np.zeros((B, M, N), np.float64)
+    mag = np.zeros((B, M, N), np.float64)
+    for t in range(taps):
+        rows = np.arange(M) + t * dil - pad
+        ok = (rows >= 0) & (rows < Tin)
+        a = np.zeros((B, M, K), np.float64)
+        a[:, ok] = A[:, rows[ok]]
+        wt = W[:, :, t].transpose(0, 2, 1)
+        out += a @ wt
+        mag += np.abs(a) @ np.abs(wt)
+    return out, mag
+
+
+def act(x, kind):
+    """The GEMM epilogue activations (ops.h ACT_*) in float64."""
+    x = np.asarray(x, np.float64)
+    if kind == 0:
+        return x
+    if kind == 1:
+        return 0.5 * x * (1.0 + np.vectorize(math.erf)(x / math.sqrt(2.0)))
+    if kind == 2:
+        return x / (1.0 + np.exp(-x))
+    if kind == 3:
+        return x * np.tanh(np.logaddexp(0.0, x))
+    if kind == 4:
+        return 0.5 * x * (1.0 + np.tanh(math.sqrt(2.0 / math.pi) * (x + 0.044715 * x ** 3)))
+    if kind == 5:
+        return np.maximum(x, 0.0)
+    raise ValueError(kind)
+
+
+def flash_attention(q, k, v, base):
+    """Full (non-causal) attention of the flash kernels on their exact inputs: q (already scaled), k, v [BH][T][64]
+    (the fp16 values the kernel reads).  Weights p_ij = base^(q_i . k_j): base 2 for the wgmma kernel (q carries
+    log2 e), e for the mma.sync kernel.  Returns (out, vmag) float64 [BH][T][64]; vmag = sum_j p_ij |v_j| / sum_j p_ij,
+    the scale of an error in the weights."""
+    q, k, v = (np.asarray(x, np.float64) for x in (q, k, v))
+    lb = math.log(base)
+    out = np.empty_like(q)
+    vmag = np.empty_like(q)
+    for i in range(q.shape[0]):
+        s = (q[i] @ k[i].T) * lb
+        p = np.exp(s - s.max(axis=1, keepdims=True))
+        l = p.sum(axis=1, keepdims=True)
+        out[i] = (p @ v[i]) / l
+        vmag[i] = (p @ np.abs(v[i])) / l
+    return out, vmag
+
+
+def rope_angles(T, hd=64):
+    """Rotary angles as the model computes them: fp32 freqs, fp32 t * freq (oracle/s2mel.py:_rope)."""
+    freqs = 1.0 / (10000 ** (torch.arange(0, hd, 2)[: hd // 2].float() / hd))
+    return torch.outer(torch.arange(T).float(), freqs).double().numpy()      # [T][hd/2], fp32 values
+
+
+def rope_table(T, hd=64):
+    """The (cos, sin) table the RoPE epilogue reads, [T][hd/2][2] fp32: cos / sin of the fp32 angles, rounded once."""
+    ang = rope_angles(T, hd)
+    return np.stack([np.cos(ang), np.sin(ang)], -1).astype(np.float32)
+
+
+def rope(x, hd=64):
+    """Interleaved-pair rotation of x [..., T, hd] (pairs (2i, 2i+1) by angle t * freq_i) in float64."""
+    x = np.asarray(x, np.float64)
+    ang = rope_angles(x.shape[-2], hd)
+    c, s = np.cos(ang), np.sin(ang)
+    a, b = x[..., 0::2], x[..., 1::2]
+    out = np.empty_like(x)
+    out[..., 0::2] = a * c - b * s
+    out[..., 1::2] = b * c + a * s
+    return out
+
+
+def swiglu(a, b):
+    """F.silu(a) * b in float64."""
+    a = np.asarray(a, np.float64)
+    return a / (1.0 + np.exp(-a)) * np.asarray(b, np.float64)
+
+
+def wn_gate(a, c):
+    """WaveNet fused_add_tanh_sigmoid_multiply: tanh(a) * sigmoid(c) (the conditioning g already added), float64."""
+    return np.tanh(np.asarray(a, np.float64)) / (1.0 + np.exp(-np.asarray(c, np.float64)))

@@ -1,0 +1,74 @@
+"""CPU: the float64 kernel references of tests/kernel_refs.py against PyTorch and the oracle, at small shapes."""
+import math
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+from oracle.s2mel import _rope
+from tests import kernel_refs as kr
+
+
+def test_ref_conv_matches_conv1d():
+    rng = np.random.default_rng(0)
+    B, Tin, K, N, taps, dil, pad = 2, 23, 5, 7, 3, 2, 3
+    A = rng.standard_normal((B, Tin, K))
+    w = rng.standard_normal((N, K, taps))                       # torch Conv1d weight [out][in][k]
+    wk = w.transpose(0, 2, 1).reshape(N, taps * K)              # K-major [N][taps*K]
+    M = Tin + 2 * pad - dil * (taps - 1)
+    want = F.conv1d(torch.from_numpy(A).transpose(1, 2), torch.from_numpy(w), padding=pad, dilation=dil)
+    got, mag = kr.ref_conv(A, wk, taps, dil, pad, M)
+    np.testing.assert_allclose(got, want.transpose(1, 2).numpy(), rtol=1e-12, atol=1e-12)
+    assert np.all(mag >= np.abs(got))
+    # per-batch weights and a broadcast A
+    wb = rng.standard_normal((B, N, taps * K))
+    got_b, _ = kr.ref_conv(A[:1], wb, taps, dil, pad, M)
+    for b in range(B):
+        np.testing.assert_allclose(got_b[b], kr.ref_conv(A[:1], wb[b], taps, dil, pad, M)[0][0], rtol=1e-12, atol=1e-12)
+
+
+def test_activations():
+    x = np.linspace(-9, 9, 301)
+    t = torch.from_numpy(x)
+    np.testing.assert_allclose(kr.act(x, 1), F.gelu(t).numpy(), rtol=1e-12, atol=1e-14)
+    np.testing.assert_allclose(kr.act(x, 2), F.silu(t).numpy(), rtol=1e-12, atol=1e-14)
+    np.testing.assert_allclose(kr.act(x, 3), F.mish(t).numpy(), rtol=1e-12, atol=1e-14)
+    np.testing.assert_allclose(kr.act(x, 4), F.gelu(t, approximate="tanh").numpy(), rtol=1e-12, atol=1e-14)
+    np.testing.assert_allclose(kr.act(x, 5), F.relu(t).numpy(), rtol=0, atol=0)
+
+
+def test_flash_reference_matches_sdpa():
+    rng = np.random.default_rng(1)
+    BH, T = 3, 37
+    q, k, v = (rng.standard_normal((BH, T, 64)).astype(np.float16) for _ in range(3))
+    qt, kt, vt = (torch.from_numpy(x.astype(np.float64)) for x in (q, k, v))
+    for base in (math.e, 2.0):
+        got, vmag = kr.flash_attention(q, k, v, base)
+        want = F.scaled_dot_product_attention(qt, kt, vt, scale=math.log(base))
+        np.testing.assert_allclose(got, want.numpy(), rtol=1e-10, atol=1e-12)
+        assert np.all(vmag >= np.abs(got) - 1e-12)
+
+
+def test_rope_matches_oracle():
+    rng = np.random.default_rng(2)
+    B, T, H = 2, 300, 3
+    x = rng.standard_normal((B, T, H, 64)).astype(np.float32)
+    want = _rope(torch.from_numpy(x), 64).numpy()                      # fp32, [B][T][H][64]
+    got = kr.rope(x.transpose(0, 2, 1, 3)).transpose(0, 2, 1, 3)
+    # same angles; the oracle rotates in fp32
+    assert np.abs(got - want).max() <= 4e-6 * np.abs(x).max()
+    tab = kr.rope_table(T)
+    ang = kr.rope_angles(T)
+    assert tab.shape == (T, 32, 2) and tab.dtype == np.float32
+    np.testing.assert_array_equal(tab[..., 0], np.cos(ang).astype(np.float32))
+    np.testing.assert_array_equal(tab[..., 1], np.sin(ang).astype(np.float32))
+    # the angle of pair i at position t really is fp32(t * fp32(freq_i)): the rotation of position 1 by pair 0 is 1 rad
+    assert ang[1, 0] == 1.0 and ang[0].max() == 0.0
+
+
+def test_pair_epilogue_references():
+    rng = np.random.default_rng(3)
+    a, b = rng.standard_normal((2, 50, 40)) * 4
+    np.testing.assert_allclose(kr.swiglu(a, b), (F.silu(torch.from_numpy(a)) * torch.from_numpy(b)).numpy(), rtol=1e-12, atol=1e-14)
+    ta, tc = torch.from_numpy(a), torch.from_numpy(b)
+    np.testing.assert_allclose(kr.wn_gate(a, b), (torch.tanh(ta) * torch.sigmoid(tc)).numpy(), rtol=1e-12, atol=1e-14)
