@@ -231,6 +231,18 @@ int idx_gpt_profile(idx_engine* e, int enable, int64_t* stamps_out, int n);
 /* Diagnostic (profiling enabled as above): %globaltimer stamps of EVERY CTA at the sub-phase boundaries of the middle
  * layer of the last decode step: stamps_out [num_SMs][64] (0 where a slot is unused).                          */
 int idx_gpt_profile_fine(idx_engine* e, int64_t* stamps_out, int n);
+/* Diagnostic (tests): arm an attention probe for the NEXT idx_gpt_generate call (bf16 path, num_beams = 1, one decode
+ * group: the batch-1 kernel or the 2..8-sequence kernel).  For every decode step k, probed layer l and sequence b the
+ * kernel records q as its attention reads it (fp32) and the normalised attention output before its bf16 rounding:
+ *   qo_out     [max_steps][nl][max_seqs][2][model_dim] f32, [..][0] = q, [..][1] = attention output;
+ *              nl = 1 (layer >= 0: that layer only) or layers (layer = -1); only the first max_new_tokens steps and
+ *              the first nreq sequences are written
+ *   nsplit_out [max_steps][nl] i32: the key splits per head the batch-1 kernel used at that step (0: 8-sequence kernel)
+ * Both may be host or device memory; they are written when the call returns.  The probe is disarmed by that call.   */
+int idx_gpt_probe_attention(idx_engine* e, int layer, int max_steps, int max_seqs, float* qo_out, int32_t* nsplit_out);
+/* Diagnostic (tests): the bf16 KV cache of (layer, sequence slot) at positions [pos0, pos0 + n) as f32:
+ * k_out, v_out [n][model_dim] (host or device).                                                                   */
+int idx_gpt_debug_kv(idx_engine* e, int layer, int seq, int pos0, int n, float* k_out, float* v_out);
 
 /* ------------------------------------------------------------------- BigVGAN -- */
 

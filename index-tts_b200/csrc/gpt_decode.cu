@@ -128,7 +128,18 @@ struct GptParams {
   uint2* tokt;                    // [1] tagged sampled token
   long long* prof2;     // optional: [G][64] fine globaltimer stamps of every CTA for layer prof2_layer of the last step
   int prof2_layer;
+  // attention probe of the decode kernels (idx_gpt_probe_attention), null when disarmed
+  float* probe;         // [max_new][probed layers][probe_seqs][2][D]: q as the attention reads it | normalised attention output
+  int* probe_ns;        // [max_new][probed layers]: key splits of the step (gpt_decode1_kernel)
+  int probe_layer;      // the probed layer, -1: all layers
+  int probe_seqs;
 };
+
+// Probe slot of (decode step k, layer l), or -1 when the probe is disarmed or does not record layer l
+__device__ __forceinline__ long long probe_slot(const GptParams& p, int k, int l) {
+  if (!p.probe || (p.probe_layer >= 0 && l != p.probe_layer)) return -1;
+  return p.probe_layer >= 0 ? (long long)k : (long long)k * p.L + l;
+}
 
 __device__ __forceinline__ float bf16r(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 __device__ __forceinline__ float rnd(float v, int on) { return on ? bf16r(v) : v; }
@@ -1868,6 +1879,10 @@ struct GptState {
   long long* prof = nullptr;
   long long* prof2 = nullptr;
   int prof_on = 0;
+  // attention probe armed by idx_gpt_probe_attention for the next generate call (caller buffers, host or device)
+  int probe_armed = 0, probe_layer = -1, probe_steps = 0, probe_seqs = 0;
+  float* probe_out = nullptr;
+  int32_t* probe_ns_out = nullptr;
   std::vector<void*> owned;
   double t_prefill_ms = 0, t_decode_ms = 0;
   int last_steps = 0, last_launches = 0;
@@ -2244,8 +2259,9 @@ extern "C" int idx_gpt_init(idx_engine* e, const idx_gpt_config* cfg) {
   {
     auto cdiv2 = [](int a, int b) { return (a + b - 1) / b; };
     const int mq = cdiv2(3 * D, G) + 1, mo = cdiv2(D, G) + 1, mf = cdiv2(FF, G) + 1, mh = cdiv2(V, G) + 1;
+    // G >= H: the attention phase needs at least one CTA per head
     const bool fits = mo <= TROWS && cdiv2(mq, TROWS) <= MAXIT && cdiv2(mf, TROWS) <= MAXIT && cdiv2(mh, TROWS) <= MAXIT &&
-                      FF / D <= MAXIT && G <= NCT;
+                      FF / D <= MAXIT && G <= NCT && G >= H;
     g->v2 = fits && !(getenv("IDX_GPT_V2") && atoi(getenv("IDX_GPT_V2")) == 0);
     if (g->v2) {
       int R = 0;
@@ -2638,6 +2654,15 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   // than the device samplers hold, and capping them silently would change the support of the top-p / multinomial step
   IDX_CHECK(!sp->do_sample || (sp->top_k >= 1 && sp->top_k <= CMAX), IDX_ERR_ARG,
             "do_sample needs 1 <= top_k <= 128 (the reference default is 30; top_k = 0 / larger values are not built)");
+  // an armed attention probe is consumed by this call, whatever its outcome
+  const int probe_on = g->probe_armed;
+  g->probe_armed = 0;
+  if (probe_on) {
+    const bool dec1 = nreq == 1 && g->v2, dec8 = nreq > 1 && g->v8;
+    IDX_CHECK(!g->strict && sp->num_beams == 1 && (dec1 || dec8) && nreq <= c.max_batch, IDX_ERR_ARG,
+              "the attention probe records the decode kernels gpt_decode1 / gpt_decode8 (bf16 path, num_beams = 1, one decode group)");
+    IDX_CHECK(nreq <= g->probe_seqs && sp->max_new_tokens <= g->probe_steps, IDX_ERR_ARG, "attention probe buffer too small");
+  }
   {
     // more requests than one decode group holds (max_batch rows, num_beams rows per request): run consecutive groups;
     // the sampler's sequence index stays the request's global index, so the result does not depend on the grouping
@@ -2748,6 +2773,22 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   p.seq_base = g->seq_base;
   p.pos_plain = sp->mel_pos_mode == 1;
   p.codes = d_codes; p.forced = d_forced; p.logits_dump = d_ldump;
+  struct DevBuf {
+    void* d = nullptr;
+    ~DevBuf() { if (d) cudaFree(d); }
+  } probe_q, probe_ns;
+  const int probe_nl = (g->probe_layer >= 0) ? 1 : c.layers;
+  const size_t probe_floats = (size_t)max_new * probe_nl * g->probe_seqs * 2 * D, probe_ints = (size_t)max_new * probe_nl;
+  if (probe_on) {
+    IDX_CUDA(cudaMalloc(&probe_q.d, probe_floats * sizeof(float)));
+    IDX_CUDA(cudaMalloc(&probe_ns.d, probe_ints * sizeof(int)));
+    IDX_CUDA(cudaMemsetAsync(probe_q.d, 0, probe_floats * sizeof(float), e->stream));
+    IDX_CUDA(cudaMemsetAsync(probe_ns.d, 0, probe_ints * sizeof(int), e->stream));
+    p.probe = (float*)probe_q.d;
+    p.probe_ns = (int*)probe_ns.d;
+    p.probe_layer = g->probe_layer;
+    p.probe_seqs = g->probe_seqs;
+  }
   const int SPL = (BT == 1 && g->v2) ? 64 : 32;  // steps per launch: the host looks at one flag every SPL steps
   int steps_done = 0;
   int* h_done = (int*)e->pinned_buf(64);
@@ -2775,6 +2816,10 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
     if (reqs[i].codes_out) idx_from_device(e, reqs[i].codes_out, d_codes + (size_t)i * max_new, (size_t)h_nout[i] * 4);
     if (reqs[i].logits_out)
       idx_from_device(e, reqs[i].logits_out, d_ldump + (size_t)i * max_new * V, (size_t)h_nout[i] * V * 4);
+  }
+  if (probe_on) {
+    idx_from_device(e, g->probe_out, probe_q.d, probe_floats * sizeof(float));
+    idx_from_device(e, g->probe_ns_out, probe_ns.d, probe_ints * sizeof(int));
   }
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   float ms01 = 0, ms12 = 0;
@@ -2847,6 +2892,44 @@ extern "C" int idx_gpt_profile_fine(idx_engine* e, int64_t* stamps_out, int n) {
   IDX_CUDA(cudaSetDevice(e->device));
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   IDX_CUDA(cudaMemcpy(stamps_out, e->gpt->prof2, sizeof(long long) * (size_t)std::min(n, e->gpt->G * 64), cudaMemcpyDeviceToHost));
+  IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_probe_attention(idx_engine* e, int layer, int max_steps, int max_seqs, float* qo_out, int32_t* nsplit_out) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && e->gpt && !e->gpt->strict, IDX_ERR_STATE, "idx_gpt_init (bf16 path) has not been called");
+  GptState* g = e->gpt;
+  IDX_CHECK(layer >= -1 && layer < g->cfg.layers, IDX_ERR_ARG, "layer must be -1 (all) or a layer index");
+  IDX_CHECK(max_steps >= 1 && max_seqs >= 1 && max_seqs <= 8 && qo_out && nsplit_out, IDX_ERR_ARG, "bad probe buffers");
+  g->probe_layer = layer;
+  g->probe_steps = max_steps;
+  g->probe_seqs = max_seqs;
+  g->probe_out = qo_out;
+  g->probe_ns_out = nsplit_out;
+  g->probe_armed = 1;
+  IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_debug_kv(idx_engine* e, int layer, int seq, int pos0, int n, float* k_out, float* v_out) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && e->gpt && !e->gpt->strict, IDX_ERR_STATE, "idx_gpt_init (bf16 path) has not been called");
+  GptState* g = e->gpt;
+  const idx_gpt_config& c = g->cfg;
+  IDX_CHECK(layer >= 0 && layer < c.layers && seq >= 0 && seq < c.max_batch && pos0 >= 0 && n >= 1 && pos0 + n <= g->maxpos &&
+                k_out && v_out, IDX_ERR_ARG, "bad KV-cache range");
+  IDX_CUDA(cudaSetDevice(e->device));
+  const size_t D = (size_t)c.model_dim, off = (((size_t)layer * c.max_batch + seq) * g->maxpos + pos0) * D, cnt = (size_t)n * D;
+  std::vector<uint16_t> raw(cnt);
+  std::vector<float> f(cnt);
+  for (int which = 0; which < 2; ++which) {
+    IDX_CUDA(cudaStreamSynchronize(e->stream));
+    IDX_CUDA(cudaMemcpy(raw.data(), (which ? g->vc : g->kc) + off, cnt * 2, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < cnt; ++i) {         // bf16 -> fp32 is exact: the bf16 bits are the high half of the fp32 word
+      const uint32_t u = (uint32_t)raw[i] << 16;
+      memcpy(&f[i], &u, 4);
+    }
+    IDX_CUDA(cudaMemcpy(which ? v_out : k_out, f.data(), cnt * 4, cudaMemcpyDefault));
+  }
   IDX_API_END(e)
 }
 

@@ -402,6 +402,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
     const int spin_f = ((cta * 5 + warp) % NSEG) * D + warp * (D / NCW) + (cta * 41) % (D / NCW);   // same for the gelu(fc) words (inside this warp's slices)
     const int split_at = ((p.dbg >> 16) & 0xff) ? ((p.dbg >> 16) & 0xff) * 32 : 640;     // IDX_GPT_DBG bits 16-23 / 24-30: experiment knobs
     const int split_len = ((p.dbg >> 24) & 0x7f) ? ((p.dbg >> 24) & 0x7f) * 32 : 320;
+    const int max_split = min(7, G / H);        // partt holds 7 partials per head
     const bool nowait = (p.dbg & 4) != 0;      // diagnostics only: polls do not wait (results are garbage, timing = no dependencies)
     int feed = __ldcg(p.tok + b);
     const bool already_done = __ldcg(p.finished + b) != 0;
@@ -450,8 +451,9 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
       const int posidx = (k == 0 || p.pos_plain) ? k : k + 1;   // P1: mel position k+1 with the KV cache
       const int pos = plen + k;                       // position of this token in the cache
       const int ctx = pos + 1;
-      // key splits: one CTA per head up to split_at keys, then ceil(ctx / split_len) CTAs per head (at most 7)
-      const int nsplit = (ctx <= split_at) ? 1 : min(7, (ctx + split_len - 1) / split_len);
+      // key splits: one CTA per head up to split_at keys, then ceil(ctx / split_len) CTAs per head, at most
+      // min(7, G / H): every (head, split) pair needs a CTA of the grid, or the P3 merge would wait for a partial no CTA computes
+      const int nsplit = (ctx <= split_at || max_split < 2) ? 1 : min(max_split, (ctx + split_len - 1) / split_len);
       if (step == 0) prefetch_ln(0, p.ln1_w, p.ln1_b);
       // ---- input row: mel_emb[feed] + mel_pos[posidx], built locally by every CTA (no hand-over) ----
       float v0[NPL / 8];
@@ -472,6 +474,9 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
         const unsigned f_tag = ((ep_base >> 1) % 65535u) + 1u;
         long long* f2 = (p.prof2 && l == p.prof2_layer && step == p.nsteps - 1) ? p.prof2 + (size_t)cta * 64 : nullptr;
 #define G2(i) do { if (f2 && tid == 0) { f2[(i)] = gtimer(); f2[32 + (i)] = clock64(); } } while (0)
+        const long long pslot = probe_slot(p, k, l);
+        float* const prb = (pslot >= 0) ? p.probe + pslot * p.probe_seqs * 2 * D : nullptr;   // q | attention output
+        if (prb && cta == 0 && tid == 0) p.probe_ns[pslot] = nsplit;
         G2(0);
         // ---------------- P1: LN1 -> QKV ----------------
         {
@@ -505,6 +510,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
             const int c = q0 + cl;
             if (c < D) {
               st_tagged(p.qt + c, v, ep_oproj);
+              if (prb) prb[c] = v;
             } else {
               const size_t base = (((size_t)l * p.nseq + b) * p.maxpos + pos) * D;
               const __nv_bfloat16 kvb = __float2bfloat16_rn(v);
@@ -672,6 +678,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
               // one CTA saw every key of the head: hand over the normalised output (bf16-rounded like the operand it becomes)
               const float inv = (lt > 0.f) ? 1.0f / lt : 0.f;
               st_tagged(p.ot + h * HD + tid, oa * inv, ep_oproj);
+              if (prb) prb[D + h * HD + tid] = oa * inv;
             } else {
               uint2* pw = p.partt + (size_t)cta * PART_STRIDE;
               st_tagged(pw + 2 + tid, oa, ep_oproj);
@@ -729,6 +736,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
             const float inv = (lt > 0.f) ? 1.0f / lt : 0.f;
             sm.xs[h * HD + lane] = __float2bfloat16_rn(oa * inv);
             sm.xs[h * HD + 32 + lane] = __float2bfloat16_rn(ob * inv);
+            if (prb && cta == 0) { prb[D + h * HD + lane] = oa * inv; prb[D + h * HD + 32 + lane] = ob * inv; }
           }
           G2(11);
           refill();

@@ -366,6 +366,8 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
     PROF_STAMP();
 
     for (int l = 0; l < L; ++l) {
+      const long long pslot = probe_slot(p, k, l);
+      float* const prb = (pslot >= 0) ? p.probe + pslot * p.probe_seqs * 2 * D : nullptr;   // [B][2][D]: q | attention output
       // ---------------- P1: LN1 -> QKV ----------------
       FINE8(0);
       cp_async_wait_all();
@@ -388,6 +390,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
         const int c = q0 + cl;
         if (c < D) {
           p.qg[(size_t)b * D + c] = v;
+          if (prb) prb[(size_t)b * 2 * D + c] = v;
         } else {
           const size_t base = (((size_t)l * p.nseq + b) * p.maxpos + (s_plen[b] + k)) * D;
           const __nv_bfloat16 kvb = __float2bfloat16_rn(v);
@@ -527,7 +530,9 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
             oa += base[w * PART_STRIDE + 2 + d] * c;
           }
           const int hh = 2 * (cta % (H / 2)) + hg;
-          ob[(size_t)b * D + frag_idx(hh * HD + d)] = __float2bfloat16_rn(oa * ((lt > 0.f) ? 1.0f / lt : 0.f));
+          const float o = oa * ((lt > 0.f) ? 1.0f / lt : 0.f);
+          ob[(size_t)b * D + frag_idx(hh * HD + d)] = __float2bfloat16_rn(o);
+          if (prb) prb[((size_t)b * 2 + 1) * D + hh * HD + d] = o;
         }
       }
       issue_fitting();

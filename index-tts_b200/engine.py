@@ -177,6 +177,8 @@ def load_library(path: str = None):
     lib.idx_gpt_last_timing.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
     lib.idx_gpt_profile.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
     lib.idx_gpt_profile_fine.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    lib.idx_gpt_probe_attention.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.idx_gpt_debug_kv.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.idx_v1_cond_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     lib.idx_v1_get_conditioning.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.idx_gpt_prepare_inputs_v1.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
@@ -449,6 +451,27 @@ class Engine:
         buf = np.zeros((num_sms, 64), dtype=np.int64)
         self._check(self.lib.idx_gpt_profile_fine(self.h, _ptr(buf), buf.size), "idx_gpt_profile_fine")
         return buf
+
+    def gpt_probe_attention(self, layer, max_steps, max_seqs=1):
+        """Arm the attention probe for the next gpt_generate.  Returns (qo, nsplit): qo [max_steps][nl][max_seqs][2][D]
+        float32 (q | normalised attention output of every decode step, probed layer and sequence; nl = 1 for one layer,
+        all layers for layer = -1) and nsplit [max_steps][nl] int32, filled in when that call returns."""
+        nl = 1 if layer >= 0 else self.gpt_cfg.layers
+        qo = np.zeros((max_steps, nl, max_seqs, 2, self.gpt_cfg.model_dim), dtype=np.float32)
+        ns = np.zeros((max_steps, nl), dtype=np.int32)
+        self._probe = (qo, ns)                       # the library writes them at the end of the next generate call
+        self._check(self.lib.idx_gpt_probe_attention(self.h, int(layer), int(max_steps), int(max_seqs), _ptr(qo), _ptr(ns)),
+                    "idx_gpt_probe_attention")
+        return qo, ns
+
+    def gpt_kv(self, layer, seq, pos0, n):
+        """(K, V) [n][D] float32: the bf16 KV cache of (layer, sequence slot) at positions pos0 .. pos0 + n - 1."""
+        D = self.gpt_cfg.model_dim
+        k = np.empty((n, D), dtype=np.float32)
+        v = np.empty((n, D), dtype=np.float32)
+        self._check(self.lib.idx_gpt_debug_kv(self.h, int(layer), int(seq), int(pos0), int(n), _ptr(k), _ptr(v)),
+                    "idx_gpt_debug_kv")
+        return k, v
 
     # ------------------------------------------------------------------ BigVGAN --
     @staticmethod

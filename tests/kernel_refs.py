@@ -71,6 +71,31 @@ def flash_attention(q, k, v, base):
     return out, vmag
 
 
+def ref_decode_attention(q, K, V, ctx, hd=64):
+    """Attention of GPT decode steps on the decode kernels' exact operands, in float64.  q [N][H*hd]: the query of each
+    step as the kernel read it; K, V [T][H*hd]: the cache (bf16 values); ctx [N] (or one int): step i attends to keys
+    0 .. ctx[i] - 1.  Scores q . k / sqrt(hd) (= / 8), natural-exp softmax over the keys, weighted V, per head.
+    Returns (out, vmag) float64 [N][H*hd]; vmag = sum_j p_j |v_j| / sum_j p_j, the scale of an error in the weights."""
+    q = np.atleast_2d(np.asarray(q, np.float64))
+    N, D = q.shape
+    H = D // hd
+    ctx = np.broadcast_to(np.asarray(ctx, np.int64), (N,))
+    T = int(ctx.max())
+    Kh = np.ascontiguousarray(np.asarray(K, np.float64)[:T].reshape(T, H, hd).transpose(1, 0, 2))     # [H][T][hd]
+    Vh = np.ascontiguousarray(np.asarray(V, np.float64)[:T].reshape(T, H, hd).transpose(1, 0, 2))
+    Va = np.abs(Vh)
+    out = np.empty((N, H, hd))
+    vmag = np.empty((N, H, hd))
+    for i in range(N):
+        n = int(ctx[i])
+        s = (Kh[:, :n] @ q[i].reshape(H, hd, 1))[..., 0] / math.sqrt(hd)          # [H][n]
+        p = np.exp(s - s.max(axis=1, keepdims=True))
+        l = p.sum(axis=1, keepdims=True)
+        out[i] = (p[:, None, :] @ Vh[:, :n])[:, 0] / l
+        vmag[i] = (p[:, None, :] @ Va[:, :n])[:, 0] / l
+    return out.reshape(N, D), vmag.reshape(N, D)
+
+
 def rope_angles(T, hd=64):
     """Rotary angles as the model computes them: fp32 freqs, fp32 t * freq (oracle/s2mel.py:_rope)."""
     freqs = 1.0 / (10000 ** (torch.arange(0, hd, 2)[: hd // 2].float() / hd))

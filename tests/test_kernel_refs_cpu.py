@@ -49,6 +49,26 @@ def test_flash_reference_matches_sdpa():
         assert np.all(vmag >= np.abs(got) - 1e-12)
 
 
+def test_decode_attention_reference_matches_sdpa():
+    rng = np.random.default_rng(4)
+    H, T = 3, 90
+    q = rng.standard_normal((5, H * 64)).astype(np.float32) * 2
+    K, V = (rng.standard_normal((T, H * 64)).astype(np.float32) for _ in range(2))
+    ctx = np.array([1, 2, 33, 64, T])
+    got, vmag = kr.ref_decode_attention(q, K, V, ctx)
+    for i, n in enumerate(ctx):
+        qt = torch.from_numpy(q[i].astype(np.float64)).view(H, 1, 64)
+        kt, vt = (torch.from_numpy(x[:n].astype(np.float64)).view(n, H, 64).transpose(0, 1) for x in (K, V))
+        want = F.scaled_dot_product_attention(qt, kt, vt).reshape(-1).numpy()       # default scale 1/sqrt(64)
+        np.testing.assert_allclose(got[i], want, rtol=1e-10, atol=1e-12)
+    assert np.all(vmag >= np.abs(got) - 1e-12)
+    # one key: the output is that key's value row; keys at or beyond ctx never contribute (one query, ctx as an int)
+    np.testing.assert_allclose(got[0], V[0], rtol=1e-12, atol=0)
+    K2, V2 = K.copy(), V.copy()
+    K2[64:], V2[64:] = 1e3, 1e3
+    np.testing.assert_allclose(kr.ref_decode_attention(q[3], K2, V2, 64)[0][0], got[3], rtol=1e-13, atol=1e-15)
+
+
 def test_rope_matches_oracle():
     rng = np.random.default_rng(2)
     B, T, H = 2, 300, 3
