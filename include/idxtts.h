@@ -214,7 +214,8 @@ int idx_gpt_latents_v1(idx_engine* e, const float* conds, int n_latents, const i
 /* Beam search trace of the last idx_gpt_generate call with num_beams > 1 (tests, debugging): for every step and
  * beam slot the (parent beam, token) chosen by BeamSearchScorer.process
  * (gpt/transformers_beam_search.py:215-320) and the running beam score; the score of the returned hypothesis
- * (BeamSearchScorer.finalize :322-420).
+ * (BeamSearchScorer.finalize :322-420).  Steps run after an utterance is done record the identity reorder: parent j
+ * for beam j, the stop token, the unchanged beam score.
  *   parents_tokens [max_steps][num_beams][2] i32, scores [max_steps][num_beams] f32 (either may be NULL)    */
 int idx_gpt_beam_trace(const idx_engine* e, int utterance, int32_t* parents_tokens, float* scores,
                        int max_steps, int32_t* steps_out, double* final_score);
@@ -231,15 +232,26 @@ int idx_gpt_profile(idx_engine* e, int enable, int64_t* stamps_out, int n);
 /* Diagnostic (profiling enabled as above): %globaltimer stamps of EVERY CTA at the sub-phase boundaries of the middle
  * layer of the last decode step: stamps_out [num_SMs][64] (0 where a slot is unused).                          */
 int idx_gpt_profile_fine(idx_engine* e, int64_t* stamps_out, int n);
-/* Diagnostic (tests): arm an attention probe for the NEXT idx_gpt_generate call (bf16 path, num_beams = 1, one decode
- * group: the batch-1 kernel or the 2..8-sequence kernel).  For every decode step k, probed layer l and sequence b the
- * kernel records q as its attention reads it (fp32) and the normalised attention output before its bf16 rounding:
+/* Diagnostic (tests): arm an attention probe for the NEXT idx_gpt_generate call (bf16 path, one decode group).  It
+ * records the decode kernel of that call: with num_beams = 1 the batch-1 kernel or the 2..8-sequence kernel, with
+ * num_beams > 1 the beam rows of gpt_fused_kernel (nreq * num_beams <= max_seqs, max_batch; row u * num_beams + j is
+ * beam j of request u).  For every decode step k, probed layer l and row b the kernel records q as its attention reads
+ * it (fp32) and the normalised attention output before its bf16 rounding:
  *   qo_out     [max_steps][nl][max_seqs][2][model_dim] f32, [..][0] = q, [..][1] = attention output;
  *              nl = 1 (layer >= 0: that layer only) or layers (layer = -1); only the first max_new_tokens steps and
- *              the first nreq sequences are written
- *   nsplit_out [max_steps][nl] i32: the key splits per head the batch-1 kernel used at that step (0: 8-sequence kernel)
+ *              the first nreq * num_beams rows are written (beam search: every step the call ran, pad steps included)
+ *   nsplit_out [max_steps][nl] i32: the key splits per head at that step (batch-1 kernel: by context; gpt_fused_kernel:
+ *              min(8, max(1, SMs / (rows * heads)))); 0: the 8-sequence kernel, which does not split by context
  * Both may be host or device memory; they are written when the call returns.  The probe is disarmed by that call.   */
 int idx_gpt_probe_attention(idx_engine* e, int layer, int max_steps, int max_seqs, float* qo_out, int32_t* nsplit_out);
+/* Diagnostic (tests): arm a prefill probe for the NEXT idx_gpt_generate call (bf16 path, one decode group, any
+ * num_beams).  The prompts run as tiles of 8 positions through gpt_fused_kernel; for every prompt position t of every
+ * request u and probed layer l it records q as the attention reads it (fp32) and the normalised attention output (keys
+ * 0 .. t of the request's cache slot: slot u, or u * num_beams with beams) before its bf16 rounding:
+ *   qo_out [max_seqs][max_rows][nl][2][model_dim] f32, [..][0] = q, [..][1] = attention output; nl as above;
+ *          needs nreq <= max_seqs and every prompt_len <= max_rows; rows past a prompt stay 0
+ * Host or device memory, written when the call returns.  The probe is disarmed by that call.                      */
+int idx_gpt_probe_prefill(idx_engine* e, int layer, int max_rows, int max_seqs, float* qo_out);
 /* Diagnostic (tests): the bf16 KV cache of (layer, sequence slot) at positions [pos0, pos0 + n) as f32:
  * k_out, v_out [n][model_dim] (host or device).                                                                   */
 int idx_gpt_debug_kv(idx_engine* e, int layer, int seq, int pos0, int n, float* k_out, float* v_out);

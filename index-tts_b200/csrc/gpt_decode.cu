@@ -113,7 +113,7 @@ struct GptParams {
   int pos_plain;        // 1: mel position k at step k (decoding without a cache, infer.py:101); 0: trap P1 (k + 1)
   // beam search (beam_step_kernel runs between single-step launches)
   int ext_sample;       // 1: leave the logits in p.logits and skip the sampling phase
-  int beams;            // rows per utterance
+  int beams;            // rows per utterance (also set for the beam driver's prefill launch: the prefill probe's request index)
   int phys_stride;
   const unsigned char* phys;   // [8][phys_stride]: cache slot of generated position t of row b's lineage, or null
   long long* prof;      // optional: globaltimer stamps of CTA 0 for the last step of the launch
@@ -128,17 +128,33 @@ struct GptParams {
   uint2* tokt;                    // [1] tagged sampled token
   long long* prof2;     // optional: [G][64] fine globaltimer stamps of every CTA for layer prof2_layer of the last step
   int prof2_layer;
-  // attention probe of the decode kernels (idx_gpt_probe_attention), null when disarmed
-  float* probe;         // [max_new][probed layers][probe_seqs][2][D]: q as the attention reads it | normalised attention output
-  int* probe_ns;        // [max_new][probed layers]: key splits of the step (gpt_decode1_kernel)
+  // attention probe (idx_gpt_probe_attention for decode launches, idx_gpt_probe_prefill for prefill launches), null when disarmed
+  float* probe;         // decode: [max_new][probed layers][probe_seqs][2][D]; prefill: [probe_seqs][probe_rows][probed layers][2][D]
+                        // (q as the attention reads it | normalised attention output)
+  int* probe_ns;        // decode: [max_new][probed layers]: key splits of the step
   int probe_layer;      // the probed layer, -1: all layers
   int probe_seqs;
+  int probe_rows;       // prefill: prompt positions per request
 };
 
 // Probe slot of (decode step k, layer l), or -1 when the probe is disarmed or does not record layer l
 __device__ __forceinline__ long long probe_slot(const GptParams& p, int k, int l) {
   if (!p.probe || (p.probe_layer >= 0 && l != p.probe_layer)) return -1;
   return p.probe_layer >= 0 ? (long long)k : (long long)k * p.L + l;
+}
+
+// gpt_fused_kernel: probe record ([0] = q, [1] = attention output: 2 * D floats) of row b at the first probed layer, or null.
+// Decode: row b of step k.  Prefill: prompt position `pos` of the request whose first cache slot is `seq` (beam search:
+// seq / beams).  fused_probe_at moves it to layer l (null when l is not probed).
+__device__ __forceinline__ float* fused_probe_row(const GptParams& p, int k, int b, int seq, int pos) {
+  const long long D2 = 2LL * p.D;
+  if (p.mode == 1) return p.probe + (probe_slot(p, k, max(p.probe_layer, 0)) * p.probe_seqs + b) * D2;
+  const int nl = p.probe_layer >= 0 ? 1 : p.L, req = p.beams > 1 ? seq / p.beams : seq;
+  return p.probe + ((long long)req * p.probe_rows + pos) * nl * D2;
+}
+__device__ __forceinline__ float* fused_probe_at(const GptParams& p, float* row, int l) {
+  if (p.probe_layer >= 0) return l == p.probe_layer ? row : nullptr;
+  return row + (long long)l * 2 * p.D * (p.mode == 1 ? p.probe_seqs : 1);
 }
 
 __device__ __forceinline__ float bf16r(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
@@ -525,7 +541,8 @@ __device__ __forceinline__ int col_begin(int N, int i, int G) {
   return (int)(((long long)N * i) / G);
 }
 
-template <int BT, int NPL>
+// PROBE: the instantiation launched while an attention / prefill probe is armed (the other one has no probe code at all)
+template <int BT, int NPL, bool PROBE>
 __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int D = NPL * 32, FF = 4 * D;
@@ -627,6 +644,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
     unsigned cons_idx = 0;
     unsigned bar_target = 0;
     __shared__ int row_seq[8], row_pos[8], row_valid[8], row_posidx[8];
+    __shared__ float* prb_row[8];   // PROBE: record of row b of the current step at its first probed layer, or null
     const int nsplit = min(8, max(1, G / (p.B * H)));
 
     int pi = 0;
@@ -659,6 +677,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
           row_pos[b] = (b < p.B) ? p.prompt_len[b] + k : 0;
           row_valid[b] = (b < p.B);
           row_posidx[b] = (k == 0 || p.pos_plain) ? k : k + 1;  // P1: mel position k+1 with KV cache
+        }
+        if constexpr (PROBE) {
+          // probe records of this step's rows (published to the attention phases by the barriers below)
+          prb_row[b] = (b < p.B && row_valid[b]) ? fused_probe_row(p, p.step0 + step, b, row_seq[b], row_pos[b]) : nullptr;
+          if (p.mode == 1 && cta == 0 && b == 0)
+            for (int l = 0; l < L; ++l)
+              if (probe_slot(p, p.step0 + step, l) >= 0) p.probe_ns[probe_slot(p, p.step0 + step, l)] = nsplit;
         }
       }
       ptx::named_bar_sync(1, NCT);
@@ -770,6 +795,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
               const float* qp = p.qg + (size_t)b * D + h * HD + sub * 8;
 #pragma unroll
               for (int i = 0; i < 8; ++i) qv[i] = __ldcg(qp + i);
+            }
+            if (PROBE && sp == 0 && warp == 0 && g4 == 0) {
+              float* const pr = prb_row[b];
+              if (pr) {
+                float* const pl = fused_probe_at(p, pr, l);
+                if (pl)
+#pragma unroll
+                  for (int i = 0; i < 8; ++i) pl[h * HD + sub * 8 + i] = qv[i];
+              }
             }
             // tagged mode: the position being decoded comes from the tagged words, not from the cache
             const int kend = tagged ? min(k1, ctx - 1) : k1;
@@ -968,6 +1002,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
             const float inv = (lt > 0.f) ? 1.0f / lt : 0.f;
             sm.xs[(size_t)b * FF + xs_idx(b, h * HD + lane)] = __float2bfloat16_rn(o0v * inv);
             sm.xs[(size_t)b * FF + xs_idx(b, h * HD + 32 + lane)] = __float2bfloat16_rn(o1v * inv);
+            float* const pr = PROBE ? prb_row[b] : nullptr;
+            if (PROBE && pr && cta == 0) {
+              float* const pl = fused_probe_at(p, pr, l);
+              if (pl) { pl[D + h * HD + lane] = o0v * inv; pl[D + h * HD + 32 + lane] = o1v * inv; }
+            }
           }
         }
         ptx::named_bar_sync(1, NCT);
@@ -1594,6 +1633,11 @@ __global__ void __launch_bounds__(256) beam_step_kernel(const BeamParams p) {
         p.hist_nxt[r * hs + k] = p.stop_tok;
         p.phys_nxt[r * hs + k + 1] = (unsigned char)r;
         p.tok[r] = p.stop_tok;
+        if (p.trace_pt) {           // the trace records the identity reorder too (the beam score is left as it was)
+          p.trace_pt[((size_t)k * 8 + r) * 2] = i;
+          p.trace_pt[((size_t)k * 8 + r) * 2 + 1] = p.stop_tok;
+          p.trace_sc[(size_t)k * 8 + r] = p.beam_scores[r];
+        }
       }
     }
     return;
@@ -1883,6 +1927,9 @@ struct GptState {
   int probe_armed = 0, probe_layer = -1, probe_steps = 0, probe_seqs = 0;
   float* probe_out = nullptr;
   int32_t* probe_ns_out = nullptr;
+  // prefill probe armed by idx_gpt_probe_prefill for the next generate call
+  int pprobe_armed = 0, pprobe_layer = -1, pprobe_rows = 0, pprobe_seqs = 0;
+  float* pprobe_out = nullptr;
   std::vector<void*> owned;
   double t_prefill_ms = 0, t_decode_ms = 0;
   int last_steps = 0, last_launches = 0;
@@ -2079,7 +2126,8 @@ static void launch_fused_t(idx_engine* e, GptState* g, GptParams& p) {
     g->epoch += need;
   }
   void* args[] = {(void*)&p};
-  IDX_CUDA(cudaLaunchCooperativeKernel((void*)gpt_fused_kernel<BT, NPL>, dim3(g->G), dim3(NTHREADS),
+  const void* fn = p.probe ? (const void*)gpt_fused_kernel<BT, NPL, true> : (const void*)gpt_fused_kernel<BT, NPL, false>;
+  IDX_CUDA(cudaLaunchCooperativeKernel(fn, dim3(g->G), dim3(NTHREADS),
                                        args, smem, e->stream));
   e->launches++;
   g->last_launches++;
@@ -2147,8 +2195,13 @@ static void launch_decode8(idx_engine* e, GptState* g, GptParams& p) {
 
 template <int BT>
 static void set_smem_attr(int npl, size_t bytes) {
-  if (npl == 40) IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 40>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  else IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  if (npl == 40) {
+    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 40, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 40, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  } else {
+    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  }
 }
 
 extern "C" int idx_gpt_init(idx_engine* e, const idx_gpt_config* cfg) {
@@ -2428,6 +2481,49 @@ static void fill_common(idx_engine* e, GptState* g, GptParams& p) {
   p.prof2_layer = c.layers / 2;
 }
 
+// Device buffers of the probes armed for one generate call (idx_gpt_probe_attention / idx_gpt_probe_prefill); the
+// caller's buffers are written by probe_copy_out when the call has run.
+struct ProbeBufs {
+  float* q = nullptr;     // decode records
+  int* ns = nullptr;      // decode split counts
+  float* pf = nullptr;    // prefill records
+  size_t nq = 0, nns = 0, npf = 0;
+  ~ProbeBufs() { if (q) cudaFree(q); if (ns) cudaFree(ns); if (pf) cudaFree(pf); }
+};
+
+static void probe_arm_prefill(idx_engine* e, GptState* g, GptParams& p, ProbeBufs& pb) {
+  const int nl = (g->pprobe_layer >= 0) ? 1 : g->cfg.layers;
+  pb.npf = (size_t)g->pprobe_seqs * g->pprobe_rows * nl * 2 * g->cfg.model_dim;
+  IDX_CUDA(cudaMalloc(&pb.pf, pb.npf * sizeof(float)));
+  IDX_CUDA(cudaMemsetAsync(pb.pf, 0, pb.npf * sizeof(float), e->stream));
+  p.probe = pb.pf;
+  p.probe_layer = g->pprobe_layer;
+  p.probe_seqs = g->pprobe_seqs;
+  p.probe_rows = g->pprobe_rows;
+}
+
+static void probe_arm_decode(idx_engine* e, GptState* g, GptParams& p, ProbeBufs& pb, int max_new) {
+  const int nl = (g->probe_layer >= 0) ? 1 : g->cfg.layers;
+  pb.nq = (size_t)max_new * nl * g->probe_seqs * 2 * g->cfg.model_dim;
+  pb.nns = (size_t)max_new * nl;
+  IDX_CUDA(cudaMalloc(&pb.q, pb.nq * sizeof(float)));
+  IDX_CUDA(cudaMalloc(&pb.ns, pb.nns * sizeof(int)));
+  IDX_CUDA(cudaMemsetAsync(pb.q, 0, pb.nq * sizeof(float), e->stream));
+  IDX_CUDA(cudaMemsetAsync(pb.ns, 0, pb.nns * sizeof(int), e->stream));
+  p.probe = pb.q;
+  p.probe_ns = pb.ns;
+  p.probe_layer = g->probe_layer;
+  p.probe_seqs = g->probe_seqs;
+}
+
+static void probe_copy_out(idx_engine* e, GptState* g, const ProbeBufs& pb) {
+  if (pb.q) {
+    idx_from_device(e, g->probe_out, pb.q, pb.nq * sizeof(float));
+    idx_from_device(e, g->probe_ns_out, pb.ns, pb.nns * sizeof(int));
+  }
+  if (pb.pf) idx_from_device(e, g->pprobe_out, pb.pf, pb.npf * sizeof(float));
+}
+
 // ------------------------------------------------------------------ beam-sample host driver --
 struct BeamTrace {
   int nutt = 0, m = 0, steps = 0, max_new = 0;
@@ -2438,7 +2534,8 @@ struct BeamTrace {
 
 static void beam_trace_free(GptState* g) { delete g->beam_trace; g->beam_trace = nullptr; }
 
-static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* reqs, int nreq, const idx_sampling* sp) {
+static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* reqs, int nreq, const idx_sampling* sp,
+                          bool probe_on, bool pprobe_on) {
   const idx_gpt_config& c = g->cfg;
   const int D = c.model_dim, V = c.number_mel_codes, max_new = sp->max_new_tokens, m = sp->num_beams;
   IDX_CHECK(m >= 2 && m <= BEAM_MAX, IDX_ERR_ARG, "num_beams must be 1..4");
@@ -2519,15 +2616,19 @@ static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* req
   }
 
   GptParams p;
+  ProbeBufs pb;
   fill_common(e, g, p);
   p.B = 8; p.mode = 0; p.nsteps = (int)tiles.size(); p.prompt = d_prompt; p.tiles = d_tiles;
   p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
+  p.beams = m;                                   // the prefill probe's request index is the tile's slot / m
+  if (pprobe_on) probe_arm_prefill(e, g, p, pb);
   launch_fused_bt(e, g, p, 8);
   IDX_CUDA(cudaEventRecord(g->ev1, st));
 
   fill_common(e, g, p);
   p.B = rows; p.mode = 1; p.max_new = max_new; p.ext_sample = 1; p.beams = m; p.phys_stride = hs;
   p.pos_plain = sp->mel_pos_mode == 1;
+  if (probe_on) probe_arm_decode(e, g, p, pb, max_new);
   BeamParams bp;
   memset(&bp, 0, sizeof(bp));
   bp.logits = g->logits; bp.V = V; bp.m = m; bp.max_new = max_new; bp.stop_tok = c.stop_mel_token;
@@ -2585,6 +2686,7 @@ static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* req
   IDX_CUDA(cudaMemcpyAsync(h_bs.data(), d_bscore, 32, cudaMemcpyDeviceToHost, st));
   IDX_CUDA(cudaMemcpyAsync(tr->pt.data(), d_trpt, tr->pt.size() * 4, cudaMemcpyDeviceToHost, st));
   IDX_CUDA(cudaMemcpyAsync(tr->sc.data(), d_trsc, tr->sc.size() * 4, cudaMemcpyDeviceToHost, st));
+  probe_copy_out(e, g, pb);
   IDX_CUDA(cudaStreamSynchronize(st));
   int maxn = 0;
   for (int u = 0; u < nreq; ++u) {
@@ -2655,13 +2757,21 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   IDX_CHECK(!sp->do_sample || (sp->top_k >= 1 && sp->top_k <= CMAX), IDX_ERR_ARG,
             "do_sample needs 1 <= top_k <= 128 (the reference default is 30; top_k = 0 / larger values are not built)");
   // an armed attention probe is consumed by this call, whatever its outcome
-  const int probe_on = g->probe_armed;
-  g->probe_armed = 0;
+  const int probe_on = g->probe_armed, pprobe_on = g->pprobe_armed;
+  g->probe_armed = g->pprobe_armed = 0;
+  const int rows = nreq * sp->num_beams;      // decode rows of one group
   if (probe_on) {
     const bool dec1 = nreq == 1 && g->v2, dec8 = nreq > 1 && g->v8;
-    IDX_CHECK(!g->strict && sp->num_beams == 1 && (dec1 || dec8) && nreq <= c.max_batch, IDX_ERR_ARG,
-              "the attention probe records the decode kernels gpt_decode1 / gpt_decode8 (bf16 path, num_beams = 1, one decode group)");
-    IDX_CHECK(nreq <= g->probe_seqs && sp->max_new_tokens <= g->probe_steps, IDX_ERR_ARG, "attention probe buffer too small");
+    IDX_CHECK(!g->strict && (sp->num_beams > 1 || dec1 || dec8) && rows <= c.max_batch, IDX_ERR_ARG,
+              "the attention probe records one decode group of gpt_decode1 / gpt_decode8 (num_beams = 1) or of gpt_fused_kernel "
+              "(num_beams > 1), bf16 path");
+    IDX_CHECK(rows <= g->probe_seqs && sp->max_new_tokens <= g->probe_steps, IDX_ERR_ARG, "attention probe buffer too small");
+  }
+  if (pprobe_on) {
+    IDX_CHECK(!g->strict && rows <= c.max_batch, IDX_ERR_ARG, "the prefill probe records the prefill of one decode group (bf16 path)");
+    IDX_CHECK(nreq <= g->pprobe_seqs, IDX_ERR_ARG, "prefill probe buffer too small");
+    for (int i = 0; i < nreq; ++i)
+      IDX_CHECK(reqs[i].prompt_len <= g->pprobe_rows, IDX_ERR_ARG, "prefill probe buffer too small");
   }
   {
     // more requests than one decode group holds (max_batch rows, num_beams rows per request): run consecutive groups;
@@ -2696,7 +2806,7 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
     return IDX_OK;
   }
   if (sp->num_beams > 1) {
-    beam_generate(e, g, reqs, nreq, sp);
+    beam_generate(e, g, reqs, nreq, sp, probe_on, pprobe_on);
     return IDX_OK;
   }
 
@@ -2761,6 +2871,8 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   fill_common(e, g, p);
   p.B = 8; p.mode = 0; p.nsteps = (int)tiles.size(); p.prompt = d_prompt; p.tiles = d_tiles;
   p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
+  ProbeBufs pb;
+  if (pprobe_on) probe_arm_prefill(e, g, p, pb);
   launch_fused_bt(e, g, p, 8);
   IDX_CUDA(cudaEventRecord(g->ev1, e->stream));
 
@@ -2773,22 +2885,7 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   p.seq_base = g->seq_base;
   p.pos_plain = sp->mel_pos_mode == 1;
   p.codes = d_codes; p.forced = d_forced; p.logits_dump = d_ldump;
-  struct DevBuf {
-    void* d = nullptr;
-    ~DevBuf() { if (d) cudaFree(d); }
-  } probe_q, probe_ns;
-  const int probe_nl = (g->probe_layer >= 0) ? 1 : c.layers;
-  const size_t probe_floats = (size_t)max_new * probe_nl * g->probe_seqs * 2 * D, probe_ints = (size_t)max_new * probe_nl;
-  if (probe_on) {
-    IDX_CUDA(cudaMalloc(&probe_q.d, probe_floats * sizeof(float)));
-    IDX_CUDA(cudaMalloc(&probe_ns.d, probe_ints * sizeof(int)));
-    IDX_CUDA(cudaMemsetAsync(probe_q.d, 0, probe_floats * sizeof(float), e->stream));
-    IDX_CUDA(cudaMemsetAsync(probe_ns.d, 0, probe_ints * sizeof(int), e->stream));
-    p.probe = (float*)probe_q.d;
-    p.probe_ns = (int*)probe_ns.d;
-    p.probe_layer = g->probe_layer;
-    p.probe_seqs = g->probe_seqs;
-  }
+  if (probe_on) probe_arm_decode(e, g, p, pb, max_new);
   const int SPL = (BT == 1 && g->v2) ? 64 : 32;  // steps per launch: the host looks at one flag every SPL steps
   int steps_done = 0;
   int* h_done = (int*)e->pinned_buf(64);
@@ -2817,10 +2914,7 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
     if (reqs[i].logits_out)
       idx_from_device(e, reqs[i].logits_out, d_ldump + (size_t)i * max_new * V, (size_t)h_nout[i] * V * 4);
   }
-  if (probe_on) {
-    idx_from_device(e, g->probe_out, probe_q.d, probe_floats * sizeof(float));
-    idx_from_device(e, g->probe_ns_out, probe_ns.d, probe_ints * sizeof(int));
-  }
+  probe_copy_out(e, g, pb);
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   float ms01 = 0, ms12 = 0;
   IDX_CUDA(cudaEventElapsedTime(&ms01, g->ev0, g->ev1));
@@ -2907,6 +3001,20 @@ extern "C" int idx_gpt_probe_attention(idx_engine* e, int layer, int max_steps, 
   g->probe_out = qo_out;
   g->probe_ns_out = nsplit_out;
   g->probe_armed = 1;
+  IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_probe_prefill(idx_engine* e, int layer, int max_rows, int max_seqs, float* qo_out) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && e->gpt && !e->gpt->strict, IDX_ERR_STATE, "idx_gpt_init (bf16 path) has not been called");
+  GptState* g = e->gpt;
+  IDX_CHECK(layer >= -1 && layer < g->cfg.layers, IDX_ERR_ARG, "layer must be -1 (all) or a layer index");
+  IDX_CHECK(max_rows >= 1 && max_seqs >= 1 && max_seqs <= 8 && qo_out, IDX_ERR_ARG, "bad probe buffers");
+  g->pprobe_layer = layer;
+  g->pprobe_rows = max_rows;
+  g->pprobe_seqs = max_seqs;
+  g->pprobe_out = qo_out;
+  g->pprobe_armed = 1;
   IDX_API_END(e)
 }
 

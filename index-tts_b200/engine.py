@@ -178,6 +178,7 @@ def load_library(path: str = None):
     lib.idx_gpt_profile.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
     lib.idx_gpt_profile_fine.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     lib.idx_gpt_probe_attention.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.idx_gpt_probe_prefill.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.idx_gpt_debug_kv.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.idx_v1_cond_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     lib.idx_v1_get_conditioning.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -463,6 +464,17 @@ class Engine:
         self._check(self.lib.idx_gpt_probe_attention(self.h, int(layer), int(max_steps), int(max_seqs), _ptr(qo), _ptr(ns)),
                     "idx_gpt_probe_attention")
         return qo, ns
+
+    def gpt_probe_prefill(self, layer, max_rows, max_seqs=1):
+        """Arm the prefill probe for the next gpt_generate.  Returns qo [max_seqs][max_rows][nl][2][D] float32: q | normalised
+        attention output of every prompt position of every request at each probed layer (nl = 1 for one layer, all layers
+        for layer = -1), filled in when that call returns."""
+        nl = 1 if layer >= 0 else self.gpt_cfg.layers
+        qo = np.zeros((max_seqs, max_rows, nl, 2, self.gpt_cfg.model_dim), dtype=np.float32)
+        self._pprobe = qo                            # the library writes it at the end of the next generate call
+        self._check(self.lib.idx_gpt_probe_prefill(self.h, int(layer), int(max_rows), int(max_seqs), _ptr(qo)),
+                    "idx_gpt_probe_prefill")
+        return qo
 
     def gpt_kv(self, layer, seq, pos0, n):
         """(K, V) [n][D] float32: the bf16 KV cache of (layer, sequence slot) at positions pos0 .. pos0 + n - 1."""

@@ -71,29 +71,63 @@ def flash_attention(q, k, v, base):
     return out, vmag
 
 
-def ref_decode_attention(q, K, V, ctx, hd=64):
+def ref_decode_attention(q, K, V, ctx=None, hd=64, keys=None, chunk=64):
     """Attention of GPT decode steps on the decode kernels' exact operands, in float64.  q [N][H*hd]: the query of each
     step as the kernel read it; K, V [T][H*hd]: the cache (bf16 values); ctx [N] (or one int): step i attends to keys
-    0 .. ctx[i] - 1.  Scores q . k / sqrt(hd) (= / 8), natural-exp softmax over the keys, weighted V, per head.
-    Returns (out, vmag) float64 [N][H*hd]; vmag = sum_j p_j |v_j| / sum_j p_j, the scale of an error in the weights."""
+    0 .. ctx[i] - 1.  Instead of ctx, keys [N][T] bool names the rows of K / V that step i attends to (a beam's keys
+    spread over several cache slots).  Scores q . k / sqrt(hd) (= / 8), natural-exp softmax over the keys, weighted V,
+    per head.  Returns (out, vmag) float64 [N][H*hd]; vmag = sum_j p_j |v_j| / sum_j p_j, the scale of an error in the
+    weights."""
     q = np.atleast_2d(np.asarray(q, np.float64))
     N, D = q.shape
     H = D // hd
-    ctx = np.broadcast_to(np.asarray(ctx, np.int64), (N,))
-    T = int(ctx.max())
+    if keys is None:
+        ctx = np.broadcast_to(np.asarray(ctx, np.int64), (N,))
+        keys = np.arange(int(ctx.max()))[None, :] < ctx[:, None]
+    keys = np.asarray(keys, bool)
+    T = keys.shape[1]
+    assert keys.shape[0] == N and keys.any(axis=1).all(), "every step attends to at least one key"
     Kh = np.ascontiguousarray(np.asarray(K, np.float64)[:T].reshape(T, H, hd).transpose(1, 0, 2))     # [H][T][hd]
-    Vh = np.ascontiguousarray(np.asarray(V, np.float64)[:T].reshape(T, H, hd).transpose(1, 0, 2))
-    Va = np.abs(Vh)
+    Vt = np.ascontiguousarray(np.asarray(V, np.float64)[:T].reshape(T, H, hd).transpose(1, 2, 0))     # [H][hd][T]
+    Va = np.abs(Vt)
     out = np.empty((N, H, hd))
     vmag = np.empty((N, H, hd))
-    for i in range(N):
-        n = int(ctx[i])
-        s = (Kh[:, :n] @ q[i].reshape(H, hd, 1))[..., 0] / math.sqrt(hd)          # [H][n]
+    for i0 in range(0, N, chunk):
+        i1 = min(N, i0 + chunk)
+        qc = q[i0:i1].reshape(i1 - i0, H, hd).transpose(1, 2, 0)                  # [H][hd][n]
+        s = np.where(keys[i0:i1].T[None], (Kh @ qc) / math.sqrt(hd), -np.inf)    # [H][T][n]
         p = np.exp(s - s.max(axis=1, keepdims=True))
-        l = p.sum(axis=1, keepdims=True)
-        out[i] = (p[:, None, :] @ Vh[:, :n])[:, 0] / l
-        vmag[i] = (p[:, None, :] @ Va[:, :n])[:, 0] / l
+        l = p.sum(axis=1)[:, None, :]                                             # [H][1][n]
+        out[i0:i1] = ((Vt @ p) / l).transpose(2, 0, 1)
+        vmag[i0:i1] = ((Va @ p) / l).transpose(2, 0, 1)
     return out.reshape(N, D), vmag.reshape(N, D)
+
+
+def beam_key_slots(parents, plen, m, row0):
+    """Where the keys of every beam row live in the KV cache, from the beams' traced ancestry alone (never from the
+    engine's lineage map).  parents [steps][m]: the parent beam (0 .. m-1) that beam_step_kernel chose for each beam
+    after each decode step (idx_gpt_beam_trace; a finished utterance records the identity), plen: the utterance's prompt
+    length, row0 = u * m: its first row.  Returns slots [steps][m][plen + steps] int32: at decode step k, beam row
+    row0 + r attends to key positions j = 0 .. plen + k, and position j lives in cache slot slots[k, r, j] (-1 beyond).
+
+    Row b of gpt_fused_kernel writes its keys into cache slot b (row_seq[b] = b in decode launches), so:
+      * prompt positions 0 .. plen - 1 come from slot row0 (the beam driver's prefill tiles run in the first beam's slot);
+      * generated position plen + i (i < k) comes from the slot of r's ancestor at step i: a_k = r, a_i = parents[i][a_(i+1)]
+        (phase C of beam_step_kernel copies the parent's map, phys_nxt[r][t] = phys_cur[parent][t] for t <= k, and the
+        driver starts every row's map at phys[r][0] = r);
+      * position plen + k, the one being decoded, comes from r itself (phys_nxt[r][k + 1] = r)."""
+    parents = np.asarray(parents, np.int64)
+    steps = parents.shape[0]
+    assert parents.shape == (steps, m) and ((parents >= 0) & (parents < m)).all()
+    slots = np.full((steps, m, plen + steps), -1, np.int32)
+    slots[:, :, :plen] = row0
+    for k in range(steps):
+        a = np.arange(m)                      # a_k = r for every beam r
+        slots[k, :, plen + k] = row0 + a
+        for i in range(k - 1, -1, -1):
+            a = parents[i][a]                 # a_i = parents[i][a_(i+1)]
+            slots[k, :, plen + i] = row0 + a
+    return slots
 
 
 def rope_angles(T, hd=64):

@@ -69,6 +69,48 @@ def test_decode_attention_reference_matches_sdpa():
     np.testing.assert_allclose(kr.ref_decode_attention(q[3], K2, V2, 64)[0][0], got[3], rtol=1e-13, atol=1e-15)
 
 
+def test_decode_attention_reference_key_sets():
+    """keys= (a step's keys spread over the rows of K / V) equals the same keys gathered into a contiguous cache."""
+    rng = np.random.default_rng(6)
+    H, T, N = 2, 70, 9
+    q = rng.standard_normal((N, H * 64)) * 2
+    K, V = rng.standard_normal((T, H * 64)), rng.standard_normal((T, H * 64))
+    keys = rng.random((N, T)) < 0.3
+    keys[:, 5] = True
+    got, vmag = kr.ref_decode_attention(q, K, V, keys=keys, chunk=4)
+    for i in range(N):
+        idx = np.flatnonzero(keys[i])
+        want, wmag = kr.ref_decode_attention(q[i], K[idx], V[idx], len(idx))
+        np.testing.assert_allclose(got[i], want[0], rtol=1e-12, atol=1e-13)
+        np.testing.assert_allclose(vmag[i], wmag[0], rtol=1e-12, atol=1e-13)
+
+
+def test_beam_key_slots_follow_hf_cache_reordering():
+    """beam_key_slots against HF's own bookkeeping: every beam keeps a private cache row, appends the key it computes at
+    each step, and the whole cache is reordered by the chosen parents after the step (`cache = cache[beam_idx]`).  The
+    keys are unique tags of the (cache slot, position) the engine writes them to; the helper's slots must name the
+    same tags at every (step, beam, position), including the identity reorders after an utterance is done."""
+    rng = np.random.default_rng(7)
+    for m, u, plen, steps, done_at in ((2, 0, 1, 12, None), (3, 1, 5, 40, 25), (4, 1, 3, 60, 7), (4, 0, 2, 30, 0)):
+        row0 = u * m
+        parents = rng.integers(0, m, (steps, m))
+        parents[steps // 3] = 0                         # every beam from one parent
+        parents[steps // 2] = np.arange(m)[::-1]        # a permutation
+        if done_at is not None:
+            parents[done_at:] = np.arange(m)            # finished utterance: identity reorder
+        tag = lambda slot, pos: slot * 100000 + pos     # noqa: E731
+        cache = [[tag(row0, j) for j in range(plen)] for _ in range(m)]    # HF replicates the prompt into every beam
+        slots = kr.beam_key_slots(parents, plen, m, row0)
+        assert slots.shape == (steps, m, plen + steps)
+        for k in range(steps):
+            for r in range(m):
+                cache[r].append(tag(row0 + r, plen + k))                   # the key beam r computes at step k
+                got = [tag(int(slots[k, r, j]), j) for j in range(plen + k + 1)]
+                assert got == cache[r], (m, k, r)
+                assert (slots[k, r, plen + k + 1:] == -1).all()
+            cache = [list(cache[int(b)]) for b in parents[k]]              # cache = cache[beam_idx]
+
+
 def test_rope_matches_oracle():
     rng = np.random.default_rng(2)
     B, T, H = 2, 300, 3
