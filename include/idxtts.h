@@ -350,6 +350,12 @@ int idx_debug_conv_gemm(idx_engine* e, const idx_debug_gemm* g);
 int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16, int B,
                               int T, int H, int kernel, long long guard, float* out, uint16_t* out16);
 
+/* Diagnostic (tests): the wgmma flash attention over sequences packed along T (the batched CFM solve): q16, k16, v16
+ * [B*H][T][64] as above with T = seg_off[n_seg]; sequence u owns rows [seg_off[u], seg_off[u+1]) (seg_off[0] = 0,
+ * strictly increasing) and attends to its own keys only.  out / out16 / guard as in idx_debug_flash_attention.       */
+int idx_debug_flash_attention_varlen(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16, int B,
+                                     int H, const int32_t* seg_off, int n_seg, long long guard, float* out, uint16_t* out16);
+
 /* ---------------------------------------------------------------- s2mel + codec -- */
 
 /* Geometry of the s2mel section of config.yaml as MyModel reads it
@@ -419,6 +425,17 @@ typedef struct {
 
 /* codes → codec decode → length regulator → CFM (n_steps, cfg_rate) → BigVGAN → waveform.     */
 int idx_codes_to_wav(idx_engine* e, const idx_vocode_request* r, int n_steps, float cfg_rate);
+
+/* n utterances of the per-segment tail in one call; the CFM solves of all of them run as ONE packed solve.
+ * Each request is read and written exactly as idx_codes_to_wav reads / writes it; n_steps and cfg_rate are shared.
+ * Utterance u owns rows [o_u, o_u + P_u + F_u) of the packed solve (o_u = sum of the earlier P + F); attention, the RoPE
+ * positions, the WaveNet reflect padding and the prompt-frame zeroing all stay inside each utterance's rows, so every
+ * utterance gets the result of its own idx_codes_to_wav call.  The packed solve runs in the default tail mode (gemm_backend
+ * 0, tail_f16 1, fused epilogues, the wgmma flash attention); in any other mode the requests run one at a time through
+ * idx_codes_to_wav.  Errors: n < 1, a null reqs or a bad request (the message names its index) -> IDX_ERR_ARG, and no
+ * output is written.  Afterwards idx_s2mel_last_ms reports the packed solve as the CFM time and the codec and length
+ * regulator times summed over the requests; idx_bigvgan_last_ms the summed BigVGAN time.                             */
+int idx_codes_to_wav_batch(idx_engine* e, const idx_vocode_request* reqs, int n, int n_steps, float cfg_rate);
 
 /* Device ms of the last codec decode / length regulator / CFM solve (CUDA events).       */
 int idx_s2mel_last_ms(const idx_engine* e, double* ms3);

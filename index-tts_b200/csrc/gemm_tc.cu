@@ -368,6 +368,9 @@ void launch_bn(idx_engine* e, const ConvGemm& g, const CUtensorMap& tmA, const C
 //               registers, B = V straight from its [key][dim] rows = MN-major operand);
 //   warp 8      TMA: Q tile once, then K_j / V_j tiles of 128 keys into a 2-stage ring (SWIZZLE_128B rows of 64 fp16).
 // The two warpgroups (and the two CTAs an SM holds) fill each other's softmax bubbles on the tensor cores.
+// VARLEN: several sequences packed along T (the batched CFM solve).  CTA x takes query tile tiles[x] = (first query row,
+// segment start, segment end), which lies inside one segment; its key tiles start at the segment start, so they align as in
+// a solo run of that sequence, keys at or past the segment end are masked and query rows at or past it are not stored.
 constexpr int FA_Q = 128, FA_K = 128, FA_D = 64;
 constexpr int FA_THREADS = 288;
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -379,8 +382,9 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);
   return *(uint32_t*)&h;
 }
-struct FaParams { int T, H; float* out; __half* out16; };
+struct FaParams { int T, H; float* out; __half* out16; const int4* tiles; };
 
+template <bool VARLEN>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                 const FaParams p) {
@@ -393,8 +397,10 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint64_t* bars = (uint64_t*)(base + 5 * TILE);
   uint64_t *q_full = bars, *kv_full = bars + 1, *kv_empty = bars + 3;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int bh = blockIdx.y, q0 = blockIdx.x * FA_Q;
-  const int T = p.T, ntiles = (T + FA_K - 1) / FA_K;
+  const int bh = blockIdx.y;
+  int q0 = blockIdx.x * FA_Q;
+  const int T = p.T;
+  int kbeg = 0, kend = T, ntiles = (T + FA_K - 1) / FA_K;
   if (threadIdx.x == 0) {
     ptx::mbar_init(q_full, 1);
     for (int s = 0; s < 2; ++s) { ptx::mbar_init(&kv_full[s], 1); ptx::mbar_init(&kv_empty[s], 8); }
@@ -403,6 +409,11 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   __syncthreads();
   pdl_wait();
   pdl_trigger();
+  if constexpr (VARLEN) {
+    const int4 tl = p.tiles[blockIdx.x];
+    q0 = tl.x; kbeg = tl.y; kend = tl.z;
+    ntiles = (kend - kbeg + FA_K - 1) / FA_K;
+  }
 
   if (warp == 8) {
     if (lane == 0) {
@@ -413,8 +424,8 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const int s = j & 1;
         ptx::mbar_wait(&kv_empty[s], ((j >> 1) & 1) ^ 1u);
         ptx::mbar_arrive_expect_tx(&kv_full[s], 2 * TILE);
-        ptx::tma_load_3d(sK + s * TILE, &tmK, &kv_full[s], 0, j * FA_K, bh);
-        ptx::tma_load_3d(sV + s * TILE, &tmV, &kv_full[s], 0, j * FA_K, bh);
+        ptx::tma_load_3d(sK + s * TILE, &tmK, &kv_full[s], 0, kbeg + j * FA_K, bh);
+        ptx::tma_load_3d(sV + s * TILE, &tmV, &kv_full[s], 0, kbeg + j * FA_K, bh);
       }
     }
     return;
@@ -441,8 +452,9 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_regs(S);
-    // keys beyond T (zero-filled rows of the last tile) are masked; element 4c + i is key 8c + 2 t4 + (i & 1)
-    const int nvalid = T - j * FA_K;
+    // keys beyond the sequence end (zero-filled rows past T, or the next packed sequence) are masked;
+    // element 4c + i is key 8c + 2 t4 + (i & 1)
+    const int nvalid = kend - kbeg - j * FA_K;
     if (nvalid < FA_K) {
 #pragma unroll
       for (int c = 0; c < FA_K / 8; ++c) {
@@ -509,12 +521,12 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   for (int c = 0; c < FA_D / 8; ++c) {
     const int d = 8 * c + 2 * t4;
     if (p.out16) {
-      if (t0 < T) *(uint32_t*)(p.out16 + o0 + d) = pack_half2(O[4 * c] * i0, O[4 * c + 1] * i0);
-      if (t1 < T) *(uint32_t*)(p.out16 + o1 + d) = pack_half2(O[4 * c + 2] * i1, O[4 * c + 3] * i1);
+      if (t0 < kend) *(uint32_t*)(p.out16 + o0 + d) = pack_half2(O[4 * c] * i0, O[4 * c + 1] * i0);
+      if (t1 < kend) *(uint32_t*)(p.out16 + o1 + d) = pack_half2(O[4 * c + 2] * i1, O[4 * c + 3] * i1);
     }
     if (p.out) {
-      if (t0 < T) *(float2*)(p.out + o0 + d) = make_float2(O[4 * c] * i0, O[4 * c + 1] * i0);
-      if (t1 < T) *(float2*)(p.out + o1 + d) = make_float2(O[4 * c + 2] * i1, O[4 * c + 3] * i1);
+      if (t0 < kend) *(float2*)(p.out + o0 + d) = make_float2(O[4 * c] * i0, O[4 * c + 1] * i0);
+      if (t1 < kend) *(float2*)(p.out + o1 + d) = make_float2(O[4 * c + 2] * i1, O[4 * c + 3] * i1);
     }
   }
 }
@@ -530,13 +542,31 @@ void flash_attention_wgmma(idx_engine* e, const __half* Qr, const __half* Kr, co
   cuuint32_t box[3] = {FA_D, FA_K, 1};
   CUtensorMap tq = make_map(Qr, 3, dims, str, box, true), tk = make_map(Kr, 3, dims, str, box, true), tv = make_map(Vb, 3, dims, str, box, true);
   FaParams p;
-  p.T = T; p.H = H; p.out = out; p.out16 = out16;
+  p.T = T; p.H = H; p.out = out; p.out16 = out16; p.tiles = nullptr;
   const size_t smem = 5 * (size_t)(FA_K * FA_D * 2) + 1024 + 64;
   if (!(e->attr_done & (1u << 20))) {
-    IDX_CUDA(cudaFuncSetAttribute(fa_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    IDX_CUDA(cudaFuncSetAttribute(fa_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     e->attr_done |= 1u << 20;
   }
-  launch_pdl(e, fa_wgmma_kernel, dim3((T + FA_Q - 1) / FA_Q, BH), dim3(FA_THREADS), smem, tq, tk, tv, p);
+  launch_pdl(e, fa_wgmma_kernel<false>, dim3((T + FA_Q - 1) / FA_Q, BH), dim3(FA_THREADS), smem, tq, tk, tv, p);
+  e->launches++;
+}
+
+void flash_attention_wgmma_varlen(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
+                                  int B, int H, const Segments& sg) {
+  const int BH = B * H, T = sg.total();
+  cuuint64_t dims[3] = {(cuuint64_t)FA_D, (cuuint64_t)T, (cuuint64_t)BH};
+  cuuint64_t str[2] = {(cuuint64_t)FA_D * 2, (cuuint64_t)T * FA_D * 2};
+  cuuint32_t box[3] = {FA_D, FA_K, 1};
+  CUtensorMap tq = make_map(Qr, 3, dims, str, box, true), tk = make_map(Kr, 3, dims, str, box, true), tv = make_map(Vb, 3, dims, str, box, true);
+  FaParams p;
+  p.T = T; p.H = H; p.out = out; p.out16 = out16; p.tiles = sg.d_fa_tiles;
+  const size_t smem = 5 * (size_t)(FA_K * FA_D * 2) + 1024 + 64;
+  if (!(e->attr_done & (1u << 21))) {
+    IDX_CUDA(cudaFuncSetAttribute(fa_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    e->attr_done |= 1u << 21;
+  }
+  launch_pdl(e, fa_wgmma_kernel<true>, dim3(sg.fa_tiles, BH), dim3(FA_THREADS), smem, tq, tk, tv, p);
   e->launches++;
 }
 

@@ -186,6 +186,46 @@ __global__ void reflect_pad_kernel(const float* __restrict__ x, float* __restric
   if (t >= T) t = 2 * (T - 1) - t;
   put(y, y16, ((long long)bi * Tout + i) * C + c, x[((long long)bi * T + t) * C + c]);
 }
+// segment of row r in a layout where segment u starts at row off[u] + u * gap: the largest such u with start <= r
+__device__ __forceinline__ int segment_of(const int* __restrict__ off, int n, int r, int gap) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (off[mid] + mid * gap <= r) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+__global__ void reflect_pad_seg_kernel(const float* __restrict__ x, __half* __restrict__ y16, int T, int C, int left, int gap,
+                                       int Tout, const int* __restrict__ off, int n) {
+  pdl_wait();
+  const int bi = blockIdx.z, i = blockIdx.y;
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const int u = segment_of(off, n, i, gap);
+  const int t0 = off[u], Tu = off[u + 1] - t0;
+  int t = i - t0 - u * gap - left;       // reflect_pad_kernel on the segment alone
+  if (t < 0) t = -t;
+  if (t >= Tu) t = 2 * (Tu - 1) - t;
+  y16[((long long)bi * Tout + i) * C + c] = __float2half_rn(x[((long long)bi * T + t0 + t) * C + c]);
+}
+__global__ void compact_seg_kernel(const __half* __restrict__ x, __half* __restrict__ y, int T, int Mg, int C, int gap,
+                                   const int* __restrict__ off, int n) {
+  pdl_wait();
+  const int bi = blockIdx.z, r = blockIdx.y;
+  const int c = (blockIdx.x * blockDim.x + threadIdx.x) * 8;      // 16-byte vectors (C % 8 == 0)
+  if (c >= C) return;
+  const int u = segment_of(off, n, r, 0);
+  *(uint4*)(y + ((long long)bi * T + r) * C + c) = *(const uint4*)(x + ((long long)bi * Mg + r + u * gap) * C + c);
+}
+__global__ void cfg_euler_rows_kernel(float* x, const float* vc, const float* vu, float dt, float rate, int T, int C,
+                                      const unsigned char* __restrict__ zero_rows) {
+  pdl_wait();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)T * C) return;
+  const int t = (int)(i / C);
+  const float d = (1.0f + rate) * vc[i] - rate * vu[i];      // cfg_euler_kernel, with each segment's own prompt rows
+  x[i] = zero_rows[t] ? 0.f : x[i] + dt * d;
+}
 __global__ void zero_kernel(float* x, long long n) {
   pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -665,6 +705,35 @@ void reflect_pad_rows(idx_engine* e, const float* x, float* y, int B, int T, int
   launch_pdl(e, reflect_pad_kernel, grid, dim3(128), 0, x, y, T, C, left, Tout, y16);
   LAUNCH_CHECK(e);
 }
+void reflect_pad_segments(idx_engine* e, const float* x, __half* y16, int B, int C, int left, int right, const Segments& sg) {
+  const int gap = left + right, Tout = sg.total() + sg.n() * gap;
+  dim3 grid((C + 127) / 128, Tout, B);
+  launch_pdl(e, reflect_pad_seg_kernel, grid, dim3(128), 0, x, y16, sg.total(), C, left, gap, Tout, (const int*)sg.d_off, sg.n());
+  LAUNCH_CHECK(e);
+}
+void compact_segments16(idx_engine* e, const __half* x, __half* y, int B, int C, int gap, const Segments& sg) {
+  IDX_CHECK(C % 8 == 0, IDX_ERR_ARG, "compact_segments16: C must be a multiple of 8");
+  const int T = sg.total(), Mg = T + (sg.n() - 1) * gap;
+  dim3 grid((C / 8 + 63) / 64, T, B);
+  launch_pdl(e, compact_seg_kernel, grid, dim3(64), 0, x, y, T, Mg, C, gap, (const int*)sg.d_off, sg.n());
+  LAUNCH_CHECK(e);
+}
+void cfg_euler_rows(idx_engine* e, float* x, const float* v_cond, const float* v_uncond, float dt, float rate, int T, int C,
+                    const unsigned char* zero_rows) {
+  launch_pdl(e, cfg_euler_rows_kernel, dim3((unsigned)(((long long)T * C + 255) / 256)), dim3(256), 0, x, v_cond, v_uncond, dt,
+             rate, T, C, zero_rows);
+  LAUNCH_CHECK(e);
+}
+void segments_upload(idx_engine* e, Segments& sg) {
+  std::vector<int4> tiles;
+  for (int u = 0; u < sg.n(); ++u)
+    for (int q = sg.off[u]; q < sg.off[u + 1]; q += 128) tiles.push_back(make_int4(q, sg.off[u], sg.off[u + 1], 0));
+  sg.fa_tiles = (int)tiles.size();
+  sg.d_off = e->arena.get<int>(sg.off.size());
+  sg.d_fa_tiles = e->arena.get<int4>(tiles.size());
+  idx_to_device(e, sg.d_off, sg.off.data(), sg.off.size() * sizeof(int));
+  idx_to_device(e, sg.d_fa_tiles, tiles.data(), tiles.size() * sizeof(int4));
+}
 void rope_table(idx_engine* e, float* tab, int T, int hd) {
   rope_table_kernel<<<T, 32, 0, e->stream>>>(tab, T, hd);
   LAUNCH_CHECK(e);
@@ -724,7 +793,7 @@ void attention_rope(idx_engine* e, const float* qkv, float* out, int B, int T, i
   attention_kernel<<<grid, 256, smem, e->stream>>>(qkv, out, T, H, rope, lens);
   LAUNCH_CHECK(e);
 }
-static bool fa_wgmma_on() {
+bool fa_wgmma_on() {
   static const bool on = !(getenv("IDX_FA_WGMMA") && atoi(getenv("IDX_FA_WGMMA")) == 0);
   return on;
 }

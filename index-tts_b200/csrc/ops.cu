@@ -506,3 +506,38 @@ extern "C" int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, con
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   IDX_API_END(e)
 }
+
+// Diagnostic entry (tests): the varlen wgmma flash attention on packed fp16 q / k / v [B*H][T][64] (include/idxtts.h).
+extern "C" int idx_debug_flash_attention_varlen(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16,
+                                                int B, int H, const int32_t* seg_off, int n_seg, long long guard, float* out,
+                                                uint16_t* out16) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && q16 && k16 && v16 && seg_off && (out || out16), IDX_ERR_ARG, "null argument");
+  IDX_CHECK(B > 0 && H > 0 && n_seg > 0 && seg_off[0] == 0, IDX_ERR_ARG, "idx_debug_flash_attention_varlen: bad shape");
+  Segments sg;
+  sg.off.assign(seg_off, seg_off + n_seg + 1);
+  for (int u = 0; u < n_seg; ++u)
+    IDX_CHECK(sg.off[u + 1] > sg.off[u], IDX_ERR_ARG, "idx_debug_flash_attention_varlen: segment offsets must increase");
+  IDX_CHECK(guard >= 0 && guard % 8 == 0, IDX_ERR_ARG, "idx_debug_flash_attention_varlen: guard must be a non-negative multiple of 8");
+  IDX_CUDA(cudaSetDevice(e->device));
+  const int T = sg.total();
+  const size_t n = (size_t)B * H * T * 64, ng = n + 2 * (size_t)guard;
+  e->ensure_arena(3 * 2 * n + 6 * ng + 16 * (size_t)(n_seg + T / 128 + 2) + (16 << 20));
+  e->arena.reset();
+  __half* dq = (__half*)e->arena.alloc(2 * n);
+  __half* dk = (__half*)e->arena.alloc(2 * n);
+  __half* dv = (__half*)e->arena.alloc(2 * n);
+  idx_to_device(e, dq, q16, 2 * n);
+  idx_to_device(e, dk, k16, 2 * n);
+  idx_to_device(e, dv, v16, 2 * n);
+  float* dOut = out ? e->arena.get<float>(ng) : nullptr;
+  __half* dOut16 = out16 ? (__half*)e->arena.alloc(2 * ng) : nullptr;
+  if (dOut) idx_to_device(e, dOut, out - guard, 4 * ng);
+  if (dOut16) idx_to_device(e, dOut16, out16 - guard, 2 * ng);
+  segments_upload(e, sg);
+  flash_attention_wgmma_varlen(e, dq, dk, dv, dOut ? dOut + guard : nullptr, dOut16 ? dOut16 + guard : nullptr, B, H, sg);
+  if (dOut) idx_from_device(e, out - guard, dOut, 4 * ng);
+  if (dOut16) idx_from_device(e, out16 - guard, dOut16, 2 * ng);
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  IDX_API_END(e)
+}

@@ -163,6 +163,34 @@ float flash_attention_q_scale();
 // the same on wgmma (gemm_tc.cu: S and O in registers, P fed back as a register operand)
 void flash_attention_wgmma(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
                            int B, int T, int H);
+// ------------------------------------------------------------------- packed sequences --
+// Sequences of different lengths packed along T (the batched CFM solve): segment u owns rows [off[u], off[u+1]) of every
+// batch entry.  segments_upload() puts the offsets and the query-tile list of the varlen flash attention on the device
+// (arena memory, one upload per packed solve).
+struct Segments {
+  std::vector<int> off;            // o_0 = 0 .. o_n = total rows
+  int* d_off = nullptr;            // device copy of off
+  int4* d_fa_tiles = nullptr;      // (first query row, segment start, segment end) of every 128-row query tile
+  int fa_tiles = 0;
+  int n() const { return (int)off.size() - 1; }
+  int total() const { return off.back(); }
+  int len(int u) const { return off[u + 1] - off[u]; }
+};
+void segments_upload(idx_engine* e, Segments& sg);
+// flash_attention_wgmma over packed sequences: attention never crosses a segment boundary (see fa_wgmma_kernel)
+void flash_attention_wgmma_varlen(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
+                                  int B, int H, const Segments& sg);
+// reflect_pad_rows per segment into a gapped layout: segment u's padded frame of len(u) + left + right rows starts at row
+// off[u] + u * (left + right) of each batch entry [B][total + n * (left + right)][C] (fp16 only)
+void reflect_pad_segments(idx_engine* e, const float* x, __half* y16, int B, int C, int left, int right, const Segments& sg);
+// undo the gaps: y[b][off[u] + t] = x[b][off[u] + u * gap + t], x [B][total + n * gap - gap][C] fp16 (the rows a
+// multi-tap GEMM over the gapped layout produces), y [B][total][C]
+void compact_segments16(idx_engine* e, const __half* x, __half* y, int B, int C, int gap, const Segments& sg);
+// cfg_euler with the rows listed in zero_rows (1 = prompt frame of its segment) zeroed
+void cfg_euler_rows(idx_engine* e, float* x, const float* v_cond, const float* v_uncond, float dt, float rate, int T, int C,
+                    const unsigned char* zero_rows);
+// true when the wgmma flash kernel is the default (IDX_FA_WGMMA unset or non-zero)
+bool fa_wgmma_on();
 // fp32 -> fp16 (round to nearest), n elements
 void to_half(idx_engine* e, const float* x, __half* y, long long n);
 // true when the engine runs the tail with fp16 GEMM operands (tensor-core back end and not disabled by IDX_TAIL_F16=0)

@@ -324,7 +324,19 @@ struct DitBuffers {
   __half *a16 = nullptr, *att16 = nullptr, *ffh16 = nullptr, *cat16 = nullptr, *xres16 = nullptr, *wpad16 = nullptr,
          *wacts16 = nullptr, *z16 = nullptr, *wy16 = nullptr, *qkv16 = nullptr;     // qkv16: Qr | Kr | Vb [B*H][T][64] each
   int* lens;
+  // packed solve: the utterances' segments along T, and the gapped WaveNet gate output (see dit_eval)
+  const Segments* sg = nullptr;
+  __half* wacts16g = nullptr;
 };
+
+static bool tail_fused() {      // pair epilogues (A/B switch IDX_TAIL_FUSED=0)
+  static const bool fused = !(getenv("IDX_TAIL_FUSED") && atoi(getenv("IDX_TAIL_FUSED")) == 0);
+  return fused;
+}
+static bool attn_unfused() {
+  static const bool unfused = getenv("IDX_ATTN_UNFUSED") != nullptr;
+  return unfused;
+}
 
 // one DiT evaluation for batch Bn. x_t [T][80] (shared when x_bcast), C0 [Bn][T][H] constant part
 // of the merge linear, mod/wncond/flmod: rows of the per-timestep tables. out v [Bn][T][80].
@@ -339,7 +351,7 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
     conv_gemm(e, g);
   }
   const bool hf = b.a16 != nullptr;     // fp16 GEMM operands (alloc_dit decides; see ops.h tail_half)
-  static const bool fused = !(getenv("IDX_TAIL_FUSED") && atoi(getenv("IDX_TAIL_FUSED")) == 0);   // pair epilogues (A/B switch)
+  const bool fused = tail_fused();
   auto G = [&](const PackedW& w, const float* A32, const __half* A16, int Bb, int Tt, float* out) {
     return hf ? gemm_of16(w, A16, Bb, Tt, out) : gemm_of(w, A32, Bb, Tt, out);
   };
@@ -364,7 +376,8 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
       g.scale = flash_attention_q_scale();          // 1/sqrt(64), times log2(e) when the wgmma flash kernel takes q
       conv_gemm(e, g);
       const size_t one = (size_t)Bn * nh * T * 64;
-      flash_attention_split(e, b.qkv16, b.qkv16 + one, b.qkv16 + 2 * one, nullptr, b.att16, Bn, T, nh);
+      if (b.sg) flash_attention_wgmma_varlen(e, b.qkv16, b.qkv16 + one, b.qkv16 + 2 * one, nullptr, b.att16, Bn, nh, *b.sg);
+      else flash_attention_split(e, b.qkv16, b.qkv16 + one, b.qkv16 + 2 * one, nullptr, b.att16, Bn, T, nh);
     } else {
       conv_gemm(e, G(s->wqkv[l], b.a, b.a16, Bn, T, b.qkv));
       attention_rope(e, b.qkv, hf ? nullptr : b.att, Bn, T, nh, b.rope, b.lens, b.att16);
@@ -410,16 +423,29 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
     // SConv1d pad_mode='reflect' (encodec.py:196-229): materialise the reflected halo rows so the
     // conv is a plain zero-pad-free multi-tap GEMM (tensor-core path; TMA cannot reflect)
     const int kk = s->wn_in[i].taps, pl = (kk - 1) - (kk - 1) / 2, pr = (kk - 1) / 2;
-    reflect_pad_rows(e, b.wy, hf ? nullptr : b.wpad, Bn, T, WH, pl, pr, b.wpad16);
-    ConvGemm gi = G(s->wn_in[i], b.wpad, b.wpad16, Bn, T + kk - 1, b.wxin);
-    gi.pad = 0; gi.M = T;
-    if (hf && fused) {        // the gate in the epilogue (tanh / sigmoid halves interleaved): fp16 acts, no [T][2 WH] round trip
-      gi.Wk16 = s->wn_in_i16[i]; gi.bias = s->wn_in_bias_i[i]; gi.out = nullptr;
-      gi.epi = EPI_WNGATE; gi.out16 = b.wacts16; gi.aux = wncond + (size_t)i * 2 * WH; gi.aux_stride = 0;
+    if (b.sg) {
+      // packed: each segment gets its own reflected frame (kk - 1 rows more than the segment, so no tap reaches another
+      // utterance); the conv runs once over the gapped frames and the gate output is compacted back to the packed rows
+      const int gap = kk - 1, ng = b.sg->n();
+      reflect_pad_segments(e, b.wy, b.wpad16, Bn, WH, pl, pr, *b.sg);
+      ConvGemm gi = gemm_of16(s->wn_in[i], b.wpad16, Bn, T + ng * gap, nullptr);
+      gi.pad = 0; gi.M = T + (ng - 1) * gap;
+      gi.Wk16 = s->wn_in_i16[i]; gi.bias = s->wn_in_bias_i[i];
+      gi.epi = EPI_WNGATE; gi.out16 = b.wacts16g; gi.aux = wncond + (size_t)i * 2 * WH; gi.aux_stride = 0;
       conv_gemm(e, gi);
+      compact_segments16(e, b.wacts16g, b.wacts16, Bn, WH, gap, *b.sg);
     } else {
-      conv_gemm(e, gi);
-      wn_gate(e, b.wxin, wncond + (size_t)i * 2 * WH, 0, hf ? nullptr : b.wacts, Bn, T, WH, b.wacts16);
+      reflect_pad_rows(e, b.wy, hf ? nullptr : b.wpad, Bn, T, WH, pl, pr, b.wpad16);
+      ConvGemm gi = G(s->wn_in[i], b.wpad, b.wpad16, Bn, T + kk - 1, b.wxin);
+      gi.pad = 0; gi.M = T;
+      if (hf && fused) {        // the gate in the epilogue (tanh / sigmoid halves interleaved): fp16 acts, no [T][2 WH] round trip
+        gi.Wk16 = s->wn_in_i16[i]; gi.bias = s->wn_in_bias_i[i]; gi.out = nullptr;
+        gi.epi = EPI_WNGATE; gi.out16 = b.wacts16; gi.aux = wncond + (size_t)i * 2 * WH; gi.aux_stride = 0;
+        conv_gemm(e, gi);
+      } else {
+        conv_gemm(e, gi);
+        wn_gate(e, b.wxin, wncond + (size_t)i * 2 * WH, 0, hf ? nullptr : b.wacts, Bn, T, WH, b.wacts16);
+      }
     }
     if (i < NL - 1) {
       ConvGemm gr = G(s->wn_res[i], b.wacts, b.wacts16, Bn, T, b.wy);
@@ -442,7 +468,8 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
   conv_gemm(e, G(s->conv2, b.wy, b.wy16, Bn, T, b.v));
 }
 
-static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T) {
+// sg (packed solve, fp16 fused mode only): RoPE positions restart at every segment, room for the per-segment WaveNet frames
+static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T, const Segments* sg = nullptr) {
   const idx_s2mel_config& c = s->cfg;
   const int H = c.hidden, WH = c.wn_hidden, C = c.in_channels;
   const size_t bt = (size_t)Bn * T;
@@ -454,7 +481,8 @@ static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T
   b.cat = e->arena.get<float>(bt * 2 * H);
   b.xres = e->arena.get<float>(bt * H);
   b.wy = e->arena.get<float>(bt * WH);
-  b.wpad = e->arena.get<float>((size_t)Bn * (T + 8) * WH);
+  const size_t padT = (size_t)T + 8 * (sg ? sg->n() : 1);
+  b.wpad = e->arena.get<float>((size_t)Bn * padT * WH);
   b.wxin = e->arena.get<float>(bt * 2 * WH);
   b.wacts = e->arena.get<float>(bt * WH);
   b.wout = e->arena.get<float>(bt * WH);
@@ -462,15 +490,21 @@ static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T
   b.v = e->arena.get<float>(bt * C);
   b.rope = e->arena.get<float>((size_t)T * 64);
   b.lens = nullptr;
-  static const bool unfused = getenv("IDX_ATTN_UNFUSED") != nullptr;
-  if (tail_half(e) && !unfused && H % 8 == 0 && WH % 8 == 0 && (H + C) % 8 == 0 && s->inter % 8 == 0) {
+  if (tail_half(e) && !attn_unfused() && H % 8 == 0 && WH % 8 == 0 && (H + C) % 8 == 0 && s->inter % 8 == 0) {
     auto hb = [&](size_t n) { return (__half*)e->arena.alloc(n * sizeof(__half) + 16); };
     b.a16 = hb(bt * H); b.att16 = hb(bt * H); b.ffh16 = hb(bt * s->inter); b.cat16 = hb(bt * 2 * H);
-    b.xres16 = hb(bt * H); b.wpad16 = hb((size_t)Bn * (T + 8) * WH); b.wacts16 = hb(bt * WH); b.z16 = hb(bt * WH);
+    b.xres16 = hb(bt * H); b.wpad16 = hb((size_t)Bn * padT * WH); b.wacts16 = hb(bt * WH); b.z16 = hb(bt * WH);
     b.wy16 = hb(bt * WH);
     b.qkv16 = hb(3 * bt * H);
   }
-  rope_table(e, b.rope, T, 64);
+  b.sg = sg;
+  if (sg) {
+    IDX_CHECK(b.a16 && tail_fused() && fa_wgmma_on(), IDX_ERR_STATE, "packed solve outside the fp16 fused tail mode");
+    b.wacts16g = (__half*)e->arena.alloc((size_t)Bn * padT * WH * sizeof(__half) + 16);
+    for (int u = 0; u < sg->n(); ++u) rope_table(e, b.rope + (size_t)sg->off[u] * 64, sg->len(u), 64);
+  } else {
+    rope_table(e, b.rope, T, 64);
+  }
 }
 static size_t dit_arena_bytes(const S2melState* s, int Bn, int T) {
   const idx_s2mel_config& c = s->cfg;
@@ -480,6 +514,15 @@ static size_t dit_arena_bytes(const S2melState* s, int Bn, int T) {
   const size_t half_bytes = 2 * (bt * c.hidden * 8 + bt * s->inter + bt * c.wn_hidden * 4 + (size_t)Bn * 8 * c.wn_hidden) + 16 * 512;
   return attn + half_bytes + 4 * (bt * c.hidden * (12 + 1 + 3 + 1 + 2 + 1) + bt * 3 * s->inter + bt * c.wn_hidden * 7 + (size_t)Bn * 8 * c.wn_hidden + bt * c.in_channels +
               (size_t)T * 64) + 64 * 256;
+}
+
+// the packed solve never takes the T x T attention scratch of dit_arena_bytes: linear in the packed length
+static size_t dit_arena_bytes_packed(const S2melState* s, int Bn, int T, int nseg) {
+  const idx_s2mel_config& c = s->cfg;
+  const size_t bt = (size_t)Bn * T, pad = (size_t)Bn * (T + 8 * (size_t)nseg) * c.wn_hidden;
+  const size_t half_bytes = 2 * (bt * c.hidden * 8 + bt * s->inter + bt * c.wn_hidden * 3 + 2 * pad) + 16 * 512;
+  return half_bytes + 4 * (bt * c.hidden * 20 + bt * 3 * s->inter + bt * c.wn_hidden * 6 + pad + bt * c.in_channels +
+                           (size_t)T * 64) + 64 * 256;
 }
 
 // timestep tables for a list of nt timesteps (device float [nt])
@@ -512,8 +555,10 @@ static TimeTables time_tables(idx_engine* e, S2melState* s, const float* d_t, in
 }
 
 // C0[b] = [prompt_x | cond_projection(mu_b) | style_b] · W_rest^T + bias   for b in {cond, uncond}
+// packed (sg): d_style is [Bn][n][style], one style per segment
 static float* merge_const(idx_engine* e, S2melState* s, int Bn, int T, const float* d_prompt_x /*[Bn][T][80]*/,
-                          const float* d_mu /*[Bn][T][content]*/, const float* d_style /*[Bn][style]*/) {
+                          const float* d_mu /*[Bn][T][content]*/, const float* d_style /*[Bn][style]*/,
+                          const Segments* sg = nullptr) {
   const idx_s2mel_config& c = s->cfg;
   const int H = c.hidden, C = c.in_channels, Sd = c.style_dim;
   const int Kr = C + H + Sd;
@@ -523,7 +568,14 @@ static float* merge_const(idx_engine* e, S2melState* s, int Bn, int T, const flo
   conv_gemm(e, gemm_of(s->cond_proj, d_mu, Bn, T, cp));
   copy_cols(e, d_prompt_x, C, rest, Kr, 0, (long long)Bn * T, C);
   copy_cols(e, cp, H, rest, Kr, C, (long long)Bn * T, H);
-  bcast_cols(e, d_style, rest, Kr, C + H, Bn, T, Sd);
+  if (!sg) {
+    bcast_cols(e, d_style, rest, Kr, C + H, Bn, T, Sd);
+  } else {
+    for (int bi = 0; bi < Bn; ++bi)
+      for (int u = 0; u < sg->n(); ++u)
+        bcast_cols(e, d_style + ((size_t)bi * sg->n() + u) * Sd, rest + ((size_t)bi * T + sg->off[u]) * Kr, Kr, C + H, 1,
+                   sg->len(u), Sd);
+  }
   conv_gemm(e, gemm_of(s->merge_rest, rest, Bn, T, C0));
   return C0;
 }
@@ -586,6 +638,40 @@ void cfm_solve_dev(idx_engine* e, S2melState* s, const float* d_mu, int T, const
   }
   transpose_btc_to_bct(e, x, d_mel, 1, T, C);
   (void)H;
+}
+
+// The CFM solves of several utterances as ONE solve over their frames packed along T (sg; see include/idxtts.h
+// idx_codes_to_wav_batch).  x [T][80] holds every z with its prompt frames zeroed, px / mu2 [2][T][*] the cond | uncond
+// inputs, st [2][n][style], zero_rows [T] marks each segment's prompt frames.  x is updated in place to the mel.
+void cfm_solve_packed_dev(idx_engine* e, S2melState* s, const Segments& sg, float* x, const float* px, const float* mu2,
+                          const float* st, const unsigned char* zero_rows, int n_steps, float rate) {
+  const idx_s2mel_config& c = s->cfg;
+  const int C = c.in_channels, T = sg.total(), Bn = 2;
+  std::vector<float> ts, dts;
+  euler_times(n_steps, ts, dts);
+  float* d_t = e->arena.get<float>(n_steps);
+  IDX_CUDA(cudaMemcpyAsync(d_t, ts.data(), (size_t)n_steps * 4, cudaMemcpyHostToDevice, e->stream));
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  TimeTables tt = time_tables(e, s, d_t, n_steps);
+  float* C0 = merge_const(e, s, Bn, T, px, mu2, st, &sg);
+  DitBuffers b;
+  alloc_dit(e, s, b, Bn, T, &sg);
+  for (int k = 0; k < n_steps; ++k) {
+    dit_eval(e, s, b, Bn, T, x, 1, C0, tt.mod + (size_t)k * s->mod_width,
+             tt.wncond + (size_t)k * 2 * c.wn_hidden * c.wn_layers, tt.flmod + (size_t)k * 2 * c.wn_hidden);
+    cfg_euler_rows(e, x, b.v, b.v + (size_t)T * C, dts[k], rate, T, C, zero_rows);
+  }
+}
+size_t cfm_packed_arena_bytes(const S2melState* s, int T, int nseg, int n_steps) {
+  const idx_s2mel_config& c = s->cfg;
+  return dit_arena_bytes_packed(s, 2, T, nseg) + 4 * (size_t)T * (8 * c.in_channels + 3 * c.content_dim + 6 * c.hidden + 2 * c.style_dim) +
+         4 * (size_t)n_steps * (s->mod_width + 2 * c.wn_hidden * (c.wn_layers + 1) + 6 * c.hidden + 512) +
+         16 * (size_t)nseg * 256 + (4 << 20);
+}
+bool cfm_packed_supported(const idx_engine* e, const S2melState* s) {
+  const idx_s2mel_config& c = s->cfg;
+  return tail_half(e) && tail_fused() && !attn_unfused() && fa_wgmma_on() && getenv("IDX_NO_TC") == nullptr &&
+         c.hidden % 8 == 0 && c.wn_hidden % 8 == 0 && (c.hidden + c.in_channels) % 8 == 0 && s->inter % 8 == 0;
 }
 
 size_t codec_arena_bytes(const S2melState* s, int n) {

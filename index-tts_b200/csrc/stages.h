@@ -13,6 +13,11 @@ void length_regulate_dev(idx_engine* e, S2melState* s, const float* d_S, int n_i
 size_t cfm_arena_bytes(const S2melState* s, int T, int n_steps);
 void cfm_solve_dev(idx_engine* e, S2melState* s, const float* d_mu, int T, const float* d_prompt, int P,
                    const float* d_style, const float* d_z, int n_steps, float rate, float* d_mel);
+// several utterances' solves as one solve over their frames packed along T (s2mel.cu)
+bool cfm_packed_supported(const idx_engine* e, const S2melState* s);
+size_t cfm_packed_arena_bytes(const S2melState* s, int T, int nseg, int n_steps);
+void cfm_solve_packed_dev(idx_engine* e, S2melState* s, const Segments& sg, float* x, const float* px, const float* mu2,
+                          const float* st, const unsigned char* zero_rows, int n_steps, float rate);
 int s2mel_content_dim(const S2melState* s);
 int s2mel_style_dim(const S2melState* s);
 int s2mel_codec_hidden(const S2melState* s);

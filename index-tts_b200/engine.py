@@ -196,6 +196,8 @@ def load_library(path: str = None):
     lib.idx_debug_conv_gemm.argtypes = [C.c_void_p, C.POINTER(DebugGemm)]
     lib.idx_debug_flash_attention.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                               C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]
+    lib.idx_debug_flash_attention_varlen.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                     C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]
     lib.idx_s2mel_init.argtypes = [C.c_void_p, C.POINTER(S2melConfig)]
     lib.idx_codec_init.argtypes = [C.c_void_p, C.POINTER(CodecConfig)]
     lib.idx_codec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -207,6 +209,7 @@ def load_library(path: str = None):
     lib.idx_emo_init.argtypes = [C.c_void_p, C.POINTER(EmoConfig)]
     lib.idx_merge_emovec.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_void_p]
     lib.idx_codes_to_wav.argtypes = [C.c_void_p, C.POINTER(VocodeRequest), C.c_int, C.c_float]
+    lib.idx_codes_to_wav_batch.argtypes = [C.c_void_p, C.POINTER(VocodeRequest), C.c_int, C.c_int, C.c_float]
     _lib = lib
     return lib
 
@@ -629,6 +632,28 @@ class Engine:
                      want_wav=True, want_pcm16=False, want_mel=False, out=None):
         """infer_v2_5.py:827-856 for one segment.  Host or device (torch.cuda) buffers.
         Returns dict(wav=[F*256] f32, pcm16=..., mel=[80,F])."""
+        r, res, _ = self._vocode_request(codes, prompt_condition, ref_mel, style, z, F, want_wav, want_pcm16, want_mel)
+        self._check(self.lib.idx_codes_to_wav(self.h, C.byref(r), int(n_steps), float(cfg_rate)), "idx_codes_to_wav")
+        return res
+
+    def codes_to_wav_batch(self, requests, n_steps=25, cfg_rate=0.7, want_wav=True, want_pcm16=False, want_mel=False):
+        """codes_to_wav for several segments in one call (include/idxtts.h idx_codes_to_wav_batch): their CFM solves run as
+        one solve over the frames of all of them.  requests: list of dicts with the codes_to_wav arguments (codes,
+        prompt_condition, ref_mel, style, z, F).  Returns one result dict per request, as codes_to_wav returns it."""
+        reqs = (VocodeRequest * max(1, len(requests)))()
+        results, keep = [], []
+        for i, q in enumerate(requests):
+            r, res, k = self._vocode_request(q["codes"], q["prompt_condition"], q["ref_mel"], q["style"], q["z"], q["F"],
+                                             want_wav, want_pcm16, want_mel)
+            reqs[i] = r
+            results.append(res)
+            keep.append(k)
+        self._check(self.lib.idx_codes_to_wav_batch(self.h, reqs, len(requests), int(n_steps), float(cfg_rate)),
+                    "idx_codes_to_wav_batch")
+        return results
+
+    def _vocode_request(self, codes, prompt_condition, ref_mel, style, z, F, want_wav, want_pcm16, want_mel):
+        """(VocodeRequest, result dict, the arrays its pointers refer to) of one segment."""
         on_dev = torch is not None and isinstance(z, torch.Tensor) and z.is_cuda
         if on_dev and isinstance(codes, torch.Tensor):
             codes_t = codes.to(torch.int32).contiguous()
@@ -651,8 +676,7 @@ class Engine:
             res["mel"] = mk((80, F), np.float32, torch.float32 if torch else None)
         r = VocodeRequest(_ptr(codes_t), int(codes_t.shape[0]), _ptr(pc), _ptr(rm), P, _ptr(st), _ptr(zz), int(F),
                           _ptr(res.get("wav")), _ptr(res.get("pcm16")), _ptr(res.get("mel")))
-        self._check(self.lib.idx_codes_to_wav(self.h, C.byref(r), int(n_steps), float(cfg_rate)), "idx_codes_to_wav")
-        return res
+        return r, res, (codes_t, pc, rm, st, zz)
 
     # --------------------------------------------------------------- diagnostics --
     def debug_conv_gemm(self, A, wk, taps=1, dil=1, pad=0, M=None, bias=None, act=0, res=None, accum=False,
@@ -739,6 +763,31 @@ class Engine:
                 res.append(None)
                 continue
             _check_guard(buf, guard, n, "idx_debug_flash_attention")
+            dt = np.float32 if buf.dtype == np.uint32 else np.float16
+            res.append(buf[guard:guard + n].view(dt).reshape(B, T, H * 64).copy())
+        return tuple(res)
+
+    def debug_flash_attention_varlen(self, q16, k16, v16, B, H, seg_off, out=True, out16=True):
+        """The wgmma flash attention over sequences packed along T (include/idxtts.h idx_debug_flash_attention_varlen):
+        q (already scaled by log2(e)/8), k, v [B*H][T][64] fp16, sequence u = rows seg_off[u] .. seg_off[u+1] - 1.
+        Returns (out [B][T][H*64] f32 or None, out16 fp16 or None); raises AssertionError when the kernel wrote outside them."""
+        q16, k16, v16 = (np.ascontiguousarray(x, dtype=np.float16) for x in (q16, k16, v16))
+        so = np.ascontiguousarray(np.asarray(seg_off, dtype=np.int32))
+        BH, T, D = q16.shape
+        assert D == 64 and BH == B * H and k16.shape == q16.shape and v16.shape == q16.shape and int(so[-1]) == T
+        n, guard = B * T * H * 64, _guard_len(H * 64)
+        b32 = _guarded(n, guard, np.float32) if out else None
+        b16 = _guarded(n, guard, np.float16) if out16 else None
+        self._check(self.lib.idx_debug_flash_attention_varlen(
+            self.h, _ptr(q16), _ptr(k16), _ptr(v16), B, H, _ptr(so), len(so) - 1, guard,
+            None if b32 is None else b32.ctypes.data + 4 * guard, None if b16 is None else b16.ctypes.data + 2 * guard),
+            "idx_debug_flash_attention_varlen")
+        res = []
+        for buf in (b32, b16):
+            if buf is None:
+                res.append(None)
+                continue
+            _check_guard(buf, guard, n, "idx_debug_flash_attention_varlen")
             dt = np.float32 if buf.dtype == np.uint32 else np.float16
             res.append(buf[guard:guard + n].view(dt).reshape(B, T, H * 64).copy())
         return tuple(res)
