@@ -423,7 +423,9 @@ typedef struct {
   float* mel_out;                 /* optional [80, F] generated mel (tests)                           */
 } idx_vocode_request;
 
-/* codes → codec decode → length regulator → CFM (n_steps, cfg_rate) → BigVGAN → waveform.     */
+/* codes → codec decode → length regulator → CFM (n_steps, cfg_rate) → BigVGAN → waveform.  The one-request case of
+ * idx_codes_to_wav_batch.  Errors: a bad request, cfg_rate <= 0 -> IDX_ERR_ARG before any work; a code outside the
+ * codebook -> IDX_ERR_ARG after the tail has run.  In both cases no output is written.                              */
 int idx_codes_to_wav(idx_engine* e, const idx_vocode_request* r, int n_steps, float cfg_rate);
 
 /* n utterances of the per-segment tail in one call; the CFM solves of all of them run as ONE packed solve.
@@ -431,9 +433,9 @@ int idx_codes_to_wav(idx_engine* e, const idx_vocode_request* r, int n_steps, fl
  * Utterance u owns rows [o_u, o_u + P_u + F_u) of the packed solve (o_u = sum of the earlier P + F); attention, the RoPE
  * positions, the WaveNet reflect padding and the prompt-frame zeroing all stay inside each utterance's rows, so every
  * utterance gets the result of its own idx_codes_to_wav call.  The packed solve runs in the default tail mode (gemm_backend
- * 0, tail_f16 1, fused epilogues, the wgmma flash attention); in any other mode the requests run one at a time through
- * idx_codes_to_wav.  Errors: n < 1, a null reqs or a bad request (the message names its index) -> IDX_ERR_ARG, and no
- * output is written.  Afterwards idx_s2mel_last_ms reports the packed solve as the CFM time and the codec and length
+ * 0, tail_f16 1, fused epilogues, the wgmma flash attention); in any other mode each request gets a solve of its own,
+ * in the same call.  Errors: n < 1, a null reqs or a bad request (the message names its index) -> IDX_ERR_ARG, and no
+ * output is written.  Afterwards idx_s2mel_last_ms reports the solves as the CFM time and the codec and length
  * regulator times summed over the requests; idx_bigvgan_last_ms the summed BigVGAN time.                             */
 int idx_codes_to_wav_batch(idx_engine* e, const idx_vocode_request* reqs, int n, int n_steps, float cfg_rate);
 

@@ -17,6 +17,7 @@
 //     into a per-solve constant C0, so each step starts with a K = 80 GEMM;
 //   * the cond / uncond CFG pair runs as batch 2 exactly like the reference (flow_matching.py:88-104).
 #include "stages.h"
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 
@@ -324,7 +325,8 @@ struct DitBuffers {
   __half *a16 = nullptr, *att16 = nullptr, *ffh16 = nullptr, *cat16 = nullptr, *xres16 = nullptr, *wpad16 = nullptr,
          *wacts16 = nullptr, *z16 = nullptr, *wy16 = nullptr, *qkv16 = nullptr;     // qkv16: Qr | Kr | Vb [B*H][T][64] each
   int* lens;
-  // packed solve: the utterances' segments along T, and the gapped WaveNet gate output (see dit_eval)
+  // packed solve (two or more segments; null otherwise): the utterances' segments along T, and the gapped WaveNet gate
+  // output (see dit_eval)
   const Segments* sg = nullptr;
   __half* wacts16g = nullptr;
 };
@@ -468,11 +470,13 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
   conv_gemm(e, G(s->conv2, b.wy, b.wy16, Bn, T, b.v));
 }
 
-// sg (packed solve, fp16 fused mode only): RoPE positions restart at every segment, room for the per-segment WaveNet frames
+// sg with more than one segment (packed solve, fp16 fused mode only): RoPE positions restart at every segment, room for the
+// per-segment WaveNet frames.  One segment (or none) is the single-sequence layout.
 static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T, const Segments* sg = nullptr) {
   const idx_s2mel_config& c = s->cfg;
   const int H = c.hidden, WH = c.wn_hidden, C = c.in_channels;
   const size_t bt = (size_t)Bn * T;
+  if (sg && sg->n() == 1) sg = nullptr;
   for (int i = 0; i < 12; ++i) b.h[i] = e->arena.get<float>(bt * H);
   b.a = e->arena.get<float>(bt * H);
   b.qkv = e->arena.get<float>(bt * (size_t)std::max(3 * H, s->inter));
@@ -506,23 +510,16 @@ static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T
     rope_table(e, b.rope, T, 64);
   }
 }
-static size_t dit_arena_bytes(const S2melState* s, int Bn, int T) {
-  const idx_s2mel_config& c = s->cfg;
-  const size_t bt = (size_t)Bn * T;
-  const size_t Tp = (size_t)((T + 3) & ~3);
-  const size_t attn = 4 * (size_t)Bn * c.heads * (3 * (size_t)T * 64 + 64 * Tp + (size_t)T * Tp) + 8 * 256;
-  const size_t half_bytes = 2 * (bt * c.hidden * 8 + bt * s->inter + bt * c.wn_hidden * 4 + (size_t)Bn * 8 * c.wn_hidden) + 16 * 512;
-  return attn + half_bytes + 4 * (bt * c.hidden * (12 + 1 + 3 + 1 + 2 + 1) + bt * 3 * s->inter + bt * c.wn_hidden * 7 + (size_t)Bn * 8 * c.wn_hidden + bt * c.in_channels +
-              (size_t)T * 64) + 64 * 256;
-}
-
-// the packed solve never takes the T x T attention scratch of dit_arena_bytes: linear in the packed length
-static size_t dit_arena_bytes_packed(const S2melState* s, int Bn, int T, int nseg) {
+// alloc_dit over nseg segments, plus the scratch attention_rope takes when the solve is not packed (the T x T scores only
+// on the unfused path): a packed solve is linear in its length
+static size_t dit_arena_bytes(const S2melState* s, int Bn, int T, int nseg) {
   const idx_s2mel_config& c = s->cfg;
   const size_t bt = (size_t)Bn * T, pad = (size_t)Bn * (T + 8 * (size_t)nseg) * c.wn_hidden;
-  const size_t half_bytes = 2 * (bt * c.hidden * 8 + bt * s->inter + bt * c.wn_hidden * 3 + 2 * pad) + 16 * 512;
-  return half_bytes + 4 * (bt * c.hidden * 20 + bt * 3 * s->inter + bt * c.wn_hidden * 6 + pad + bt * c.in_channels +
-                           (size_t)T * 64) + 64 * 256;
+  const size_t Tp = (size_t)((T + 3) & ~3);
+  const size_t attn = nseg > 1 ? 0 : 4 * (size_t)Bn * c.heads * (3 * (size_t)T * 64 + 64 * Tp + (attn_unfused() ? (size_t)T * Tp : 0)) + 8 * 256;
+  const size_t half_bytes = 2 * (bt * c.hidden * 8 + bt * s->inter + bt * c.wn_hidden * 3 + (nseg > 1 ? 2 : 1) * pad) + 16 * 512;
+  return attn + half_bytes + 4 * (bt * c.hidden * 20 + bt * 3 * s->inter + bt * c.wn_hidden * 6 + pad + bt * c.in_channels +
+                                  (size_t)T * 64) + 64 * 256;
 }
 
 // timestep tables for a list of nt timesteps (device float [nt])
@@ -555,7 +552,7 @@ static TimeTables time_tables(idx_engine* e, S2melState* s, const float* d_t, in
 }
 
 // C0[b] = [prompt_x | cond_projection(mu_b) | style_b] · W_rest^T + bias   for b in {cond, uncond}
-// packed (sg): d_style is [Bn][n][style], one style per segment
+// sg with more than one segment (packed): d_style is [Bn][n][style], one style per segment
 static float* merge_const(idx_engine* e, S2melState* s, int Bn, int T, const float* d_prompt_x /*[Bn][T][80]*/,
                           const float* d_mu /*[Bn][T][content]*/, const float* d_style /*[Bn][style]*/,
                           const Segments* sg = nullptr) {
@@ -568,13 +565,13 @@ static float* merge_const(idx_engine* e, S2melState* s, int Bn, int T, const flo
   conv_gemm(e, gemm_of(s->cond_proj, d_mu, Bn, T, cp));
   copy_cols(e, d_prompt_x, C, rest, Kr, 0, (long long)Bn * T, C);
   copy_cols(e, cp, H, rest, Kr, C, (long long)Bn * T, H);
-  if (!sg) {
-    bcast_cols(e, d_style, rest, Kr, C + H, Bn, T, Sd);
-  } else {
+  if (sg && sg->n() > 1) {
     for (int bi = 0; bi < Bn; ++bi)
       for (int u = 0; u < sg->n(); ++u)
         bcast_cols(e, d_style + ((size_t)bi * sg->n() + u) * Sd, rest + ((size_t)bi * T + sg->off[u]) * Kr, Kr, C + H, 1,
                    sg->len(u), Sd);
+  } else {
+    bcast_cols(e, d_style, rest, Kr, C + H, Bn, T, Sd);
   }
   conv_gemm(e, gemm_of(s->merge_rest, rest, Bn, T, C0));
   return C0;
@@ -596,77 +593,71 @@ static void euler_times(int n, std::vector<float>& t, std::vector<float>& dt) {
   }
 }
 
-// full solve on device buffers. d_mu [T][content], d_prompt [80][P] (NCT), d_style [style],
-// d_z [80][T] (NCT) -> d_mel [80][T] (NCT).
-void cfm_solve_dev(idx_engine* e, S2melState* s, const float* d_mu, int T, const float* d_prompt, int P,
-                          const float* d_style, const float* d_z, int n_steps, float rate, float* d_mel) {
+CfmInputs cfm_inputs(idx_engine* e, const S2melState* s, int T, int n) {
   const idx_s2mel_config& c = s->cfg;
-  const int C = c.in_channels, H = c.hidden, Cd = c.content_dim, Sd = c.style_dim;
-  IDX_CHECK(P >= 0 && P <= T, IDX_ERR_ARG, "prompt longer than sequence");
-  IDX_CHECK(rate > 0.f, IDX_ERR_ARG, "inference_cfg_rate must be > 0 (the CFG pair path is the one built)");
-  const int Bn = 2;
-  // state x [T][80]; stacked inputs (cond, uncond)
-  float* x = e->arena.get<float>((size_t)T * C);
-  float* px = e->arena.get<float>((size_t)Bn * T * C);
-  float* mu2 = e->arena.get<float>((size_t)Bn * T * Cd);
-  float* st2 = e->arena.get<float>((size_t)Bn * Sd);
-  float* tmp = e->arena.get<float>((size_t)C * std::max(T, 1));
-  transpose_bct_to_btc(e, d_z, x, 1, C, T);
-  fill_zero(e, px, (long long)Bn * T * C);
-  if (P > 0) {
-    transpose_bct_to_btc(e, d_prompt, tmp, 1, C, P);   // [P][80]
-    IDX_CUDA(cudaMemcpyAsync(px, tmp, (size_t)P * C * 4, cudaMemcpyDeviceToDevice, e->stream));
-    fill_zero(e, x, (long long)P * C);                 // x[..., :prompt_len] = 0
-  }
-  fill_zero(e, mu2, (long long)Bn * T * Cd);
-  IDX_CUDA(cudaMemcpyAsync(mu2, d_mu, (size_t)T * Cd * 4, cudaMemcpyDeviceToDevice, e->stream));
-  fill_zero(e, st2, (long long)Bn * Sd);
-  IDX_CUDA(cudaMemcpyAsync(st2, d_style, (size_t)Sd * 4, cudaMemcpyDeviceToDevice, e->stream));
-  std::vector<float> ts, dts;
-  euler_times(n_steps, ts, dts);
-  float* d_t = e->arena.get<float>(n_steps);
-  IDX_CUDA(cudaMemcpyAsync(d_t, ts.data(), (size_t)n_steps * 4, cudaMemcpyHostToDevice, e->stream));
-  IDX_CUDA(cudaStreamSynchronize(e->stream));
-  TimeTables tt = time_tables(e, s, d_t, n_steps);
-  float* C0 = merge_const(e, s, Bn, T, px, mu2, st2);
-  DitBuffers b;
-  alloc_dit(e, s, b, Bn, T);
-  for (int k = 0; k < n_steps; ++k) {
-    dit_eval(e, s, b, Bn, T, x, 1, C0, tt.mod + (size_t)k * s->mod_width,
-             tt.wncond + (size_t)k * 2 * c.wn_hidden * c.wn_layers, tt.flmod + (size_t)k * 2 * c.wn_hidden);
-    cfg_euler(e, x, b.v, b.v + (size_t)T * C, dts[k], rate, T, C, P);
-  }
-  transpose_btc_to_bct(e, x, d_mel, 1, T, C);
-  (void)H;
+  CfmInputs in;
+  in.x = e->arena.get<float>((size_t)T * c.in_channels);
+  in.px = e->arena.get<float>((size_t)2 * T * c.in_channels);
+  in.mu2 = e->arena.get<float>((size_t)2 * T * c.content_dim);
+  in.st = e->arena.get<float>((size_t)2 * n * c.style_dim);
+  fill_zero(e, in.px, (long long)2 * T * c.in_channels);
+  fill_zero(e, in.mu2, (long long)2 * T * c.content_dim);
+  fill_zero(e, in.st, (long long)2 * n * c.style_dim);
+  return in;
 }
 
-// The CFM solves of several utterances as ONE solve over their frames packed along T (sg; see include/idxtts.h
-// idx_codes_to_wav_batch).  x [T][80] holds every z with its prompt frames zeroed, px / mu2 [2][T][*] the cond | uncond
-// inputs, st [2][n][style], zero_rows [T] marks each segment's prompt frames.  x is updated in place to the mel.
-void cfm_solve_packed_dev(idx_engine* e, S2melState* s, const Segments& sg, float* x, const float* px, const float* mu2,
-                          const float* st, const unsigned char* zero_rows, int n_steps, float rate) {
+void cfm_stage(idx_engine* e, const S2melState* s, const CfmInputs& in, int u, int o, int Tu, int P, const float* z,
+               const float* ref_mel, const float* mu, int mu_rows, const float* style) {
+  const idx_s2mel_config& c = s->cfg;
+  const int C = c.in_channels, Cd = c.content_dim, Sd = c.style_dim;
+  const size_t mark = e->arena.off;
+  float* d_z = e->arena.get<float>((size_t)C * Tu);
+  idx_to_device(e, d_z, z, (size_t)C * Tu * 4);
+  transpose_bct_to_btc(e, d_z, in.x + (size_t)o * C, 1, C, Tu);
+  if (P > 0) {
+    float* d_prompt = e->arena.get<float>((size_t)C * P);
+    idx_to_device(e, d_prompt, ref_mel, (size_t)C * P * 4);
+    transpose_bct_to_btc(e, d_prompt, in.px + (size_t)o * C, 1, C, P);
+    fill_zero(e, in.x + (size_t)o * C, (long long)P * C);          // x[..., :prompt_len] = 0
+  }
+  idx_to_device(e, in.mu2 + (size_t)o * Cd, mu, (size_t)mu_rows * Cd * 4);
+  idx_to_device(e, in.st + (size_t)u * Sd, style, (size_t)Sd * 4);
+  e->arena.off = mark;
+}
+
+void cfm_solve_dev(idx_engine* e, S2melState* s, Segments& sg, const int* P, const CfmInputs& in, int n_steps, float rate) {
   const idx_s2mel_config& c = s->cfg;
   const int C = c.in_channels, T = sg.total(), Bn = 2;
+  unsigned char* zero_rows = nullptr;       // packed: 1 on each segment's own prompt frames
+  if (sg.n() > 1) {
+    segments_upload(e, sg);
+    std::vector<unsigned char> zr(T, 0);
+    for (int u = 0; u < sg.n(); ++u) std::fill(zr.begin() + sg.off[u], zr.begin() + sg.off[u] + P[u], 1);
+    zero_rows = (unsigned char*)e->arena.alloc(T);
+    idx_to_device(e, zero_rows, zr.data(), T);
+  }
   std::vector<float> ts, dts;
   euler_times(n_steps, ts, dts);
   float* d_t = e->arena.get<float>(n_steps);
   IDX_CUDA(cudaMemcpyAsync(d_t, ts.data(), (size_t)n_steps * 4, cudaMemcpyHostToDevice, e->stream));
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   TimeTables tt = time_tables(e, s, d_t, n_steps);
-  float* C0 = merge_const(e, s, Bn, T, px, mu2, st, &sg);
+  float* C0 = merge_const(e, s, Bn, T, in.px, in.mu2, in.st, &sg);
   DitBuffers b;
   alloc_dit(e, s, b, Bn, T, &sg);
   for (int k = 0; k < n_steps; ++k) {
-    dit_eval(e, s, b, Bn, T, x, 1, C0, tt.mod + (size_t)k * s->mod_width,
+    dit_eval(e, s, b, Bn, T, in.x, 1, C0, tt.mod + (size_t)k * s->mod_width,
              tt.wncond + (size_t)k * 2 * c.wn_hidden * c.wn_layers, tt.flmod + (size_t)k * 2 * c.wn_hidden);
-    cfg_euler_rows(e, x, b.v, b.v + (size_t)T * C, dts[k], rate, T, C, zero_rows);
+    if (zero_rows) cfg_euler_rows(e, in.x, b.v, b.v + (size_t)T * C, dts[k], rate, T, C, zero_rows);
+    else cfg_euler(e, in.x, b.v, b.v + (size_t)T * C, dts[k], rate, T, C, P[0]);
   }
 }
-size_t cfm_packed_arena_bytes(const S2melState* s, int T, int nseg, int n_steps) {
+size_t cfm_arena_bytes(const S2melState* s, const Segments& sg, int n_steps) {
   const idx_s2mel_config& c = s->cfg;
-  return dit_arena_bytes_packed(s, 2, T, nseg) + 4 * (size_t)T * (8 * c.in_channels + 3 * c.content_dim + 6 * c.hidden + 2 * c.style_dim) +
+  const int T = sg.total(), n = sg.n();
+  return dit_arena_bytes(s, 2, T, n) + 4 * (size_t)T * (8 * c.in_channels + 3 * c.content_dim + 6 * c.hidden + 2 * c.style_dim) +
          4 * (size_t)n_steps * (s->mod_width + 2 * c.wn_hidden * (c.wn_layers + 1) + 6 * c.hidden + 512) +
-         16 * (size_t)nseg * 256 + (4 << 20);
+         (n > 1 ? (size_t)T + 16 * ((size_t)T / 128 + 2 * (size_t)n + 1) + 768 : 0) + (4 << 20);   // segment tables, zero_rows
 }
 bool cfm_packed_supported(const idx_engine* e, const S2melState* s) {
   const idx_s2mel_config& c = s->cfg;
@@ -681,11 +672,6 @@ size_t codec_arena_bytes(const S2melState* s, int n) {
 size_t lr_arena_bytes(const S2melState* s, int n_in, int ylen) {
   const idx_s2mel_config& c = s->cfg;
   return 4 * ((size_t)n_in * (c.lr_in + c.content_dim) + 4 * (size_t)ylen * c.content_dim) + (1 << 20);
-}
-size_t cfm_arena_bytes(const S2melState* s, int T, int n_steps) {
-  const idx_s2mel_config& c = s->cfg;
-  return dit_arena_bytes(s, 2, T) + 4 * (size_t)T * (8 * c.in_channels + 3 * c.content_dim + 6 * c.hidden + 2 * c.style_dim) +
-         4 * (size_t)n_steps * (s->mod_width + 2 * c.wn_hidden * (c.wn_layers + 1) + 6 * c.hidden + 512) + (4 << 20);
 }
 int s2mel_style_dim(const S2melState* s) { return s->cfg.style_dim; }
 int s2mel_content_dim(const S2melState* s) { return s->cfg.content_dim; }
@@ -746,7 +732,7 @@ extern "C" int idx_dit_forward(idx_engine* e, const float* x, const float* promp
   S2melState* s = e->s2mel;
   const idx_s2mel_config& c = s->cfg;
   const int C = c.in_channels;
-  e->ensure_arena(dit_arena_bytes(s, B, T) + 4 * (size_t)B * T * (4 * C + c.content_dim + 3 * c.hidden + c.style_dim) +
+  e->ensure_arena(dit_arena_bytes(s, B, T, 1) + 4 * (size_t)B * T * (4 * C + c.content_dim + 3 * c.hidden + c.style_dim) +
                   4 * (size_t)B * (s->mod_width + 2 * c.wn_hidden * (c.wn_layers + 1) + 6 * c.hidden + 512) + (4 << 20));
   e->arena.reset();
   float* d_x = e->arena.get<float>((size_t)B * C * T);
@@ -788,24 +774,21 @@ extern "C" int idx_cfm_solve(idx_engine* e, const float* mu, int T, const float*
   IDX_API_BEGIN
   IDX_CHECK(e && e->s2mel && e->s2mel->has_s2mel, IDX_ERR_STATE, "idx_s2mel_init has not been called");
   IDX_CHECK(mu && style && z && mel_out && T >= 1 && n_steps >= 1 && (P == 0 || prompt), IDX_ERR_ARG, "bad arguments");
+  IDX_CHECK(P >= 0 && P <= T, IDX_ERR_ARG, "prompt longer than sequence");
+  IDX_CHECK(cfg_rate > 0.f, IDX_ERR_ARG, "inference_cfg_rate must be > 0 (the CFG pair path is the one built)");
   IDX_CUDA(cudaSetDevice(e->device));
   S2melState* s = e->s2mel;
-  const idx_s2mel_config& c = s->cfg;
-  const int C = c.in_channels;
-  e->ensure_arena(dit_arena_bytes(s, 2, T) + 4 * (size_t)T * (8 * C + 3 * c.content_dim + 6 * c.hidden + 2 * c.style_dim) +
-                  4 * (size_t)n_steps * (s->mod_width + 2 * c.wn_hidden * (c.wn_layers + 1) + 6 * c.hidden + 512) + (4 << 20));
+  const int C = s->cfg.in_channels;
+  Segments sg;
+  sg.off = {0, T};
+  e->ensure_arena(cfm_arena_bytes(s, sg, n_steps));     // with room for the staged inputs and the mel
   e->arena.reset();
-  float* d_mu = e->arena.get<float>((size_t)T * c.content_dim);
-  float* d_prompt = e->arena.get<float>((size_t)C * std::max(P, 1));
-  float* d_style = e->arena.get<float>(c.style_dim);
-  float* d_z = e->arena.get<float>((size_t)C * T);
   float* d_mel = e->arena.get<float>((size_t)C * T);
-  idx_to_device(e, d_mu, mu, (size_t)T * c.content_dim * 4);
-  if (P > 0) idx_to_device(e, d_prompt, prompt, (size_t)C * P * 4);
-  idx_to_device(e, d_style, style, (size_t)c.style_dim * 4);
-  idx_to_device(e, d_z, z, (size_t)C * T * 4);
+  CfmInputs in = cfm_inputs(e, s, T, 1);
+  cfm_stage(e, s, in, 0, 0, T, P, z, prompt, mu, T, style);
   IDX_CUDA(cudaEventRecord(s->ev0, e->stream));
-  cfm_solve_dev(e, s, d_mu, T, d_prompt, P, d_style, d_z, n_steps, cfg_rate, d_mel);
+  cfm_solve_dev(e, s, sg, &P, in, n_steps, cfg_rate);
+  transpose_btc_to_bct(e, in.x, d_mel, 1, T, C);
   IDX_CUDA(cudaEventRecord(s->ev1, e->stream));
   idx_from_device(e, mel_out, d_mel, (size_t)C * T * 4);
   IDX_CUDA(cudaStreamSynchronize(e->stream));

@@ -10,14 +10,25 @@ size_t codec_arena_bytes(const S2melState* s, int n);
 void codec_decode_dev(idx_engine* e, S2melState* s, const int* d_codes, int n, float* d_out);
 size_t lr_arena_bytes(const S2melState* s, int n_in, int ylen);
 void length_regulate_dev(idx_engine* e, S2melState* s, const float* d_S, int n_in, int ylen, float* d_out);
-size_t cfm_arena_bytes(const S2melState* s, int T, int n_steps);
-void cfm_solve_dev(idx_engine* e, S2melState* s, const float* d_mu, int T, const float* d_prompt, int P,
-                   const float* d_style, const float* d_z, int n_steps, float rate, float* d_mel);
-// several utterances' solves as one solve over their frames packed along T (s2mel.cu)
+// The inputs of one CFM solve over T rows holding n utterances, in the CFG pair layout (cond, uncond): x [T][80] (the
+// noise; the mel [T][80] when the solve returns), px / mu2 [2][T][80 | content] and st [2][n][style].
+struct CfmInputs { float *x, *px, *mu2, *st; };
+// takes them from the arena, px / mu2 / st zeroed (the uncond entry stays zero)
+CfmInputs cfm_inputs(idx_engine* e, const S2melState* s, int T, int n);
+// utterance u at rows [o, o + Tu): x = z^T with the first P frames zeroed, cond px = ref_mel^T, the first mu_rows cond rows
+// of mu2 = mu, cond style u.  z [80][Tu], ref_mel [80][P], mu [mu_rows][content], style: host or device memory.
+void cfm_stage(idx_engine* e, const S2melState* s, const CfmInputs& in, int u, int o, int Tu, int P, const float* z,
+               const float* ref_mel, const float* mu, int mu_rows, const float* style);
+// The CFM solve of the utterances of sg as ONE solve over their frames packed along T: segment u owns rows
+// [off[u], off[u+1]) of both CFG batch entries and its first P[u] rows are prompt frames (include/idxtts.h
+// idx_codes_to_wav_batch).  One segment issues the launches of a single-utterance solve; two or more upload sg and take
+// the packed kernels, which exist only where cfm_packed_supported() holds.
+void cfm_solve_dev(idx_engine* e, S2melState* s, Segments& sg, const int* P, const CfmInputs& in, int n_steps, float rate);
+// arena of cfm_solve_dev over sg, with room for its staged inputs; the T x T attention scratch only where a one-segment
+// solve can take the unfused attention
+size_t cfm_arena_bytes(const S2melState* s, const Segments& sg, int n_steps);
+// true in the tail mode that has the packed solve (the default one)
 bool cfm_packed_supported(const idx_engine* e, const S2melState* s);
-size_t cfm_packed_arena_bytes(const S2melState* s, int T, int nseg, int n_steps);
-void cfm_solve_packed_dev(idx_engine* e, S2melState* s, const Segments& sg, float* x, const float* px, const float* mu2,
-                          const float* st, const unsigned char* zero_rows, int n_steps, float rate);
 int s2mel_content_dim(const S2melState* s);
 int s2mel_style_dim(const S2melState* s);
 int s2mel_codec_hidden(const S2melState* s);

@@ -7,6 +7,7 @@ packed result is expected to equal the solo one bit for bit; the bounds below al
 whether the results were bitwise equal.  Utterances are at least 32 frames long: below about 2^18 / (N K) rows the solo
 call runs its three fp32 input GEMMs (merge of x, cond projection, merge constant) on the SIMT kernel instead of tf32
 tensor cores, and the packed solve, having more rows, does not."""
+import ctypes
 import os
 
 import numpy as np
@@ -156,6 +157,26 @@ def test_errors_write_nothing(engine):
     for res in outs:
         for a in res.values():
             assert np.all(a == 7)
+
+
+def test_codebook_error_writes_nothing(engine):
+    """A code outside the codebook fails idx_codes_to_wav after the whole tail has run, before any output is written."""
+    c, cc = _load(engine, full=False)
+    u = _small_set(1, cc, c)[0]
+    u["codes"][5] = cc["codebook_size"] + 7
+    r, res, keep = engine._vocode_request(u["codes"], u["prompt_condition"], u["ref_mel"], u["style"], u["z"], u["F"],
+                                          True, True, True)
+    for a in res.values():
+        a[...] = 7
+    rc = engine.lib.idx_codes_to_wav(engine.h, ctypes.byref(r), 25, 0.7)
+    msg = engine.lib.idx_last_error(engine.h).decode()
+    print("code outside the codebook at position 5:", rc, msg)
+    assert rc == 2 and "outside the codebook" in msg and "request" not in msg
+    for a in res.values():
+        assert np.all(a == 7)
+    u["codes"][5] = 3      # the engine stays usable afterwards
+    out = engine.codes_to_wav(u["codes"], u["prompt_condition"], u["ref_mel"], u["style"], u["z"], u["F"], 25, 0.7)
+    assert np.isfinite(out["wav"]).all()
 
 
 # ------------------------------------------------------------------------------------- varlen flash attention --
