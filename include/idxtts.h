@@ -356,6 +356,42 @@ int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, const uint16_t
 int idx_debug_flash_attention_varlen(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16, int B,
                                      int H, const int32_t* seg_off, int n_seg, long long guard, float* out, uint16_t* out16);
 
+/* Diagnostic (tests): one of the tail's non-GEMM kernels, run through the host function the model calls (op below).
+ * x, x2, x3 and x16 are row-indexed inputs: the entry stages each whole [B][rows][C] block with 8 rows of NaN before and
+ * after it, so a read before the first or after the last row shows up as NaN in the output and never touches memory
+ * the call does not own (a read past the end of one batch entry lands in the next entry's rows, not in NaN).  out (fp32) and out16
+ * (fp16) are optional where the op writes both; each carries `guard` caller elements on both sides (see idx_debug_gemm).
+ * x is [B][T][C] unless stated.
+ *   0 layernorm:       w, b affine [C] or null; m0 = scale, m1 = shift [B][mod_stride] or null (mod_stride 0: one row)
+ *   1 rmsnorm_adaln:   w = norm weight [C]; m0 = modulation weight, m1 = modulation bias [B][mod_stride] or null
+ *   2 groupnorm1_mish: w, b [C]; out only
+ *   3 dwconv1d:        w [C][n2] (kernel n2), b [C] or null; out only
+ *   4 nearest_interp:  out [B][n2][C]
+ *   5 reflect_pad_rows:      out / out16 [B][T + left + right][C]
+ *   6 reflect_pad_segments:  x [B][seg_off[n_seg]][C]; out16 [B][seg_off[n_seg] + n_seg * (left + right)][C]
+ *   7 compact_segments16:    x16 [B][seg_off[n_seg] + (n_seg - 1) * gap][C] fp16; out16 [B][seg_off[n_seg]][C]
+ *   8 cfg_euler:       B = 1; x = state, x2 = v_cond, x3 = v_uncond [T][C]; rows < P zeroed; out = the new state [T][C]
+ *   9 cfg_euler_rows:  as 8 with zero_rows [T] (1 = zero the row) instead of P
+ *  10 rope_table:      head dim n2; out [T][n2 / 2][2]; with n_seg > 0 one table per segment (positions restart at 0)
+ *  11 Activation1d(SnakeBeta) of BigVGAN: w = alpha, b = beta [C] (exp'ed when logscale); out / out16
+ *  12 conv_post:       w [7][C], b [1] or null; tanh when use_tanh, else clamp to [-1, 1]; out [B][T]          */
+typedef struct {
+  int32_t op;
+  int32_t B, T, C, n2;
+  const float* x; const uint16_t* x16; const float* x2; const float* x3;
+  const float* w; const float* b;
+  const float* m0; const float* m1; int32_t mod_stride;
+  float eps;
+  const int32_t* seg_off; int32_t n_seg;     /* seg_off[0] = 0, strictly increasing                           */
+  int32_t left, right, gap;
+  float dt, rate; int32_t P; const uint8_t* zero_rows;
+  int32_t logscale, use_tanh;
+  int64_t guard;
+  float* out;
+  uint16_t* out16;
+} idx_debug_tail;
+int idx_debug_tail_op(idx_engine* e, const idx_debug_tail* d);
+
 /* ---------------------------------------------------------------- s2mel + codec -- */
 
 /* Geometry of the s2mel section of config.yaml as MyModel reads it

@@ -359,6 +359,26 @@ static void run_act(idx_engine* e, const BigvganState* s, const ActP& a, const f
   e->launches++;
 }
 
+void snake_params_dev(idx_engine* e, const float* alpha, const float* beta, float* ea, float* ib, int C, int logscale) {
+  exp_params_kernel<<<(C + 127) / 128, 128, 0, e->stream>>>(alpha, beta, ea, ib, C, logscale);
+  IDX_CUDA(cudaGetLastError());
+  e->launches++;
+}
+
+void snake_act_dev(idx_engine* e, const float* ea, const float* ib, int C, const float* x, float* y, int B, int T, __half* y16) {
+  BigvganState tmp;
+  if (e->bigvgan) tmp.taps = e->bigvgan->taps; else kaiser_sinc_taps(tmp.taps.f);
+  ActP a; a.ea = (float*)ea; a.ib = (float*)ib; a.C = C;
+  run_act(e, &tmp, a, x, y, B, T, y16);
+}
+
+void conv_post_dev(idx_engine* e, const float* x, const float* w, const float* bias, float* y, int B, int T, int C, int use_tanh) {
+  dim3 grid((T + 127) / 128, B);
+  conv_post_kernel<<<grid, 128, 0, e->stream>>>(x, w, bias, y, T, C, use_tanh);
+  IDX_CUDA(cudaGetLastError());
+  e->launches++;
+}
+
 static void run_conv(idx_engine* e, const ConvW& c, const float* x, float* out, int B, int T, const float* res, int accum, float scale,
                      const __half* x16 = nullptr) {
   ConvGemm g;
@@ -464,12 +484,7 @@ static void bigvgan_forward_impl(idx_engine* e, BigvganState* s, const float* d_
   }
   // NOTE: accumulate-then-scale: (xs0 + xs1 + xs2)/3 computed as ((xs0 + xs1) + xs2) * (1/3)
   run_act(e, s, s->act_post, P, ta, B, T);
-  {
-    dim3 grid((T + 127) / 128, B);
-    conv_post_kernel<<<grid, 128, 0, e->stream>>>(ta, s->conv_post_w, s->conv_post_b, d_wav, T, s->act_post.C, cfg.use_tanh_at_final);
-    IDX_CUDA(cudaGetLastError());
-    e->launches++;
-  }
+  conv_post_dev(e, ta, s->conv_post_w, s->conv_post_b, d_wav, B, T, s->act_post.C, cfg.use_tanh_at_final);
 }
 
 void bigvgan_forward_dev(idx_engine* e, BigvganState* s, const float* d_mel, int B, int F, float* d_wav) {
@@ -641,16 +656,11 @@ extern "C" int idx_antialias_snake(idx_engine* e, const float* x, const float* a
   idx_to_device(e, d_x, x, n * 4);
   idx_to_device(e, d_a, alpha, (size_t)C * 4);
   idx_to_device(e, d_b, beta, (size_t)C * 4);
-  exp_params_kernel<<<(C + 127) / 128, 128, 0, e->stream>>>(d_a, d_b, d_ea, d_ib, C, logscale);
-  IDX_CUDA(cudaGetLastError());
+  snake_params_dev(e, d_a, d_b, d_ea, d_ib, C, logscale);
   transpose_bct_to_btc(e, d_x, d_xt, B, C, T);
-  BigvganState tmp;
-  if (e->bigvgan) tmp.taps = e->bigvgan->taps; else kaiser_sinc_taps(tmp.taps.f);
-  ActP a; a.ea = d_ea; a.ib = d_ib; a.C = C;
-  run_act(e, &tmp, a, d_xt, d_yt, B, T);
+  snake_act_dev(e, d_ea, d_ib, C, d_xt, d_yt, B, T, nullptr);
   transpose_btc_to_bct(e, d_yt, d_x, B, T, C);
   idx_from_device(e, y, d_x, n * 4);
   IDX_CUDA(cudaStreamSynchronize(e->stream));
-  e->launches += 1;
   IDX_API_END(e)
 }

@@ -89,31 +89,36 @@ __global__ void gn_apply_mish_kernel(const float* __restrict__ x, float* __restr
   }
 }
 
+// Row-indexed kernels below take their rows from grid y with a grid-stride loop (row_grid): gridDim.y stops at 65535, and a
+// packed CFM solve can hold more rows than that.
 __global__ void dwconv_kernel(const float* __restrict__ x, float* __restrict__ y, int T, int C,
                               const float* __restrict__ w, const float* __restrict__ b, int k) {
   const int bi = blockIdx.z;
-  const int t = blockIdx.y;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const float* xb = x + (long long)bi * T * C;
-  float acc = b ? b[c] : 0.f;
   const int pad = (k - 1) / 2;
-  for (int j = 0; j < k; ++j) {
-    const int ts = t + j - pad;
-    if (ts >= 0 && ts < T) acc = fmaf(xb[(long long)ts * C + c], w[c * k + j], acc);
+  for (int t = blockIdx.y; t < T; t += gridDim.y) {
+    float acc = b ? b[c] : 0.f;
+    for (int j = 0; j < k; ++j) {
+      const int ts = t + j - pad;
+      if (ts >= 0 && ts < T) acc = fmaf(xb[(long long)ts * C + c], w[c * k + j], acc);
+    }
+    y[((long long)bi * T + t) * C + c] = acc;
   }
-  y[((long long)bi * T + t) * C + c] = acc;
 }
 
 __global__ void nearest_kernel(const float* __restrict__ x, float* __restrict__ y, int Tin, int Tout, int C) {
-  const int bi = blockIdx.z, t = blockIdx.y;
+  const int bi = blockIdx.z;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   // aten nearest_idx: scale = (float)in/out; src = min((int)floorf(dst * scale), in - 1)
   const float scale = (float)Tin / (float)Tout;
-  int src = (int)floorf((float)t * scale);
-  if (src > Tin - 1) src = Tin - 1;
-  y[((long long)bi * Tout + t) * C + c] = x[((long long)bi * Tin + src) * C + c];
+  for (int t = blockIdx.y; t < Tout; t += gridDim.y) {
+    int src = (int)floorf((float)t * scale);
+    if (src > Tin - 1) src = Tin - 1;
+    y[((long long)bi * Tout + t) * C + c] = x[((long long)bi * Tin + src) * C + c];
+  }
 }
 
 // ids outside [0, nrows) never index the table: the row is zero-filled and the engine flag records the position
@@ -175,16 +180,26 @@ __global__ void silu_kernel(float* x, long long n) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) { const float v = x[i]; x[i] = v / (1.f + expf(-v)); }
 }
-__global__ void reflect_pad_kernel(const float* __restrict__ x, float* __restrict__ y, int T, int C, int left,
-                                   int Tout, __half* __restrict__ y16) {
-  pdl_wait();
-  const int bi = blockIdx.z, i = blockIdx.y;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
+// Source row of output row i of a reflect-padded frame of T rows (encodec.py pad1d): an input no longer than the larger pad
+// is first zero-extended to Tr = max(left, right) + 1 rows, reflected, then cropped back.  Returns the row, or -1 where the
+// frame holds one of those zeros.  For T > max(left, right) this is F.pad(mode='reflect').
+__device__ __forceinline__ int reflect_src(int i, int T, int left, int right) {
+  const int Tr = max(T, max(left, right) + 1);
   int t = i - left;
   if (t < 0) t = -t;
-  if (t >= T) t = 2 * (T - 1) - t;
-  put(y, y16, ((long long)bi * Tout + i) * C + c, x[((long long)bi * T + t) * C + c]);
+  if (t >= Tr) t = 2 * (Tr - 1) - t;
+  return t < T ? t : -1;
+}
+__global__ void reflect_pad_kernel(const float* __restrict__ x, float* __restrict__ y, int T, int C, int left, int right,
+                                   int Tout, __half* __restrict__ y16) {
+  pdl_wait();
+  const int bi = blockIdx.z;
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  for (int i = blockIdx.y; i < Tout; i += gridDim.y) {
+    const int t = reflect_src(i, T, left, right);
+    put(y, y16, ((long long)bi * Tout + i) * C + c, t >= 0 ? x[((long long)bi * T + t) * C + c] : 0.f);
+  }
 }
 // segment of row r in a layout where segment u starts at row off[u] + u * gap: the largest such u with start <= r
 __device__ __forceinline__ int segment_of(const int* __restrict__ off, int n, int r, int gap) {
@@ -198,24 +213,26 @@ __device__ __forceinline__ int segment_of(const int* __restrict__ off, int n, in
 __global__ void reflect_pad_seg_kernel(const float* __restrict__ x, __half* __restrict__ y16, int T, int C, int left, int gap,
                                        int Tout, const int* __restrict__ off, int n) {
   pdl_wait();
-  const int bi = blockIdx.z, i = blockIdx.y;
+  const int bi = blockIdx.z;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const int u = segment_of(off, n, i, gap);
-  const int t0 = off[u], Tu = off[u + 1] - t0;
-  int t = i - t0 - u * gap - left;       // reflect_pad_kernel on the segment alone
-  if (t < 0) t = -t;
-  if (t >= Tu) t = 2 * (Tu - 1) - t;
-  y16[((long long)bi * Tout + i) * C + c] = __float2half_rn(x[((long long)bi * T + t0 + t) * C + c]);
+  for (int i = blockIdx.y; i < Tout; i += gridDim.y) {
+    const int u = segment_of(off, n, i, gap);
+    const int t0 = off[u], Tu = off[u + 1] - t0;
+    const int t = reflect_src(i - t0 - u * gap, Tu, left, gap - left);     // reflect_pad_kernel on the segment alone
+    y16[((long long)bi * Tout + i) * C + c] = __float2half_rn(t >= 0 ? x[((long long)bi * T + t0 + t) * C + c] : 0.f);
+  }
 }
 __global__ void compact_seg_kernel(const __half* __restrict__ x, __half* __restrict__ y, int T, int Mg, int C, int gap,
                                    const int* __restrict__ off, int n) {
   pdl_wait();
-  const int bi = blockIdx.z, r = blockIdx.y;
+  const int bi = blockIdx.z;
   const int c = (blockIdx.x * blockDim.x + threadIdx.x) * 8;      // 16-byte vectors (C % 8 == 0)
   if (c >= C) return;
-  const int u = segment_of(off, n, r, 0);
-  *(uint4*)(y + ((long long)bi * T + r) * C + c) = *(const uint4*)(x + ((long long)bi * Mg + r + u * gap) * C + c);
+  for (int r = blockIdx.y; r < T; r += gridDim.y) {
+    const int u = segment_of(off, n, r, 0);
+    *(uint4*)(y + ((long long)bi * T + r) * C + c) = *(const uint4*)(x + ((long long)bi * Mg + r + u * gap) * C + c);
+  }
 }
 __global__ void cfg_euler_rows_kernel(float* x, const float* vc, const float* vu, float dt, float rate, int T, int C,
                                       const unsigned char* __restrict__ zero_rows) {
@@ -635,6 +652,9 @@ __global__ void __launch_bounds__(128) flash_attn_tc_kernel(const __half* __rest
     (e)->launches++;               \
   } while (0)
 
+// grid y of the row-indexed kernels: one block row per row up to the hardware limit, the kernels loop beyond it
+static unsigned row_grid(long long rows) { return (unsigned)std::min<long long>(rows, 65535); }
+
 void layernorm(idx_engine* e, const float* x, float* y, int B, int T, int C, const float* w, const float* b,
                float eps, const float* scale, const float* shift, int mod_stride, __half* y16) {
   const long long rows = (long long)B * T;
@@ -659,12 +679,12 @@ void groupnorm1_mish(idx_engine* e, const float* x, float* y, int B, int T, int 
   LAUNCH_CHECK(e);
 }
 void dwconv1d(idx_engine* e, const float* x, float* y, int B, int T, int C, const float* w, const float* b, int k) {
-  dim3 grid((C + 127) / 128, T, B);
+  dim3 grid((C + 127) / 128, row_grid(T), B);
   dwconv_kernel<<<grid, 128, 0, e->stream>>>(x, y, T, C, w, b, k);
   LAUNCH_CHECK(e);
 }
 void nearest_interp(idx_engine* e, const float* x, float* y, int B, int Tin, int Tout, int C) {
-  dim3 grid((C + 127) / 128, Tout, B);
+  dim3 grid((C + 127) / 128, row_grid(Tout), B);
   nearest_kernel<<<grid, 128, 0, e->stream>>>(x, y, Tin, Tout, C);
   LAUNCH_CHECK(e);
 }
@@ -701,20 +721,20 @@ void fill_zero(idx_engine* e, float* x, long long n) {
 }
 void reflect_pad_rows(idx_engine* e, const float* x, float* y, int B, int T, int C, int left, int right, __half* y16) {
   const int Tout = T + left + right;
-  dim3 grid((C + 127) / 128, Tout, B);
-  launch_pdl(e, reflect_pad_kernel, grid, dim3(128), 0, x, y, T, C, left, Tout, y16);
+  dim3 grid((C + 127) / 128, row_grid(Tout), B);
+  launch_pdl(e, reflect_pad_kernel, grid, dim3(128), 0, x, y, T, C, left, right, Tout, y16);
   LAUNCH_CHECK(e);
 }
 void reflect_pad_segments(idx_engine* e, const float* x, __half* y16, int B, int C, int left, int right, const Segments& sg) {
   const int gap = left + right, Tout = sg.total() + sg.n() * gap;
-  dim3 grid((C + 127) / 128, Tout, B);
+  dim3 grid((C + 127) / 128, row_grid(Tout), B);
   launch_pdl(e, reflect_pad_seg_kernel, grid, dim3(128), 0, x, y16, sg.total(), C, left, gap, Tout, (const int*)sg.d_off, sg.n());
   LAUNCH_CHECK(e);
 }
 void compact_segments16(idx_engine* e, const __half* x, __half* y, int B, int C, int gap, const Segments& sg) {
   IDX_CHECK(C % 8 == 0, IDX_ERR_ARG, "compact_segments16: C must be a multiple of 8");
   const int T = sg.total(), Mg = T + (sg.n() - 1) * gap;
-  dim3 grid((C / 8 + 63) / 64, T, B);
+  dim3 grid((C / 8 + 63) / 64, row_grid(T), B);
   launch_pdl(e, compact_seg_kernel, grid, dim3(64), 0, x, y, T, Mg, C, gap, (const int*)sg.d_off, sg.n());
   LAUNCH_CHECK(e);
 }
@@ -737,6 +757,9 @@ void segments_upload(idx_engine* e, Segments& sg) {
 void rope_table(idx_engine* e, float* tab, int T, int hd) {
   rope_table_kernel<<<T, 32, 0, e->stream>>>(tab, T, hd);
   LAUNCH_CHECK(e);
+}
+void rope_table_segments(idx_engine* e, float* tab, const Segments& sg, int hd) {
+  for (int u = 0; u < sg.n(); ++u) rope_table(e, tab + (size_t)sg.off[u] * hd, sg.len(u), hd);
 }
 void attention_rope(idx_engine* e, const float* qkv, float* out, int B, int T, int H, const float* rope,
                     const int* lens, __half* out16) {

@@ -3,7 +3,7 @@
 //   * wgmma implicit GEMM (gemm_tc.cu): TMA-staged operands, register accumulators, tf32 or fp16;
 //   * a plain SIMT fp32 tile kernel (this file): bring-up / odd-shape path and the reference
 //     the tensor-core path is tested against.  Both are CUDA; neither is a CPU fallback.
-#include "ops.h"
+#include "stages.h"
 #include <cstdlib>
 #include <cstdio>
 
@@ -538,6 +538,121 @@ extern "C" int idx_debug_flash_attention_varlen(idx_engine* e, const uint16_t* q
   flash_attention_wgmma_varlen(e, dq, dk, dv, dOut ? dOut + guard : nullptr, dOut16 ? dOut16 + guard : nullptr, B, H, sg);
   if (dOut) idx_from_device(e, out - guard, dOut, 4 * ng);
   if (dOut16) idx_from_device(e, out16 - guard, dOut16, 2 * ng);
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  IDX_API_END(e)
+}
+
+// Diagnostic entry (tests): one of the tail's non-GEMM kernels through the host function the model calls
+// (include/idxtts.h, idx_debug_tail).  Row-indexed inputs sit between NaN guard rows; outputs travel with their guard bands.
+extern "C" int idx_debug_tail_op(idx_engine* e, const idx_debug_tail* d) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && d, IDX_ERR_ARG, "null argument");
+  IDX_CHECK(d->op >= 0 && d->op <= 12, IDX_ERR_ARG, "idx_debug_tail_op: unknown op");
+  IDX_CHECK(d->B > 0 && d->T > 0 && d->C > 0, IDX_ERR_ARG, "idx_debug_tail_op: bad shape");
+  IDX_CHECK(d->out || d->out16, IDX_ERR_ARG, "idx_debug_tail_op: no output");
+  IDX_CHECK(d->guard >= 0 && d->guard % 8 == 0, IDX_ERR_ARG, "idx_debug_tail_op: guard must be a non-negative multiple of 8");
+  IDX_CUDA(cudaSetDevice(e->device));
+  const int op = d->op, B = d->B, T = d->T, C = d->C;
+  Segments sg;
+  if (op == 6 || op == 7 || (op == 10 && d->n_seg > 0)) {
+    IDX_CHECK(d->seg_off && d->n_seg > 0 && d->seg_off[0] == 0, IDX_ERR_ARG, "idx_debug_tail_op: bad segment table");
+    sg.off.assign(d->seg_off, d->seg_off + d->n_seg + 1);
+    for (int u = 0; u < d->n_seg; ++u)
+      IDX_CHECK(sg.off[u + 1] > sg.off[u], IDX_ERR_ARG, "idx_debug_tail_op: segment offsets must increase");
+    IDX_CHECK(op == 7 || sg.total() == T, IDX_ERR_ARG, "idx_debug_tail_op: T must be the packed length");
+  }
+  // rows of x / x16 and of the output
+  long long xrows = (long long)B * T, orows = (long long)B * T;
+  int ocols = C;
+  switch (op) {
+    case 4: orows = (long long)B * d->n2; break;
+    case 5: orows = (long long)B * (T + d->left + d->right); break;
+    case 6: orows = (long long)B * (T + (long long)sg.n() * (d->left + d->right)); break;
+    case 7: xrows = (long long)B * (sg.total() + (long long)(sg.n() - 1) * d->gap); orows = (long long)B * sg.total(); break;
+    case 10: ocols = d->n2; break;
+    case 12: ocols = 1; break;
+    default: break;
+  }
+  IDX_CHECK((op == 8 || op == 9 || op == 10) ? B == 1 : true, IDX_ERR_ARG, "idx_debug_tail_op: ops 8-10 take B = 1");
+  IDX_CHECK(op == 7 ? d->x16 != nullptr : (op == 10 || d->x != nullptr), IDX_ERR_ARG, "idx_debug_tail_op: input missing");
+  IDX_CHECK((op != 8 && op != 9) || (d->x2 && d->x3 && (op == 8 || d->zero_rows)), IDX_ERR_ARG, "idx_debug_tail_op: cfg_euler inputs missing");
+  IDX_CHECK((op != 1 && op != 2 && op != 3 && op != 11 && op != 12) || d->w, IDX_ERR_ARG, "idx_debug_tail_op: weight missing");
+  IDX_CHECK((op != 2 && op != 11) || d->b, IDX_ERR_ARG, "idx_debug_tail_op: second parameter vector missing");
+  IDX_CHECK(!d->m0 == !d->m1 && d->mod_stride >= 0, IDX_ERR_ARG, "idx_debug_tail_op: modulation needs both vectors");
+  const bool f16_out = op == 0 || op == 1 || op == 5 || op == 6 || op == 7 || op == 11;
+  const bool f32_out = !(op == 6 || op == 7);
+  IDX_CHECK(f16_out || !d->out16, IDX_ERR_ARG, "idx_debug_tail_op: this op has no fp16 output");
+  IDX_CHECK(f32_out || !d->out, IDX_ERR_ARG, "idx_debug_tail_op: this op has no fp32 output");
+  IDX_CHECK(op != 10 || (d->n2 > 0 && d->n2 % 2 == 0 && d->n2 <= 64), IDX_ERR_ARG, "idx_debug_tail_op: rope head dim");
+  IDX_CHECK(op != 3 || d->n2 > 0, IDX_ERR_ARG, "idx_debug_tail_op: dwconv kernel size");
+  IDX_CHECK(op != 4 || d->n2 > 0, IDX_ERR_ARG, "idx_debug_tail_op: nearest output length");
+
+  constexpr int G = 8;                              // NaN guard rows on each side of a row-indexed input
+  const size_t nx = (size_t)xrows * C, gx = (size_t)G * C, no = (size_t)orows * ocols, g2 = 2 * (size_t)d->guard;
+  const size_t nmod = d->m0 ? (size_t)(B - 1) * d->mod_stride + C : 0;
+  const size_t nw = op == 3 ? (size_t)C * d->n2 : (op == 12 ? 7 * (size_t)C : C);
+  e->ensure_arena(3 * 4 * (nx + 2 * gx) + 2 * (nx + 2 * gx) + 6 * (no + g2) + 4 * (2 * nw + 2 * nmod + 4 * (size_t)C) +
+                  (size_t)T + 16 * (size_t)(sg.off.size() + T / 128 + 2) + (16 << 20));
+  e->arena.reset();
+  auto stage_rows = [&](const void* src, size_t esz) -> void* {     // [G NaN rows][rows][G NaN rows]
+    if (!src) return nullptr;
+    char* p = (char*)e->arena.alloc((nx + 2 * gx) * esz);
+    IDX_CUDA(cudaMemsetAsync(p, 0xFF, (nx + 2 * gx) * esz, e->stream));   // all-ones: NaN in fp32 and fp16
+    idx_to_device(e, p + gx * esz, src, nx * esz);
+    return p + gx * esz;
+  };
+  auto stage = [&](const void* src, size_t bytes) -> void* {
+    if (!src) return nullptr;
+    void* p = e->arena.alloc(bytes);
+    idx_to_device(e, p, src, bytes);
+    return p;
+  };
+  const float* dx = (const float*)stage_rows(op == 7 ? nullptr : d->x, 4);
+  const __half* dx16 = (const __half*)stage_rows(op == 7 ? d->x16 : nullptr, 2);
+  const float* dx2 = (const float*)stage_rows(d->x2, 4);
+  const float* dx3 = (const float*)stage_rows(d->x3, 4);
+  const float* dw = (const float*)stage(d->w, nw * 4);
+  const float* db = (const float*)stage(d->b, (op == 12 ? 1 : C) * 4);
+  const float* dm0 = (const float*)stage(d->m0, nmod * 4);
+  const float* dm1 = (const float*)stage(d->m1, nmod * 4);
+  const unsigned char* dz = (op == 9) ? (const unsigned char*)stage(d->zero_rows, (size_t)T) : nullptr;
+  float* dOut = d->out ? e->arena.get<float>(no + g2) : nullptr;
+  __half* dOut16 = d->out16 ? (__half*)e->arena.alloc((no + g2) * 2) : nullptr;
+  if (dOut) idx_to_device(e, dOut, d->out - d->guard, (no + g2) * 4);
+  if (dOut16) idx_to_device(e, dOut16, d->out16 - d->guard, (no + g2) * 2);
+  float* y = dOut ? dOut + d->guard : nullptr;
+  __half* y16 = dOut16 ? dOut16 + d->guard : nullptr;
+  if (!sg.off.empty()) segments_upload(e, sg);
+  switch (op) {
+    case 0: layernorm(e, dx, y, B, T, C, dw, db, d->eps, dm0, dm1, d->mod_stride, y16); break;
+    case 1: rmsnorm_adaln(e, dx, y, B, T, C, dw, dm0, dm1, d->mod_stride, d->eps, y16); break;
+    case 2: groupnorm1_mish(e, dx, y, B, T, C, dw, db, d->eps); break;
+    case 3: dwconv1d(e, dx, y, B, T, C, dw, db, d->n2); break;
+    case 4: nearest_interp(e, dx, y, B, T, d->n2, C); break;
+    case 5: reflect_pad_rows(e, dx, y, B, T, C, d->left, d->right, y16); break;
+    case 6: reflect_pad_segments(e, dx, y16, B, C, d->left, d->right, sg); break;
+    case 7: compact_segments16(e, dx16, y16, B, C, d->gap, sg); break;
+    case 8:
+    case 9:
+      IDX_CUDA(cudaMemcpyAsync(y, dx, nx * 4, cudaMemcpyDeviceToDevice, e->stream));    // the state is updated in place
+      if (op == 8) cfg_euler(e, y, dx2, dx3, d->dt, d->rate, T, C, d->P);
+      else cfg_euler_rows(e, y, dx2, dx3, d->dt, d->rate, T, C, dz);
+      break;
+    case 10:
+      if (sg.off.empty()) rope_table(e, y, T, d->n2);
+      else rope_table_segments(e, y, sg, d->n2);
+      break;
+    case 11: {
+      float* ea = e->arena.get<float>(C);
+      float* ib = e->arena.get<float>(C);
+      snake_params_dev(e, dw, db, ea, ib, C, d->logscale);
+      snake_act_dev(e, ea, ib, C, dx, y, B, T, y16);
+      break;
+    }
+    case 12: conv_post_dev(e, dx, dw, db, y, B, T, C, d->use_tanh); break;
+  }
+  if (dOut) idx_from_device(e, d->out - d->guard, dOut, (no + g2) * 4);
+  if (dOut16) idx_from_device(e, d->out16 - d->guard, dOut16, (no + g2) * 2);
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   IDX_API_END(e)
 }

@@ -122,7 +122,8 @@ void attention_rope(idx_engine* e, const float* qkv, float* out, int B, int T, i
 void cfg_euler(idx_engine* e, float* x, const float* v_cond, const float* v_uncond, float dt, float rate,
                int T, int C, int P);
 void fill_zero(idx_engine* e, float* x, long long n);
-// y[b][i][:] = x[b][reflect(i - left)][:], i in [0, T + left + right)   (F.pad mode='reflect')
+// y[b][i][:] = x[b][reflect(i - left)][:], i in [0, T + left + right)   (encodec.py pad1d mode='reflect': F.pad's reflection,
+// with an input no longer than max(left, right) zero-extended to max(left, right) + 1 rows first)
 void reflect_pad_rows(idx_engine* e, const float* x, float* y, int B, int T, int C, int left, int right, __half* y16 = nullptr);
 
 // ------------------------------------------------------------------------ packed weights --
@@ -186,6 +187,8 @@ void reflect_pad_segments(idx_engine* e, const float* x, __half* y16, int B, int
 // undo the gaps: y[b][off[u] + t] = x[b][off[u] + u * gap + t], x [B][total + n * gap - gap][C] fp16 (the rows a
 // multi-tap GEMM over the gapped layout produces), y [B][total][C]
 void compact_segments16(idx_engine* e, const __half* x, __half* y, int B, int C, int gap, const Segments& sg);
+// rope_table per segment: segment u's positions restart at 0 in rows [off[u], off[u+1]) of tab [total][hd/2][2]
+void rope_table_segments(idx_engine* e, float* tab, const Segments& sg, int hd);
 // cfg_euler with the rows listed in zero_rows (1 = prompt frame of its segment) zeroed
 void cfg_euler_rows(idx_engine* e, float* x, const float* v_cond, const float* v_uncond, float dt, float rate, int T, int C,
                     const unsigned char* zero_rows);

@@ -505,7 +505,7 @@ static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T
   if (sg) {
     IDX_CHECK(b.a16 && tail_fused() && fa_wgmma_on(), IDX_ERR_STATE, "packed solve outside the fp16 fused tail mode");
     b.wacts16g = (__half*)e->arena.alloc((size_t)Bn * padT * WH * sizeof(__half) + 16);
-    for (int u = 0; u < sg->n(); ++u) rope_table(e, b.rope + (size_t)sg->off[u] * 64, sg->len(u), 64);
+    rope_table_segments(e, b.rope, *sg, 64);
   } else {
     rope_table(e, b.rope, T, 64);
   }

@@ -38,6 +38,12 @@ size_t bigvgan_arena_bytes(const BigvganState* s, int B, int F);
 int bigvgan_total_up(const BigvganState* s);
 // d_mel [B][num_mels][F] (NCT) -> d_wav [B][F*total_up]
 void bigvgan_forward_dev(idx_engine* e, BigvganState* s, const float* d_mel, int B, int F, float* d_wav);
+// BigVGAN's fused Activation1d(SnakeBeta) over x [B][T][C] with the per-channel ea = exp(alpha) (or alpha) and
+// ib = 1 / (exp(beta) (or beta) + 1e-9) of snake_params_dev; FIR taps of the loaded generator, else the computed ones
+void snake_params_dev(idx_engine* e, const float* alpha, const float* beta, float* ea, float* ib, int C, int logscale);
+void snake_act_dev(idx_engine* e, const float* ea, const float* ib, int C, const float* x, float* y, int B, int T, __half* y16);
+// BigVGAN conv_post: Conv1d(C -> 1, k 7, pad 3) with w [7][C], optional bias [1], then tanh or a clamp to [-1, 1]; y [B][T]
+void conv_post_dev(idx_engine* e, const float* x, const float* w, const float* bias, float* y, int B, int T, int C, int use_tanh);
 void s2mel_set_ms(S2melState* s, double codec, double lr, double cfm);
 void bigvgan_set_ms(BigvganState* s, double ms);
 

@@ -90,6 +90,25 @@ class DebugGemm(C.Structure):
                 ("heads", C.c_int32), ("guard", C.c_int64), ("out", C.c_void_p), ("out16", C.c_void_p)]
 
 
+class DebugTail(C.Structure):
+    """include/idxtts.h idx_debug_tail."""
+    _fields_ = [("op", C.c_int32), ("B", C.c_int32), ("T", C.c_int32), ("C", C.c_int32), ("n2", C.c_int32),
+                ("x", C.c_void_p), ("x16", C.c_void_p), ("x2", C.c_void_p), ("x3", C.c_void_p),
+                ("w", C.c_void_p), ("b", C.c_void_p), ("m0", C.c_void_p), ("m1", C.c_void_p), ("mod_stride", C.c_int32),
+                ("eps", C.c_float), ("seg_off", C.c_void_p), ("n_seg", C.c_int32),
+                ("left", C.c_int32), ("right", C.c_int32), ("gap", C.c_int32),
+                ("dt", C.c_float), ("rate", C.c_float), ("P", C.c_int32), ("zero_rows", C.c_void_p),
+                ("logscale", C.c_int32), ("use_tanh", C.c_int32), ("guard", C.c_int64),
+                ("out", C.c_void_p), ("out16", C.c_void_p)]
+
+
+_byref = C.byref          # debug_tail_op takes a parameter named C
+
+TAIL_OPS = {"layernorm": 0, "rmsnorm_adaln": 1, "groupnorm1_mish": 2, "dwconv1d": 3, "nearest_interp": 4,
+            "reflect_pad_rows": 5, "reflect_pad_segments": 6, "compact_segments16": 7, "cfg_euler": 8,
+            "cfg_euler_rows": 9, "rope_table": 10, "snake_act": 11, "conv_post": 12}
+
+
 # Guard bands of the diagnostic entries: sentinel NaNs (a payload no kernel produces) on both sides of every output,
 # at least one 128-row tile long, so a store to a row or column outside the output lands in them.
 _SENTINEL32 = np.uint32(0x7FC0DEAD)
@@ -198,6 +217,7 @@ def load_library(path: str = None):
                                               C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]
     lib.idx_debug_flash_attention_varlen.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                                      C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]
+    lib.idx_debug_tail_op.argtypes = [C.c_void_p, C.POINTER(DebugTail)]
     lib.idx_s2mel_init.argtypes = [C.c_void_p, C.POINTER(S2melConfig)]
     lib.idx_codec_init.argtypes = [C.c_void_p, C.POINTER(CodecConfig)]
     lib.idx_codec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -790,6 +810,58 @@ class Engine:
             _check_guard(buf, guard, n, "idx_debug_flash_attention_varlen")
             dt = np.float32 if buf.dtype == np.uint32 else np.float16
             res.append(buf[guard:guard + n].view(dt).reshape(B, T, H * 64).copy())
+        return tuple(res)
+
+    def debug_tail_op(self, op, x=None, B=1, T=None, C=None, n2=0, x16=None, x2=None, x3=None, w=None, b=None, m0=None,
+                      m1=None, mod_stride=0, eps=0.0, seg_off=None, left=0, right=0, gap=0, dt=0.0, rate=0.0, P=0,
+                      zero_rows=None, logscale=0, use_tanh=0, out=True, out16=False):
+        """One of the tail's non-GEMM kernels (include/idxtts.h idx_debug_tail; op is a name of TAIL_OPS) through the host
+        function the model calls.  x is [B][T][C] fp32 (x16 fp16 for compact_segments16); T and C default to its shape.
+        Returns (out or None, out16 or None), shaped [B][rows][C] ([T][n2/2][2] for rope_table, [B][T] for conv_post);
+        raises AssertionError when the kernel wrote outside them."""
+        op = TAIL_OPS[op]
+        src = x if x is not None else x16
+        if src is not None:
+            src = np.asarray(src)
+            B, T, C = (src.shape if src.ndim == 3 else (1,) + src.shape) if T is None else (B, T, C)
+        so = None if seg_off is None else np.ascontiguousarray(np.asarray(seg_off, dtype=np.int32))
+        n_seg = 0 if so is None else len(so) - 1
+        if op == 7:
+            T = int(so[-1])
+        if op == 4:
+            rows, cols = n2, C
+        elif op == 5:
+            rows, cols = T + left + right, C
+        elif op == 6:
+            rows, cols = T + n_seg * (left + right), C
+        elif op == 10:
+            rows, cols = T, n2
+        elif op == 12:
+            rows, cols = T, 1
+        else:
+            rows, cols = T, C
+        f32 = lambda v: None if v is None else np.ascontiguousarray(v, dtype=np.float32)   # noqa: E731
+        keep = [f32(x), None if x16 is None else np.ascontiguousarray(x16, dtype=np.float16), f32(x2), f32(x3), f32(w),
+                f32(b), f32(m0), f32(m1), so, None if zero_rows is None else np.ascontiguousarray(zero_rows, np.uint8)]
+        n, guard = B * rows * cols, _guard_len(cols)
+        b32 = _guarded(n, guard, np.float32) if out else None
+        b16 = _guarded(n, guard, np.float16) if out16 else None
+        d = DebugTail(op=op, B=B, T=T, C=C, n2=int(n2), mod_stride=int(mod_stride), eps=float(eps), n_seg=n_seg,
+                      left=int(left), right=int(right), gap=int(gap), dt=float(dt), rate=float(rate), P=int(P),
+                      logscale=int(logscale), use_tanh=int(use_tanh), guard=guard,
+                      out=None if b32 is None else b32.ctypes.data + 4 * guard,
+                      out16=None if b16 is None else b16.ctypes.data + 2 * guard)
+        d.x, d.x16, d.x2, d.x3, d.w, d.b, d.m0, d.m1, d.seg_off, d.zero_rows = (_ptr(v) for v in keep)
+        self._check(self.lib.idx_debug_tail_op(self.h, _byref(d)), "idx_debug_tail_op")
+        shape = (T, n2 // 2, 2) if op == 10 else ((B, T) if op == 12 else (B, rows, cols))
+        res = []
+        for buf in (b32, b16):
+            if buf is None:
+                res.append(None)
+                continue
+            _check_guard(buf, guard, n, "idx_debug_tail_op")
+            dt_ = np.float32 if buf.dtype == np.uint32 else np.float16
+            res.append(buf[guard:guard + n].view(dt_).reshape(shape).copy())
         return tuple(res)
 
     # ------------------------------------------------------------------- emotion --

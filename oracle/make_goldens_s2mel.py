@@ -6,7 +6,12 @@ the restatement oracle/s2mel.py against them.
 Writes tests/golden/s2mel_small.npz (reduced dims: codec decode, length regulator, one DiT
 evaluation, full 6-step CFM solve) and tests/golden/s2mel_full_dit.npz (the [ASSUMED] full
 IndexTTS-2.5 dims, one DiT evaluation at T=96 and a codec/length-regulator pass).  Weights are
-regenerated from seeds by oracle.s2mel.make_*_weights on the GPU box."""
+regenerated from seeds by oracle.s2mel.make_*_weights on the GPU box.
+
+    python -m oracle.make_goldens_s2mel short
+
+writes only tests/golden/s2mel_short.npz: the reference's reflect-padded SConv1d (encodec.py pad1d) at 1, 2 and 3 frames
+and one small-dims DiT evaluation at T = 1 and 2, the lengths where pad1d zero-extends before it reflects."""
 import os
 import sys
 
@@ -16,8 +21,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import refimport  # noqa: E402
-from oracle.s2mel import (CODEC_CFG, S2MEL_CFG, cfm_inference, codec_decode, dit_forward, fold_weight_norm,  # noqa: E402
-                          length_regulate, make_codec_weights, make_s2mel_weights, small_codec_cfg,
+from oracle.s2mel import (CODEC_CFG, S2MEL_CFG, _reflect_conv, cfm_inference, codec_decode, dit_forward,  # noqa: E402
+                          fold_weight_norm, length_regulate, make_codec_weights, make_s2mel_weights, small_codec_cfg,
                           small_s2mel_cfg)
 
 GOLD = os.path.join(ROOT, "tests", "golden")
@@ -121,7 +126,44 @@ def main():
                         ylen=ylen, cond=cond_ref.numpy(), mu=mu.numpy(), prompt=prompt.numpy(), style=style.numpy(),
                         z=z.numpy(), t=tt.numpy(), dit=d_ref.numpy(), seed_s2mel=1234, seed_codec=4321)
     print("wrote s2mel goldens")
+    short_goldens()
+
+
+@torch.no_grad()
+def short_goldens():
+    refimport.setup()
+    from indextts.s2mel.modules.encodec import SConv1d
+    out = {}
+    g = torch.Generator().manual_seed(21)
+    conv = SConv1d(6, 5, kernel_size=5, pad_mode="reflect")     # the WaveNet in-layer's padding, (2, 2)
+    with torch.no_grad():
+        for p in conv.parameters():
+            p.copy_(torch.randn(p.shape, generator=g))
+    out["sconv_weight"], out["sconv_bias"] = conv.conv.conv.weight.numpy(), conv.conv.conv.bias.numpy()
+    for T in (1, 2, 3):
+        x = torch.randn(1, 6, T, generator=g)
+        y = conv(x)
+        assert (y - _reflect_conv(x, conv.conv.conv.weight, conv.conv.conv.bias, 5)).abs().max() < 1e-5
+        out[f"sconv_x{T}"], out[f"sconv_y{T}"] = x.numpy(), y.numpy()
+    c = small_s2mel_cfg()
+    w = make_s2mel_weights(c, seed=1234)
+    est = ref_s2mel(c, w).models["cfm"].estimator
+    for T in (1, 2):
+        mu, _, style, z = inputs(c, T, 0, 30 + T)
+        px = torch.zeros(1, 80, T)
+        tt = torch.tensor([0.45])
+        d_ref = est(z, px, torch.LongTensor([T]), tt, style, mu)
+        d_or = dit_forward(fold_weight_norm(w), c, z, px, torch.LongTensor([T]), tt, style, mu)
+        print(f"DiT forward T={T}: max|ref-oracle| =", (d_ref - d_or).abs().max().item())
+        assert (d_ref - d_or).abs().max() < 2e-4
+        out.update({f"dit{T}_mu": mu.numpy(), f"dit{T}_style": style.numpy(), f"dit{T}_z": z.numpy(), f"dit{T}_t": tt.numpy(),
+                    f"dit{T}": d_ref.numpy()})
+    np.savez_compressed(os.path.join(GOLD, "s2mel_short.npz"), seed_s2mel=1234, **out)
+    print("wrote s2mel_short.npz")
 
 
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["short"]:
+        short_goldens()
+    else:
+        main()

@@ -130,10 +130,19 @@ def _rope(x, hd):
     return o.flatten(3)
 
 
+def pad1d_reflect(x, left, right):
+    """encodec.py pad1d(mode='reflect'): an input no longer than the larger pad is zero-extended to max(left, right) + 1
+    frames, reflected, and the extension cropped off again (F.pad alone refuses such short inputs)."""
+    extra = max(max(left, right) + 1 - x.shape[-1], 0)
+    x = F.pad(x, (0, extra))
+    y = F.pad(x, (left, right), mode="reflect")
+    return y[..., :y.shape[-1] - extra]
+
+
 def _reflect_conv(x, weight, bias, k):
     if k > 1:
         pt = k - 1
-        x = F.pad(x, (pt - pt // 2, pt // 2), mode="reflect")   # encodec.py:214-229 (stride 1)
+        x = pad1d_reflect(x, pt - pt // 2, pt // 2)             # encodec.py:214-229 (stride 1)
     return F.conv1d(x, weight, bias)
 
 

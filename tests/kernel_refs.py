@@ -163,3 +163,158 @@ def swiglu(a, b):
 def wn_gate(a, c):
     """WaveNet fused_add_tanh_sigmoid_multiply: tanh(a) * sigmoid(c) (the conditioning g already added), float64."""
     return np.tanh(np.asarray(a, np.float64)) / (1.0 + np.exp(-np.asarray(c, np.float64)))
+
+
+# ---------------------------------------------------------------- the tail's non-GEMM kernels ----
+U = 2.0 ** -24            # unit roundoff of fp32
+
+
+def pad1d_reflect_rows(T, left, right):
+    """Source row of every row of a reflect-padded frame of T rows (encodec.py pad1d mode='reflect'), -1 for a zero row:
+    an input of T <= max(left, right) rows is zero-extended to max(left, right) + 1 rows, reflected by F.pad, cropped."""
+    Tr = max(T, max(left, right) + 1)
+    idx = np.pad(np.arange(Tr), (left, right), mode="reflect")[:T + left + right]
+    return np.where(idx < T, idx, -1)
+
+
+def pad1d_reflect(x, left, right):
+    """x [..., T, C] reflect-padded along T as pad1d does, float64."""
+    x = np.asarray(x, np.float64)
+    src = pad1d_reflect_rows(x.shape[-2], left, right)
+    out = np.take(x, np.maximum(src, 0), axis=-2)
+    out[..., src < 0, :] = 0.0
+    return out
+
+
+def rownorm(x, T, mode, w=None, b=None, eps=0.0, m0=None, m1=None, mod_stride=0):
+    """The row norms of rownorm_kernel on x [rows][C], float64: mode 0 LayerNorm (affine w, b; modulation
+    v * (1 + m0[r // T]) + m1[r // T]), mode 1 RMSNorm times w (modulation m0[r // T] * v + m1[r // T]).  m0 / m1 are flat
+    [B * mod_stride (+ C)] vectors read at (r // T) * mod_stride.  Returns (out, bound): bound is the worst-case error of
+    the kernel's fp32 evaluation: warp sums of C / 32 terms and a 5-level tree (n = C / 32 + 5), rsqrtf (2 ulp), and one
+    rounding per later product / sum."""
+    x = np.asarray(x, np.float64)
+    R, C = x.shape
+    n = -(-C // 32) + 5
+    bi = np.arange(R) // T
+    if mode == 0:
+        mean = x.mean(1, keepdims=True)
+        dm = (n + 1) * U * np.abs(x).sum(1, keepdims=True) / C          # error of the fp32 mean
+    else:
+        mean, dm = 0.0, 0.0
+    d = x - mean
+    q = (d * d).mean(1, keepdims=True)
+    rstd = 1.0 / np.sqrt(q + eps)
+    v = d * rstd
+    # q: n + 2 roundings per term, plus the mean's error through 2|d|; the variance + eps and rsqrtf
+    rel_q = (n + 3) * U + 2 * np.abs(d).mean(1, keepdims=True) * dm / np.maximum(q + eps, 1e-300)
+    rel_rstd = 0.5 * rel_q + 4 * U
+    err = np.abs(v) * (rel_rstd + 2 * U) + dm * rstd
+    one = np.ones(C)
+    ww = one if w is None else np.asarray(w, np.float64)
+    bb = np.zeros(C) if b is None else np.asarray(b, np.float64)
+    v = v * ww + bb
+    err = err * np.abs(ww) + 2 * U * (np.abs(v) + np.abs(bb))
+    if m0 is not None:
+        m0, m1 = np.asarray(m0, np.float64), np.asarray(m1, np.float64)
+        rows = bi[:, None] * mod_stride + np.arange(C)[None]
+        s, t = m0[rows], m1[rows]
+        f = 1.0 + s if mode == 0 else s
+        vo = v * f + t
+        err = err * np.abs(f) + 3 * U * (np.abs(v * f) + np.abs(t)) + (U * np.abs(v * f) if mode == 0 else 0.0)
+        v = vo
+    return v, err + U * np.abs(v)
+
+
+def gn_mish(x, w, b, eps):
+    """GroupNorm(1 group) over each [T][C] block of x [B][T][C], per-channel affine, then Mish (F.mish), float64.
+    Returns (out, y): y = the normalised, affine value Mish is applied to."""
+    x = np.asarray(x, np.float64)
+    mean = x.mean(axis=(1, 2), keepdims=True)
+    var = x.var(axis=(1, 2), keepdims=True)
+    y = (x - mean) / np.sqrt(var + eps) * np.asarray(w, np.float64) + np.asarray(b, np.float64)
+    return y * np.tanh(np.logaddexp(0.0, y)), y
+
+
+def dwconv(x, w, b, k):
+    """Depthwise Conv1d of x [B][T][C] with w [C][k], zero padding (k - 1) // 2, bias b [C] or None.  Returns (out, mag)
+    float64; mag = the same sum over absolute values."""
+    x = np.asarray(x, np.float64)
+    w = np.asarray(w, np.float64)
+    B, T, C = x.shape
+    pad = (k - 1) // 2
+    out = np.zeros((B, T, C)) + (0.0 if b is None else np.asarray(b, np.float64))
+    mag = np.abs(out)
+    for j in range(k):
+        src = np.arange(T) + j - pad
+        ok = (src >= 0) & (src < T)
+        out[:, ok] += x[:, src[ok]] * w[:, j]
+        mag[:, ok] += np.abs(x[:, src[ok]] * w[:, j])
+    return out, mag
+
+
+def activation1d(x, alpha, beta, taps, logscale):
+    """BigVGAN's Activation1d(SnakeBeta) on channels-last x [B][T][C] with the 12 FIR taps, float64 (sine included):
+        u[2j] = 2 sum_q x[clamp(j - 3 + q)] f[11 - 2q],  u[2j + 1] = 2 sum_q x[clamp(j - 2 + q)] f[10 - 2q]
+        a[m] = u[m] + sin(u[m] ea)^2 / (eb + 1e-9),        y[t] = sum_k a[clamp(2t - 5 + k)] f[k]
+    (resample.py UpSample1d / DownSample1d and activations.py SnakeBeta on one line each).  Returns (y, bound): the
+    worst-case error of the kernel's fp32 evaluation: 6- and 12-term fma chains (taps within one fp32 rounding of f),
+    the argument u * ea, the two-constant reduction and __sinf (2^-21.41 absolute on [-pi, pi])."""
+    x = np.asarray(x, np.float64)
+    f = np.asarray(taps, np.float64)
+    B, T, C = x.shape
+    a, bt = np.asarray(alpha, np.float64), np.asarray(beta, np.float64)
+    ea, eb = (np.exp(a), np.exp(bt)) if logscale else (a, bt)
+    ib = 1.0 / (eb + 1e-9)
+    cl = lambda i: np.clip(i, 0, T - 1)                                  # noqa: E731
+    j = np.arange(T)
+    u = np.zeros((B, 2 * T, C))
+    um = np.zeros((B, 2 * T, C))
+    for q in range(6):
+        u[:, 0::2] += 2 * x[:, cl(j - 3 + q)] * f[11 - 2 * q]
+        um[:, 0::2] += 2 * np.abs(x[:, cl(j - 3 + q)] * f[11 - 2 * q])
+        u[:, 1::2] += 2 * x[:, cl(j - 2 + q)] * f[10 - 2 * q]
+        um[:, 1::2] += 2 * np.abs(x[:, cl(j - 2 + q)] * f[10 - 2 * q])
+    arg = u * ea
+    s = np.sin(arg)
+    act = u + ib * s * s
+    du = 9 * U * um                                                      # 6 fmas + the tap rounding
+    dsin = 2.0 ** -21.41 + U * (4 * np.abs(arg) + 8) + np.abs(ea) * du   # argument rounding (ea 2 ulp), reduction, __sinf
+    dact = du + ib * (2 * np.abs(s) * dsin + 8 * U * s * s) + U * np.abs(act)
+    y = np.zeros((B, T, C))
+    bound = np.zeros((B, T, C))
+    for k in range(12):
+        m = np.clip(2 * j - 5 + k, 0, 2 * T - 1)
+        y += act[:, m] * f[k]
+        bound += dact[:, m] * abs(f[k]) + 15 * U * np.abs(act[:, m] * f[k])
+    return y, bound
+
+
+def conv_post(x, w, bias, use_tanh):
+    """BigVGAN conv_post on x [B][T][C]: Conv1d(C -> 1, k 7, pad 3) with w [7][C] (+ bias), then tanh or a clamp to
+    [-1, 1], float64.  Returns (y, pre, mag): pre = the conv before the final function, mag = its sum of |terms|."""
+    x = np.asarray(x, np.float64)
+    w = np.asarray(w, np.float64)
+    B, T, C = x.shape
+    b0 = 0.0 if bias is None else float(np.asarray(bias).reshape(-1)[0])
+    pre = np.full((B, T), b0)
+    mag = np.full((B, T), abs(b0))
+    for k in range(7):
+        src = np.arange(T) + k - 3
+        ok = (src >= 0) & (src < T)
+        pre[:, ok] += x[:, src[ok]] @ w[k]
+        mag[:, ok] += np.abs(x[:, src[ok]]) @ np.abs(w[k])
+    y = np.tanh(pre) if use_tanh else np.clip(pre, -1.0, 1.0)
+    return y, pre, mag
+
+
+def cfg_euler(x, vc, vu, dt, rate, zero_rows):
+    """One CFG Euler step of flow_matching.py:96-113, float64: x + dt * ((1 + r) vc - r vu), rows with zero_rows set
+    to 0.  x, vc, vu [T][C]; zero_rows [T] bool.  Returns (out, mag): mag bounds the terms of the fp32 evaluation."""
+    x, vc, vu = (np.asarray(v, np.float64) for v in (x, vc, vu))
+    d = (1.0 + rate) * vc - rate * vu
+    out = x + dt * d
+    mag = np.abs(x) + abs(dt) * ((1.0 + abs(rate)) * np.abs(vc) + abs(rate) * np.abs(vu))
+    z = np.asarray(zero_rows, bool)
+    out[z] = 0.0
+    mag[z] = 0.0
+    return out, mag

@@ -107,3 +107,37 @@ def test_tail_minimal_sizes_vs_oracle(engine):
     with pytest.raises(RuntimeError, match="outside the codebook"):
         engine.codec_decode(np.array([3, cc["codebook_size"] + 7], dtype=np.int32))
     assert engine.codec_decode(np.array([3], dtype=np.int32)).shape[0] == 2      # the engine stays usable afterwards
+
+
+@pytest.mark.parametrize("backend,tol", [(1, 1e-4), (0, 1e-2)])
+def test_dit_forward_one_to_three_frames(engine, backend, tol):
+    """1, 2 and 3 frames, where the WaveNet's reflect padding (encodec.py pad1d) zero-extends a 1- or 2-frame input
+    before it reflects: the DiT against the oracle, and at 1 and 2 frames against the reference golden."""
+    import os
+    from oracle.s2mel import dit_forward, small_codec_cfg, small_s2mel_cfg
+    from tests.test_s2mel_gpu import _load
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "s2mel_short.npz"))
+    c = small_s2mel_cfg()
+    w, _ = _load(engine, c, small_codec_cfg(), int(g["seed_s2mel"]), 4321)
+    engine.set_option("gemm_backend", backend)
+    try:
+        rng = np.random.default_rng(12)
+        for T in (1, 2, 3):
+            if T < 3:
+                mu, style, z, t = (g[f"dit{T}_{k}"] for k in ("mu", "style", "z", "t"))
+            else:
+                mu = rng.standard_normal((1, T, c["content_dim"])).astype(np.float32)
+                style = rng.standard_normal((1, c["style_dim"])).astype(np.float32)
+                z = rng.standard_normal((1, 80, T)).astype(np.float32)
+                t = np.array([0.45], np.float32)
+            px = np.zeros((1, 80, T), np.float32)
+            d = engine.dit_forward(z, px, t, style, mu)
+            ref = dit_forward(w, c, *(torch.from_numpy(a) for a in (z, px)), torch.LongTensor([T]),
+                              torch.from_numpy(t), torch.from_numpy(style), torch.from_numpy(mu)).numpy()
+            err = np.abs(d - ref).max()
+            print(f"[backend {backend}] DiT T={T}: max err vs oracle {err:.2e}")
+            assert np.all(np.isfinite(d)) and err < tol
+            if T < 3:
+                assert np.abs(d - g[f"dit{T}"]).max() < tol
+    finally:
+        engine.set_option("gemm_backend", 0)

@@ -1,5 +1,6 @@
 """CPU: the float64 kernel references of tests/kernel_refs.py against PyTorch and the oracle, at small shapes."""
 import math
+import os
 
 import numpy as np
 import torch
@@ -134,3 +135,95 @@ def test_pair_epilogue_references():
     np.testing.assert_allclose(kr.swiglu(a, b), (F.silu(torch.from_numpy(a)) * torch.from_numpy(b)).numpy(), rtol=1e-12, atol=1e-14)
     ta, tc = torch.from_numpy(a), torch.from_numpy(b)
     np.testing.assert_allclose(kr.wn_gate(a, b), (torch.tanh(ta) * torch.sigmoid(tc)).numpy(), rtol=1e-12, atol=1e-14)
+
+
+def test_pad1d_reflect_matches_reference_golden():
+    """pad1d_reflect against the reference's SConv1d (encodec.py pad1d) at 1, 2 and 3 frames, and against F.pad beyond."""
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "s2mel_short.npz"))
+    w, b = torch.from_numpy(g["sconv_weight"]).double(), torch.from_numpy(g["sconv_bias"]).double()
+    for T in (1, 2, 3):
+        x = g[f"sconv_x{T}"][0].T                                        # [T][C]
+        xp = torch.from_numpy(kr.pad1d_reflect(x, 2, 2)).T[None]
+        np.testing.assert_allclose(F.conv1d(xp, w, b).numpy(), g[f"sconv_y{T}"], rtol=1e-5, atol=1e-5)
+    assert kr.pad1d_reflect_rows(2, 2, 2).tolist() == [-1, 1, 0, 1, -1, 1]
+    assert kr.pad1d_reflect_rows(1, 2, 2).tolist() == [-1, -1, 0, -1, -1]
+    for T in (3, 4, 9):
+        x = np.random.default_rng(T).standard_normal((T, 3))
+        want = F.pad(torch.from_numpy(x).T[None], (2, 2), mode="reflect")[0].T.numpy()
+        np.testing.assert_array_equal(kr.pad1d_reflect(x, 2, 2), want)
+
+
+def test_row_norm_references():
+    rng = np.random.default_rng(8)
+    B, T, C = 2, 5, 48
+    x = rng.standard_normal((B * T, C)) * 3 + 1
+    w, b = rng.standard_normal(C), rng.standard_normal(C)
+    m0, m1 = rng.standard_normal(B * C), rng.standard_normal(B * C)
+    xt = torch.from_numpy(x)
+    got, bound = kr.rownorm(x, T, 0, w, b, 1e-6)
+    np.testing.assert_allclose(got, F.layer_norm(xt, (C,), torch.from_numpy(w), torch.from_numpy(b), 1e-6).numpy(), atol=1e-12)
+    assert np.all(bound > 0)
+    ln = F.layer_norm(xt, (C,), None, None, 1e-6).view(B, T, C)
+    sc, sh = torch.from_numpy(m0).view(B, 1, C), torch.from_numpy(m1).view(B, 1, C)
+    got, _ = kr.rownorm(x, T, 0, None, None, 1e-6, m0, m1, C)
+    np.testing.assert_allclose(got, (ln * (1 + sc) + sh).view(B * T, C).numpy(), atol=1e-12)
+    got, _ = kr.rownorm(x, T, 0, None, None, 1e-6, m0[:C], m1[:C], 0)           # one modulation row for every batch entry
+    np.testing.assert_allclose(got, (ln * (1 + sc[:1]) + sh[:1]).view(B * T, C).numpy(), atol=1e-12)
+    rms = xt * torch.rsqrt(xt.pow(2).mean(-1, keepdim=True) + 1e-5) * torch.from_numpy(w)     # gpt_fast RMSNorm
+    got, _ = kr.rownorm(x, T, 1, w, None, 1e-5, m0, m1, C)
+    np.testing.assert_allclose(got, (sc * rms.view(B, T, C) + sh).view(B * T, C).numpy(), atol=1e-12)
+
+
+def test_groupnorm_mish_and_dwconv_references():
+    rng = np.random.default_rng(9)
+    B, T, C, k = 2, 11, 6, 7
+    x = rng.standard_normal((B, T, C)) * 4
+    w, b = rng.standard_normal(C), rng.standard_normal(C)
+    want = F.mish(F.group_norm(torch.from_numpy(x).transpose(1, 2), 1, torch.from_numpy(w), torch.from_numpy(b), 1e-5))
+    np.testing.assert_allclose(kr.gn_mish(x, w, b, 1e-5)[0], want.transpose(1, 2).numpy(), atol=1e-12)
+    wd, bd = rng.standard_normal((C, k)), rng.standard_normal(C)
+    for TT in (1, 2, 3, 11):
+        xs = x[:, :TT]
+        want = F.conv1d(torch.from_numpy(xs).transpose(1, 2), torch.from_numpy(wd)[:, None], torch.from_numpy(bd),
+                        padding=(k - 1) // 2, groups=C).transpose(1, 2).numpy()
+        got, mag = kr.dwconv(xs, wd, bd, k)
+        np.testing.assert_allclose(got, want, atol=1e-12)
+        assert np.all(mag >= np.abs(got) - 1e-12)
+
+
+def test_activation1d_matches_oracle():
+    from indextts_b200.synth import kaiser_sinc_filter1d
+    from oracle.bigvgan import activation1d
+    rng = np.random.default_rng(10)
+    filt = kaiser_sinc_filter1d(0.25, 0.3, 12).double()
+    for T, logscale in ((1, True), (2, False), (7, True), (40, True)):
+        B, C = 2, 5
+        x = rng.standard_normal((B, T, C)) * 2
+        alpha, beta = rng.standard_normal(C) * 0.5, rng.standard_normal(C) * 0.5
+        if not logscale:
+            alpha, beta = np.abs(alpha) + 0.2, np.abs(beta) + 0.2
+        got, bound = kr.activation1d(x, alpha, beta, filt.reshape(-1).numpy(), logscale)
+        want = activation1d(torch.from_numpy(x).transpose(1, 2), torch.from_numpy(alpha), torch.from_numpy(beta),
+                            filt.view(1, 1, -1), logscale).transpose(1, 2).numpy()
+        np.testing.assert_allclose(got, want, rtol=1e-12, atol=1e-12)
+        assert np.all(bound > 0)
+
+
+def test_conv_post_and_cfg_euler_references():
+    rng = np.random.default_rng(11)
+    B, T, C = 2, 9, 5
+    x = rng.standard_normal((B, T, C))
+    w, bias = rng.standard_normal((7, C)), rng.standard_normal(1)
+    pre = F.conv1d(torch.from_numpy(x).transpose(1, 2), torch.from_numpy(w.T.copy())[None], torch.from_numpy(bias), padding=3)
+    for use_tanh in (0, 1):
+        got, p, mag = kr.conv_post(x, w, bias, use_tanh)
+        np.testing.assert_allclose(p, pre[:, 0].numpy(), atol=1e-12)
+        np.testing.assert_allclose(got, (torch.tanh(pre) if use_tanh else pre.clamp(-1, 1))[:, 0].numpy(), atol=1e-12)
+        assert np.all(mag >= np.abs(p) - 1e-12)
+    # flow_matching.py:96-113: dphi = (1 + r) * cond - r * uncond ; x = x + dt * dphi ; x[:, :, :P] = 0
+    xs, vc, vu = rng.standard_normal((3, 10, 4))
+    zero = np.arange(10) < 3
+    got, _ = kr.cfg_euler(xs, vc, vu, 0.125, 0.7, zero)
+    want = xs + 0.125 * ((1 + 0.7) * vc - 0.7 * vu)
+    want[:3] = 0
+    np.testing.assert_allclose(got, want, atol=1e-14)

@@ -36,3 +36,20 @@ def test_weight_norm_fold():
     w = fold_weight_norm({"c.weight_g": gg, "c.weight_v": v, "c.bias": torch.zeros(6)})
     ref = torch._weight_norm(v, gg, 0)
     assert torch.allclose(w["c.weight"], ref, atol=1e-6) and "c.bias" in w and "c.weight_v" not in w
+
+
+def test_short_sequences_match_reference_golden():
+    """1- and 2-frame inputs, where the WaveNet's reflect padding (encodec.py pad1d) zero-extends before it reflects:
+    the oracle's SConv1d and one small-dims DiT evaluation against the reference modules."""
+    from oracle.s2mel import _reflect_conv
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "s2mel_short.npz"))
+    w, b = torch.from_numpy(g["sconv_weight"]), torch.from_numpy(g["sconv_bias"])
+    for T in (1, 2, 3):
+        y = _reflect_conv(torch.from_numpy(g[f"sconv_x{T}"]), w, b, 5)
+        assert np.abs(y.numpy() - g[f"sconv_y{T}"]).max() < 1e-5
+    c = small_s2mel_cfg()
+    wd = fold_weight_norm(make_s2mel_weights(c, seed=int(g["seed_s2mel"])))
+    for T in (1, 2):
+        mu, style, z, t = (torch.from_numpy(g[f"dit{T}_{k}"]) for k in ("mu", "style", "z", "t"))
+        d = dit_forward(wd, c, z, torch.zeros(1, 80, T), torch.LongTensor([T]), t, style, mu)
+        assert np.abs(d.numpy() - g[f"dit{T}"]).max() < 2e-4

@@ -222,3 +222,80 @@ def test_varlen_flash_attention_does_not_leak(engine, B, H):
         out, out16 = engine.debug_flash_attention_varlen(q, k2, v2, B, H, off)
         assert np.array_equal(out[:, a:b], base[:, a:b]), (u, float(np.abs(out[:, a:b] - base[:, a:b]).max()))
         assert np.array_equal(out16[:, a:b], base16[:, a:b]), u
+
+
+# ------------------------------------------------------------------------------ short utterances, long batches --
+def test_one_and_two_frame_utterances_against_the_oracle_tail(engine):
+    """P = 0 and F = 1 or 2: the WaveNet's reflect padding zero-extends such a sequence (encodec.py pad1d) before it
+    reflects.  idx_codes_to_wav (strict fp32 back end) against the oracle chain of tests/test_zz_tail_wiring.py."""
+    from oracle.bigvgan import bigvgan_forward
+    from oracle.s2mel import cfm_inference, codec_decode, length_regulate
+    from oracle.s2mel import fold_weight_norm as oracle_fold
+    c, cc = _load(engine, full=False)
+    h = synth.small_config()
+    wsf, wcf = oracle_fold(synth.make_s2mel_weights(c, 1234)), oracle_fold(synth.make_codec_weights(cc, 4321))
+    wb = synth.make_bigvgan_weights(h, 1)
+    for F in (1, 2):
+        u = _utterance(300 + F, 0, 1, F, cc["codebook_size"], c["content_dim"])
+        cond = length_regulate(wsf, codec_decode(wcf, torch.from_numpy(u["codes"]).long()[None]), F)
+        mel_ref = cfm_inference(wsf, c, cond, torch.LongTensor([F]), torch.zeros(1, 80, 0),
+                                torch.from_numpy(u["style"])[None], torch.from_numpy(u["z"])[None], 25, 0.7)
+        wav_ref = bigvgan_forward(h, wb, mel_ref.float()).reshape(-1).numpy()
+        engine.set_option("gemm_backend", 1)
+        try:
+            res = engine.codes_to_wav(u["codes"], u["prompt_condition"], u["ref_mel"], u["style"], u["z"], F, 25, 0.7,
+                                      want_wav=True, want_mel=True)
+        finally:
+            engine.set_option("gemm_backend", 0)
+        dmel = float(np.abs(res["mel"] - mel_ref[0].numpy()).max())
+        dwav = float(np.abs(res["wav"] - wav_ref).max())
+        print(f"P=0 F={F}: max |dmel| vs oracle {dmel:.2e} (max |mel| {float(mel_ref.abs().max()):.2f}), max |dwav| {dwav:.2e}")
+        assert np.isfinite(res["mel"]).all() and dmel < 1e-3 and dwav < 1e-3
+
+
+def test_short_utterances_in_a_packed_batch_do_not_see_their_neighbours(engine):
+    """A 1-frame and a 2-frame utterance between long ones: new codes and noise for the neighbours, same lengths, and the
+    short utterances' mel does not move by a bit (a reflect read past a 1- or 2-frame segment lands in its neighbour)."""
+    c, cc = _load(engine, full=False)
+    long_ = [(40, 20, 68), (0, 40, 137), (30, 12, 41)]
+    short = [_utterance(400, 0, 1, 1, cc["codebook_size"], c["content_dim"]),
+             _utterance(401, 0, 1, 2, cc["codebook_size"], c["content_dim"])]
+    kw = dict(want_wav=True, want_pcm16=True, want_mel=True)
+    mels = []
+    for seed in (500, 600):
+        nb = [_utterance(seed + i, P, nc, F, cc["codebook_size"], c["content_dim"]) for i, (P, nc, F) in enumerate(long_)]
+        batch = engine.codes_to_wav_batch([nb[0], short[0], nb[1], short[1], nb[2]], 25, 0.7, **kw)
+        mels.append((batch[1]["mel"], batch[3]["mel"], batch[0]["mel"]))
+    assert not np.array_equal(mels[0][2], mels[1][2])            # the neighbours did change
+    for i, F in ((0, 1), (1, 2)):
+        a, b = mels[0][i], mels[1][i]
+        assert a.shape == (80, F) and np.isfinite(a).all()
+        assert np.array_equal(a, b), (F, float(np.abs(a - b).max()))
+        solo = engine.codes_to_wav(*(short[i][k] for k in ("codes", "prompt_condition", "ref_mel", "style", "z", "F")), 25, 0.7,
+                                   want_mel=True)["mel"]
+        # below 32 frames the solo call runs its fp32 input GEMMs on the SIMT kernel, the packed solve on tf32 (module doc)
+        print(f"{F}-frame utterance: bitwise unchanged by its neighbours; max |packed - solo| {float(np.abs(a - solo).max()):.2e}")
+        assert np.abs(a - solo).max() < 2e-2
+
+
+def test_batch_longer_than_65535_packed_frames(engine):
+    """One packed solve over more than 65 535 frames (the grid-y limit of a one-block-per-row launch): its first and last
+    utterances equal their solo calls."""
+    c, cc = _load(engine, full=False)
+    spec = [(20, 30, 500)] + [(0, 40, 16500)] * 4 + [(10, 25, 300)]
+    utts = [_utterance(700 + i, P, nc, F, cc["codebook_size"], c["content_dim"]) for i, (P, nc, F) in enumerate(spec)]
+    assert sum(P + F for P, _, F in spec) > 65535
+    kw = dict(want_wav=True, want_pcm16=True, want_mel=True)
+    batch = engine.codes_to_wav_batch(utts, 25, 0.7, **kw)
+    for i in (1, 2, 3, 4):
+        assert np.isfinite(batch[i]["mel"]).all()
+    for i in (0, len(utts) - 1):
+        u, b = utts[i], batch[i]
+        solo = engine.codes_to_wav(u["codes"], u["prompt_condition"], u["ref_mel"], u["style"], u["z"], u["F"], 25, 0.7, **kw)
+        dmel = float(np.abs(b["mel"] - solo["mel"]).max())
+        dwav = float(np.sqrt(((b["wav"] - solo["wav"]) ** 2).mean()))
+        same = all(np.array_equal(np.asarray(solo[k]), np.asarray(b[k])) for k in ("mel", "wav", "pcm16"))
+        print(f"[{sum(P + F for P, _, F in spec)} packed frames] utterance {i}: bitwise equal to its solo call: {same}; "
+              f"max |dmel| {dmel:.3e}, wav rms diff {dwav:.3e}")
+        assert dmel <= 1e-5 * float(np.abs(solo["mel"]).max()) and dwav <= 1e-6
+        assert np.array_equal(b["pcm16"], solo["pcm16"])
