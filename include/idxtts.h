@@ -194,6 +194,29 @@ int idx_emo_init(idx_engine* e, const idx_emo_config* cfg);
 int idx_merge_emovec(idx_engine* e, const float* spk_feats, int Ts, const float* emo_feats, int Te,
                      float alpha, float* emo_vec_out);
 
+/* w2v-BERT 2.0 semantic encoder of IndexTTS2.get_emb (infer_v2_5.py:281-290, SURVEY section 8 row f1): the feature
+ * projection and the first `layers` conformer layers of transformers' Wav2Vec2BertModel (relative_key attention), output
+ * (hidden_states[layers] - semantic_mean) / semantic_std.  Tensors are registered under "semantic." with the HF names
+ * (feature_projection.*, encoder.layers.N.*) plus semantic.semantic_mean and semantic.semantic_std [hidden].          */
+typedef struct {
+  int32_t feat_dim;      /* 160 (SeamlessM4TFeatureExtractor: 80 fbank bins x 2 stacked frames)                 */
+  int32_t hidden;        /* 1024                                                                                */
+  int32_t heads;         /* 16 (head size must be 64)                                                           */
+  int32_t ffn;           /* intermediate_size 4096                                                              */
+  int32_t layers;        /* layers to run: 17 for get_emb's hidden_states[17]                                   */
+  int32_t conv_kernel;   /* conv_depthwise_kernel_size 31 (at most 31)                                          */
+  int32_t left_max;      /* left_max_position_embeddings 64                                                     */
+  int32_t right_max;     /* right_max_position_embeddings 8 (left_max + right_max + 1 <= 80)                    */
+  float eps;             /* layer_norm_eps 1e-5                                                                 */
+} idx_semantic_config;
+int idx_semantic_init(idx_engine* e, const idx_semantic_config* cfg);
+/* feats [B, T, feat_dim] f32 (input_features), lens [B] i32 (the number of ones of each prefix attention_mask row,
+ * 1..T) -> out [B, T, hidden] f32.  Rows t >= lens[b] are masked as the HF encoder masks them; they are computed
+ * like HF computes them.  Defaults: fp16 GEMM operands, fp32 accumulate and residual stream; gemm_backend 1 or
+ * IDX_NO_TC: strict fp32.  The tail options (tail_f16, IDX_TAIL_F16, IDX_FA_WGMMA, IDX_ATTN_UNFUSED) do not apply.
+ * Errors: head size != 64, left_max + right_max + 1 > 80 (at init) or a length outside 1..T -> IDX_ERR_ARG.          */
+int idx_semantic_encode(idx_engine* e, const float* feats, const int32_t* lens, int B, int T, float* out);
+
 /* ---- IndexTTS v1 / v1.5 GPT side (SURVEY section 8 row a13, indextts/gpt/model.py) ------------------------------
  * Prompt encoder: ConformerEncoder(100-bin mel, conv2d2) + PerceiverResampler(n_latents = 32) -> conds
  * (get_conditioning, model.py:493-503); tensors "gpt.conditioning_encoder.*", "gpt.perceiver_encoder.*".           */
@@ -355,6 +378,19 @@ int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, const uint16_t
  * strictly increasing) and attends to its own keys only.  out / out16 / guard as in idx_debug_flash_attention.       */
 int idx_debug_flash_attention_varlen(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16, int B,
                                      int H, const int32_t* seg_off, int n_seg, long long guard, float* out, uint16_t* out16);
+
+/* Diagnostic (tests): the encoder's attention kernel (wgmma flash attention with relative_key positions) on fp16 q (already
+ * scaled by log2(e)/8), k, v [B*H][T][64] and E16 [left + right + 1][64] fp16; keys j >= lens[b] masked.  q E^T is
+ * computed from q16 as the encoder computes it.  out16 [B][T][H*64] fp16 with `guard` caller elements on both sides.     */
+int idx_debug_flash_attention_relkey(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16,
+                                     const uint16_t* E16, const int32_t* lens, int B, int T, int H, int left, int right,
+                                     long long guard, uint16_t* out16);
+/* Diagnostic (tests): the encoder's fused conv-module kernel: x [B][T][2C] (pointwise_conv1 output) -> GLU -> causal
+ * depthwise conv (dw [C][kernel], rows >= lens[b] zero) -> LayerNorm (ln_w, ln_b, eps) -> swish -> out [B][T][C] f32
+ * and / or out16 fp16.  Each entry's rows are staged between 8 rows of NaN; outputs carry `guard` caller elements.       */
+int idx_debug_conv_module(idx_engine* e, const float* x, const int32_t* lens, const float* dw, const float* ln_w,
+                          const float* ln_b, float eps, int B, int T, int C, int kernel, long long guard, float* out,
+                          uint16_t* out16);
 
 /* Diagnostic (tests): one of the tail's non-GEMM kernels, run through the host function the model calls (op below).
  * x, x2, x3 and x16 are row-indexed inputs: the entry stages each whole [B][rows][C] block with 8 rows of NaN before and

@@ -59,24 +59,6 @@ __global__ void relpos_split_kernel(const float* __restrict__ qkv, const float* 
     Vt[((long long)h * dk + i) * Tp + t] = vv;
   }
 }
-__global__ void softmax_rows_g_kernel(float* __restrict__ S, long long rows, int T, int Tp) {
-  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  float* r = S + row * Tp;
-  float mx = -INFINITY;
-  for (int i = lane; i < T; i += 32) mx = fmaxf(mx, r[i]);
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  float sum = 0.f;
-  for (int i = lane; i < T; i += 32) { const float p = expf(r[i] - mx); r[i] = p; sum += p; }
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float inv = 1.f / sum;
-  for (int i = lane; i < Tp; i += 32) r[i] = (i < T) ? r[i] * inv : 0.f;
-}
-__global__ void heads_merge_g_kernel(const float* __restrict__ O, float* __restrict__ out, int T, int H, int dk) {
-  const int t = blockIdx.x, h = blockIdx.y;
-  for (int i = threadIdx.x; i < dk; i += blockDim.x) out[(long long)t * H * dk + h * dk + i] = O[((long long)h * T + t) * dk + i];
-}
 __global__ void glu_kernel(const float* __restrict__ x, float* __restrict__ y, long long rows, int C) {
   // F.glu(dim=channels): first half * sigmoid(second half)  (conformer_encoder.py:151-152)
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -184,7 +166,7 @@ void emo_destroy(EmoState* s) {
 }
 
 // stack q,k,v linears into one [3*od][od] packed weight
-static PackedW pack3(idx_engine* e, WeightPool& pool, const std::string& a, const std::string& b, const std::string& c) {
+PackedW pack3(idx_engine* e, WeightPool& pool, const std::string& a, const std::string& b, const std::string& c) {
   const DevTensor& wa = e->W(a + ".weight");
   const int od = (int)wa.shape[0], K = (int)wa.shape[1];
   std::vector<float> h((size_t)3 * od * K), hb((size_t)3 * od);
@@ -340,14 +322,12 @@ static void cond_encode_dev(idx_engine* e, EmoState* s, const float* d_x, int T,
     g1.M = T2; g1.N = T2; g1.out = S; g1.ldo = Tp; g1.out_batch_stride = (long long)T2 * Tp;
     g1.scale = 1.0f / sqrtf((float)dk);               // (ac + bd) / sqrt(d_k)  (attention.py:307-308)
     conv_gemm(e, g1);
-    softmax_rows_g_kernel<<<(unsigned)(((long long)H * T2 + 7) / 8), 256, 0, e->stream>>>(S, (long long)H * T2, T2, Tp);
-    KCHECK(e);
+    softmax_rows_exact(e, S, (long long)H * T2, T2, Tp);
     ConvGemm g2;
     g2.A = S; g2.B = H; g2.Tin = T2; g2.K = Tp; g2.Wk = Vt; g2.w_batch_stride = (long long)dk * Tp;
     g2.M = T2; g2.N = dk; g2.out = O;
     conv_gemm(e, g2);
-    heads_merge_g_kernel<<<dim3(T2, H), 128, 0, e->stream>>>(O, att, T2, H, dk);
-    KCHECK(e);
+    heads_merge(e, O, att, 1, T2, H, dk);
     { ConvGemm g = gemm_of(b.out, att, 1, T2, y); g.res = y; conv_gemm(e, g); }
     // convolution module (conformer_encoder.py:113-167)
     layernorm(e, y, hbuf, 1, T2, od, b.n_conv_w, b.n_conv_b, 1e-5f, nullptr, nullptr, 0);

@@ -127,6 +127,7 @@ void idx_destroy(idx_engine* e) {
   if (e->s2mel) s2mel_destroy(e->s2mel);
   if (e->emo) emo_destroy(e->emo);
   if (e->v1cond) emo_destroy(e->v1cond);
+  if (e->semantic) semantic_destroy(e->semantic);
   if (e->v1voc) v1voc_destroy(e->v1voc);
   for (auto& kv : e->weights) cudaFree(kv.second.d);
   for (auto ev : e->events) if (ev) cudaEventDestroy(ev);

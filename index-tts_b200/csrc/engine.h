@@ -55,6 +55,7 @@ struct EmoState;      // emo.cu
 struct V1VocoderState; // bigvgan.cu (latent-conditioned BigVGAN + ECAPA-TDNN, row a13)
 struct BigvganState;  // bigvgan.cu
 struct S2melState;    // s2mel.cu
+struct SemanticState; // semantic.cu
 
 // Bump allocator for per-call activations: reset at the start of each forward call.
 struct Arena {
@@ -99,6 +100,7 @@ struct idx_engine {
   EmoState* emo = nullptr;
   EmoState* v1cond = nullptr;   // v1 prompt encoder (32-latent conformer-perceiver)
   V1VocoderState* v1voc = nullptr;
+  SemanticState* semantic = nullptr;   // w2v-BERT 2.0 prompt encoder (get_emb)
 
   const DevTensor& W(const std::string& name) const {
     auto it = weights.find(name);
@@ -131,6 +133,7 @@ void bigvgan_destroy(BigvganState*);
 void s2mel_destroy(S2melState*);
 void emo_destroy(EmoState*);
 void v1voc_destroy(V1VocoderState*);
+void semantic_destroy(SemanticState*);
 
 #define IDX_API_BEGIN try {
 #define IDX_API_END(e)                                     \

@@ -371,6 +371,11 @@ void launch_bn(idx_engine* e, const ConvGemm& g, const CUtensorMap& tmA, const C
 // VARLEN: several sequences packed along T (the batched CFM solve).  CTA x takes query tile tiles[x] = (first query row,
 // segment start, segment end), which lies inside one segment; its key tiles start at the segment start, so they align as in
 // a solo run of that sequence, keys at or past the segment end are masked and query rows at or past it are not stored.
+// RELKEY: the w2v-BERT encoder's attention (transformers wav2vec2_bert, position_embeddings_type "relative_key").  Keys at
+// or past lens[b] are masked (the padding mask; every query row of the T is stored), and query row i adds
+// qe[bh][i][clamp(j - i, -rel_l, rel_r) + rel_l] to its score against key j, where qe = Q E^T was computed from the same
+// pre-scaled fp16 q, so it lands in the log2 domain of S.  A key tile wholly left (right) of a row's band adds the row's
+// constant qe[..][0] (qe[..][rel_l + rel_r]); only the tiles that cross the band gather.
 constexpr int FA_Q = 128, FA_K = 128, FA_D = 64;
 constexpr int FA_THREADS = 288;
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -382,9 +387,30 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);
   return *(uint32_t*)&h;
 }
-struct FaParams { int T, H; float* out; __half* out16; const int4* tiles; };
-
-template <bool VARLEN>
+struct FaParams {
+  int T, H; float* out; __half* out16; const int4* tiles;
+  const int* lens; const float* qe; int rel_l, rel_r;    // RELKEY only
+};
+// RELKEY: adds the relative-position term to the elements of S that belong to query row r (SEL 0: S[4c], S[4c + 1]; SEL 2:
+// S[4c + 2], S[4c + 3]); element 4c + SEL + i is key k0 + 8c + 2 t4 + i.  qr = row r of qe [80], staged in shared memory
+// (32-bit addresses: the gathers then fit next to S, O and P in the 168 registers of this kernel).
+template <int SEL>
+__device__ __forceinline__ void fa_add_relkey(float (&S)[FA_K / 2], const float* qr, int r, int k0, int t4, int L, int R) {
+  if (k0 + FA_K - 1 - r <= -L || k0 - r >= R) {
+    const float c = qr[k0 - r >= R ? L + R : 0];
+#pragma unroll
+    for (int c8 = 0; c8 < FA_K / 8; ++c8) { S[4 * c8 + SEL] += c; S[4 * c8 + SEL + 1] += c; }
+  } else {
+#pragma unroll
+    for (int c8 = 0; c8 < FA_K / 8; ++c8) {
+      const int d = k0 + 8 * c8 + 2 * t4 - r;
+      S[4 * c8 + SEL] += qr[min(max(d, -L), R) + L];
+      S[4 * c8 + SEL + 1] += qr[min(max(d + 1, -L), R) + L];
+    }
+  }
+}
+constexpr int FA_QE = 80;              // RELKEY: floats per row of qe (left + right + 1 <= 80)
+template <bool VARLEN, bool RELKEY = false>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                 const FaParams p) {
@@ -414,6 +440,10 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     q0 = tl.x; kbeg = tl.y; kend = tl.z;
     ntiles = (kend - kbeg + FA_K - 1) / FA_K;
   }
+  if constexpr (RELKEY) {
+    kend = p.lens[bh / p.H];
+    ntiles = (kend + FA_K - 1) / FA_K;
+  }
 
   if (warp == 8) {
     if (lane == 0) {
@@ -439,6 +469,14 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
   for (int i = 0; i < FA_D / 2; ++i) O[i] = 0.f;
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running row max (log2 domain), this thread's share of the row sum
+  if constexpr (RELKEY) {
+    // this tile's 128 rows of qe into shared memory (rows past T repeat row T - 1; they are not stored)
+    float* sqe = (float*)(base + 5 * TILE + 64);
+    const float* qe = p.qe + (size_t)bh * T * FA_QE;
+    for (int i = threadIdx.x; i < FA_Q * FA_QE; i += 256)
+      sqe[i] = __ldg(qe + (size_t)min(q0 + i / FA_QE, T - 1) * FA_QE + i % FA_QE);
+    ptx::named_bar_sync(1, 256);
+  }
   ptx::mbar_wait(q_full, 0);
   const uint64_t dq = ptx::make_desc_sw128(ptx::smem_u32(sQ + wg * 64 * 128));
   for (int j = 0; j < ntiles; ++j) {
@@ -452,6 +490,11 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_regs(S);
+    if constexpr (RELKEY) {
+      const float* sqe = (const float*)(base + 5 * TILE + 64);
+      fa_add_relkey<0>(S, sqe + rA * FA_QE, q0 + rA, j * FA_K, t4, p.rel_l, p.rel_r);
+      fa_add_relkey<2>(S, sqe + (rA + 8) * FA_QE, q0 + rA + 8, j * FA_K, t4, p.rel_l, p.rel_r);
+    }
     // keys beyond the sequence end (zero-filled rows past T, or the next packed sequence) are masked;
     // element 4c + i is key 8c + 2 t4 + (i & 1)
     const int nvalid = kend - kbeg - j * FA_K;
@@ -515,6 +558,7 @@ fa_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const float i0 = l0 > 0.f ? 1.f / l0 : 0.f, i1 = l1 > 0.f ? 1.f / l1 : 0.f;
   const int b = bh / p.H, h = bh % p.H;
   const int t0 = q0 + rA, t1 = t0 + 8;
+  if constexpr (RELKEY) kend = T;                 // masked keys, but every query row is stored
   const size_t o0 = ((size_t)b * T + t0) * (size_t)p.H * FA_D + (size_t)h * FA_D;
   const size_t o1 = o0 + (size_t)8 * p.H * FA_D;
 #pragma unroll
@@ -567,6 +611,25 @@ void flash_attention_wgmma_varlen(idx_engine* e, const __half* Qr, const __half*
     e->attr_done |= 1u << 21;
   }
   launch_pdl(e, fa_wgmma_kernel<true>, dim3(sg.fa_tiles, BH), dim3(FA_THREADS), smem, tq, tk, tv, p);
+  e->launches++;
+}
+
+void flash_attention_wgmma_relkey(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, const float* qe,
+                                  const int* lens, int rel_l, int rel_r, __half* out16, int B, int T, int H) {
+  const int BH = B * H;
+  cuuint64_t dims[3] = {(cuuint64_t)FA_D, (cuuint64_t)T, (cuuint64_t)BH};
+  cuuint64_t str[2] = {(cuuint64_t)FA_D * 2, (cuuint64_t)T * FA_D * 2};
+  cuuint32_t box[3] = {FA_D, FA_K, 1};
+  CUtensorMap tq = make_map(Qr, 3, dims, str, box, true), tk = make_map(Kr, 3, dims, str, box, true), tv = make_map(Vb, 3, dims, str, box, true);
+  FaParams p;
+  p.T = T; p.H = H; p.out = nullptr; p.out16 = out16; p.tiles = nullptr;
+  p.lens = lens; p.qe = qe; p.rel_l = rel_l; p.rel_r = rel_r;
+  const size_t smem = 5 * (size_t)(FA_K * FA_D * 2) + 1024 + 64 + (size_t)FA_Q * FA_QE * 4;
+  if (!(e->attr_done & (1u << 22))) {
+    IDX_CUDA(cudaFuncSetAttribute(fa_wgmma_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    e->attr_done |= 1u << 22;
+  }
+  launch_pdl(e, fa_wgmma_kernel<false, true>, dim3((T + FA_Q - 1) / FA_Q, BH), dim3(FA_THREADS), smem, tq, tk, tv, p);
   e->launches++;
 }
 

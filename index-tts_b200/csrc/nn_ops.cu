@@ -836,3 +836,35 @@ void cfg_euler(idx_engine* e, float* x, const float* v_cond, const float* v_unco
   launch_pdl(e, cfg_euler_kernel, dim3((unsigned)(((long long)T * C + 255) / 256)), dim3(256), 0, x, v_cond, v_uncond, dt, rate, T, C, P);
   LAUNCH_CHECK(e);
 }
+
+// ---- the unfused strict-fp32 attention pieces (emotion conformer, w2v-BERT encoder with gemm_backend 1) ----
+namespace {
+// exact-exp row softmax over the first T of Tp columns (columns T..Tp-1 set to 0: the K padding of the P V GEMM)
+__global__ void softmax_rows_g_kernel(float* __restrict__ S, long long rows, int T, int Tp) {
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  float* r = S + row * Tp;
+  float mx = -INFINITY;
+  for (int i = lane; i < T; i += 32) mx = fmaxf(mx, r[i]);
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  float sum = 0.f;
+  for (int i = lane; i < T; i += 32) { const float p = expf(r[i] - mx); r[i] = p; sum += p; }
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  const float inv = 1.f / sum;
+  for (int i = lane; i < Tp; i += 32) r[i] = (i < T) ? r[i] * inv : 0.f;
+}
+__global__ void heads_merge_g_kernel(const float* __restrict__ O, float* __restrict__ out, int T, int H, int dk) {
+  const int t = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  for (int i = threadIdx.x; i < dk; i += blockDim.x)
+    out[((long long)b * T + t) * H * dk + h * dk + i] = O[(((long long)b * H + h) * T + t) * dk + i];
+}
+}  // namespace
+void softmax_rows_exact(idx_engine* e, float* S, long long rows, int T, int Tp) {
+  softmax_rows_g_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, e->stream>>>(S, rows, T, Tp);
+  LAUNCH_CHECK(e);
+}
+void heads_merge(idx_engine* e, const float* O, float* out, int B, int T, int H, int dk) {
+  heads_merge_g_kernel<<<dim3(T, H, B), 128, 0, e->stream>>>(O, out, T, H, dk);
+  LAUNCH_CHECK(e);
+}

@@ -192,6 +192,16 @@ void rope_table_segments(idx_engine* e, float* tab, const Segments& sg, int hd);
 // cfg_euler with the rows listed in zero_rows (1 = prompt frame of its segment) zeroed
 void cfg_euler_rows(idx_engine* e, float* x, const float* v_cond, const float* v_uncond, float dt, float rate, int T, int C,
                     const unsigned char* zero_rows);
+// the unfused fp32 attention (emotion conformer, strict w2v-BERT encoder): exact-exp softmax over the first T of Tp columns of
+// each row (columns T..Tp-1 zeroed), and O [B*H][T][dk] -> out [B][T][H*dk]
+void softmax_rows_exact(idx_engine* e, float* S, long long rows, int T, int Tp);
+void heads_merge(idx_engine* e, const float* O, float* out, int B, int T, int H, int dk);
+// the wgmma flash attention with w2v-BERT's relative_key positions and a key-length mask (see fa_wgmma_kernel, RELKEY):
+// qe [B*H][T][80] = Qr E^T (fp32), lens [B] valid keys (device); out16 [B][T][H*64]
+void flash_attention_wgmma_relkey(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, const float* qe,
+                                  const int* lens, int rel_l, int rel_r, __half* out16, int B, int T, int H);
+// q | k | v Linears of one attention stacked into one [3*od][K] weight with its bias
+PackedW pack3(idx_engine* e, WeightPool& pool, const std::string& a, const std::string& b, const std::string& c);
 // true when the wgmma flash kernel is the default (IDX_FA_WGMMA unset or non-zero)
 bool fa_wgmma_on();
 // fp32 -> fp16 (round to nearest), n elements

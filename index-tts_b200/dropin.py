@@ -13,6 +13,7 @@ weights of its modules with the CUDA engine and rebinds the module-level seams o
     tts.s2mel.models['length_regulator'](…)  → idx_length_regulate                  (length_regulator.py:90-141)
     tts.s2mel.models['cfm'].inference → idx_cfm_solve                               (flow_matching.py:30-115)
     tts.bigvgan(mel)                  → idx_bigvgan_forward                         (bigvgan.py:360-386)
+    tts.get_emb                       → idx_semantic_encode                         (infer_v2_5.py:281-290)
 
 `infer_v2_5.py` itself is not modified: `.infer()` keeps its signature, text front-end, prompt caching,
 segment loop and timing prints, and simply reaches these callables instead of the PyTorch modules.  Tensors
@@ -94,6 +95,38 @@ def load_reference_weights(engine: Engine, tts, max_batch: int = 1):
     return engine
 
 
+# get_emb reads hidden_states[17] of the w2v-BERT 2.0 encoder (infer_v2_5.py:288): the feature projection and the first 17
+# conformer layers; layers 17..23 are never read.
+SEMANTIC_LAYERS = 17
+
+
+def attach_semantic(tts, engine: Engine):
+    """Register the w2v-BERT weights get_emb uses (feature_projection.*, encoder.layers.0..16.*, semantic_mean / std) under
+    "semantic.", size the encoder from the tensors and semantic_model.config, and rebind tts.get_emb to the engine."""
+    sm = tts.semantic_model
+    keep = ("feature_projection.",) + tuple(f"encoder.layers.{i}." for i in range(SEMANTIC_LAYERS))
+    sd = {k: v for k, v in _sd(sm).items() if k.startswith(keep)}
+    sd["semantic_mean"] = torch.as_tensor(tts.semantic_mean).reshape(-1)
+    sd["semantic_std"] = torch.as_tensor(tts.semantic_std).reshape(-1)
+    engine.load_state_dict("semantic.", sd)
+    c = sm.config
+    p = "encoder.layers.0."
+    engine.semantic_init(dict(feat_dim=sd["feature_projection.projection.weight"].shape[1],
+                              hidden=sd["feature_projection.projection.weight"].shape[0], heads=c.num_attention_heads,
+                              ffn=sd[p + "ffn1.intermediate_dense.weight"].shape[0], layers=SEMANTIC_LAYERS,
+                              conv_kernel=sd[p + "conv_module.depthwise_conv.weight"].shape[-1],
+                              left_max=c.left_max_position_embeddings, right_max=c.right_max_position_embeddings,
+                              eps=c.layer_norm_eps))
+    dev = torch.device("cuda", engine.device)
+
+    def get_emb(input_features, attention_mask):
+        # infer_v2_5.py:281-290: (hidden_states[17] - semantic_mean) / semantic_std, [B, T, 1024] on the device
+        return torch.as_tensor(engine.get_emb(input_features, attention_mask)).to(dev)
+
+    tts.get_emb = get_emb
+    return tts
+
+
 def _fresh_seed():
     """A new Philox key per generate call, drawn from torch's global generator: `torch.manual_seed(s)` before `.infer()`
     reproduces a take, and successive calls / segments differ — like the reference's torch.multinomial draws, which
@@ -123,6 +156,8 @@ def attach(tts, engine: Engine = None, device: int = 0):
         raise NotImplementedError("attach() covers indextts.infer_v2_5.IndexTTS2; infer_v2.IndexTTS2 (row f3) is not built")
     engine = engine or Engine(device)
     load_reference_weights(engine, tts, max_batch=4)      # room for the default 3 beams
+    if hasattr(tts, "semantic_model"):
+        attach_semantic(tts, engine)
     dev = torch.device("cuda", engine.device)
     gpt = tts.gpt
 

@@ -71,6 +71,11 @@ class EmoConfig(C.Structure):
                                          "p_heads", "p_dim_head", "p_depth", "p_ff_mult", "model_dim")]
 
 
+class SemanticConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("feat_dim", "hidden", "heads", "ffn", "layers", "conv_kernel", "left_max",
+                                         "right_max")] + [("eps", C.c_float)]
+
+
 class VocodeRequest(C.Structure):
     _fields_ = [("codes", C.c_void_p), ("n_codes", C.c_int32), ("prompt_condition", C.c_void_p),
                 ("ref_mel", C.c_void_p), ("P", C.c_int32), ("style", C.c_void_p), ("z", C.c_void_p),
@@ -228,6 +233,12 @@ def load_library(path: str = None):
     lib.idx_s2mel_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
     lib.idx_emo_init.argtypes = [C.c_void_p, C.POINTER(EmoConfig)]
     lib.idx_merge_emovec.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_void_p]
+    lib.idx_semantic_init.argtypes = [C.c_void_p, C.POINTER(SemanticConfig)]
+    lib.idx_semantic_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+    lib.idx_debug_flash_attention_relkey.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int] * 5 + [C.c_longlong,
+                                                                                                        C.c_void_p]
+    lib.idx_debug_conv_module.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_float] + [C.c_int] * 4 + [
+        C.c_longlong, C.c_void_p, C.c_void_p]
     lib.idx_codes_to_wav.argtypes = [C.c_void_p, C.POINTER(VocodeRequest), C.c_int, C.c_float]
     lib.idx_codes_to_wav_batch.argtypes = [C.c_void_p, C.POINTER(VocodeRequest), C.c_int, C.c_int, C.c_float]
     _lib = lib
@@ -880,3 +891,75 @@ class Engine:
                                               0 if ef is None else int(ef.shape[0]), float(alpha), _ptr(out)),
                     "idx_merge_emovec")
         return out
+
+    # ------------------------------------------------------- w2v-BERT 2.0 semantic encoder (get_emb) --
+    def semantic_init(self, c: dict):
+        """Pack the "semantic.*" tensors (include/idxtts.h idx_semantic_init).  c: feat_dim, hidden, heads, ffn, layers,
+        conv_kernel, left_max, right_max, eps."""
+        cfg = SemanticConfig(*[int(c[k]) for k in ("feat_dim", "hidden", "heads", "ffn", "layers", "conv_kernel", "left_max",
+                                                   "right_max")], float(c["eps"]))
+        self._check(self.lib.idx_semantic_init(self.h, C.byref(cfg)), "idx_semantic_init")
+        self.semantic_cfg = cfg
+
+    @staticmethod
+    def mask_lengths(attention_mask, T):
+        """Valid lengths [B] int32 of a prefix attention mask [B, T] (ones, then zeros); any other mask raises RuntimeError."""
+        m = attention_mask.detach().cpu().numpy() if torch is not None and isinstance(attention_mask, torch.Tensor) \
+            else np.asarray(attention_mask)
+        m = np.asarray(m).reshape(-1, T) != 0
+        lens = m.sum(axis=1).astype(np.int32)
+        if not np.array_equal(m, np.arange(T)[None, :] < lens[:, None]):
+            raise RuntimeError("get_emb: attention_mask rows must be prefixes (ones, then zeros)")
+        return np.ascontiguousarray(lens)
+
+    def get_emb(self, input_features, attention_mask):
+        """IndexTTS2.get_emb (infer_v2_5.py:281-290): input_features [B, T, feat_dim], attention_mask [B, T] (prefix masks)
+        -> (hidden_states[layers] - semantic_mean) / semantic_std [B, T, hidden] float32, a CUDA tensor for CUDA input."""
+        x = _as_f32(input_features)
+        B, T, _ = x.shape
+        lens = self.mask_lengths(attention_mask, T)
+        out = _empty_like_src(x, (B, T, self.semantic_cfg.hidden))
+        self._check(self.lib.idx_semantic_encode(self.h, _ptr(x), _ptr(lens), int(B), int(T), _ptr(out)),
+                    "idx_semantic_encode")
+        return out
+
+    def debug_flash_attention_relkey(self, q16, k16, v16, E16, lens, B, H, left=64, right=8):
+        """The encoder's relative_key flash attention (include/idxtts.h idx_debug_flash_attention_relkey) on fp16 q (scaled
+        by log2(e)/8), k, v [B*H][T][64], E [left + right + 1][64].  Returns out16 [B][T][H*64] fp16."""
+        q16, k16, v16, E16 = (np.ascontiguousarray(x, dtype=np.float16) for x in (q16, k16, v16, E16))
+        ln = np.ascontiguousarray(np.asarray(lens, dtype=np.int32))
+        BH, T, D = q16.shape
+        assert D == 64 and BH == B * H and E16.shape == (left + right + 1, 64) and ln.shape == (B,)
+        n, guard = B * T * H * 64, _guard_len(H * 64)
+        b16 = _guarded(n, guard, np.float16)
+        self._check(self.lib.idx_debug_flash_attention_relkey(
+            self.h, _ptr(q16), _ptr(k16), _ptr(v16), _ptr(E16), _ptr(ln), B, T, H, int(left), int(right), guard,
+            b16.ctypes.data + 2 * guard), "idx_debug_flash_attention_relkey")
+        _check_guard(b16, guard, n, "idx_debug_flash_attention_relkey")
+        return b16[guard:guard + n].view(np.float16).reshape(B, T, H * 64).copy()
+
+    def debug_conv_module(self, x, lens, dw, ln_w, ln_b, eps=1e-5, out=True, out16=True):
+        """The encoder's fused conv-module kernel (include/idxtts.h idx_debug_conv_module): x [B][T][2C] -> (out [B][T][C]
+        f32 or None, out16 fp16 or None)."""
+        x = np.ascontiguousarray(x, dtype=np.float32)
+        B, T, C2 = x.shape
+        Cc = C2 // 2
+        dw = np.ascontiguousarray(np.asarray(dw, dtype=np.float32).reshape(Cc, -1))
+        ln = np.ascontiguousarray(np.asarray(lens, dtype=np.int32))
+        lw, lb = (np.ascontiguousarray(v, dtype=np.float32) for v in (ln_w, ln_b))
+        n, guard = B * T * Cc, _guard_len(Cc)
+        b32 = _guarded(n, guard, np.float32) if out else None
+        b16 = _guarded(n, guard, np.float16) if out16 else None
+        self._check(self.lib.idx_debug_conv_module(
+            self.h, _ptr(x), _ptr(ln), _ptr(dw), _ptr(lw), _ptr(lb), float(eps), B, T, Cc, dw.shape[1], guard,
+            None if b32 is None else b32.ctypes.data + 4 * guard, None if b16 is None else b16.ctypes.data + 2 * guard),
+            "idx_debug_conv_module")
+        res = []
+        for buf in (b32, b16):
+            if buf is None:
+                res.append(None)
+                continue
+            _check_guard(buf, guard, n, "idx_debug_conv_module")
+            dt = np.float32 if buf.dtype == np.uint32 else np.float16
+            res.append(buf[guard:guard + n].view(dt).reshape(B, T, Cc).copy())
+        return tuple(res)
