@@ -428,6 +428,32 @@ typedef struct {
 } idx_debug_tail;
 int idx_debug_tail_op(idx_engine* e, const idx_debug_tail* d);
 
+/* Diagnostic (tests): one kernel of the prompt encoders (the emotion conformer and perceiver, which are also the v1 / v1.5
+ * prompt encoder, and ECAPA's statistics) run through the host function the model calls (op below).  x and x2 are
+ * row-indexed inputs: each is staged between 8 rows of NaN, as in idx_debug_tail.  out carries `guard` caller elements on
+ * both sides (see idx_debug_gemm).
+ *   0 conv2d_sub2:      Conv2d(1 -> n2, 3, stride 2) + ReLU on x [T][C] (C feature bins), w [n2][9], b [n2];
+ *                       out [T2][n2 * Fs] with T2 = (T - 3) / 2 + 1, Fs = (C - 3) / 2 + 1 (the layout embed.out reads)
+ *   1 pos_table:        the sin / cos table of RelPositionalEncoding, out [T][C] (C even); no input
+ *   2 relpos_attention: x = q | k | v [T][3C] (C = heads * dk), x2 = linear_pos(pe) [T][C], w = pos_bias_u, b = pos_bias_v
+ *                       [C]; out [T][C].  backend: 0 the one the model takes, 1 SIMT, 2 tensor core (both GEMMs)
+ *   3 glu:              x [T][2C] -> out [T][C] = first half * sigmoid(second half)
+ *   4 latent_attention: x = q [T][C] (T latents, C = heads * dh), x2 = k | v [n2][2C] -> out [T][C]
+ *   5 geglu:            x [T][2C] (x | gate per row) -> out [T][C] = gelu(gate) * x
+ *   6 l2norm_scale:     x [T][C], w = gamma [C] -> out [T][C] = x / max(|x|, 1e-12) * sqrt(C) * gamma
+ *   7 col_mean_std:     x [T][C] -> out [C] = the mean over T (n2 = 0), or out [2C] = mean | std (n2 = 1)
+ *   8 asp_pool:         x [T][C], x2 = logits [T][C] -> out [2C] = mean | std weighted by softmax over T of the logits */
+typedef struct {
+  int32_t op;
+  int32_t T, C, n2, heads;
+  int32_t backend;
+  const float* x; const float* x2;
+  const float* w; const float* b;
+  int64_t guard;
+  float* out;
+} idx_debug_cond;
+int idx_debug_cond_op(idx_engine* e, const idx_debug_cond* d);
+
 /* ---------------------------------------------------------------- s2mel + codec -- */
 
 /* Geometry of the s2mel section of config.yaml as MyModel reads it

@@ -128,6 +128,15 @@ __global__ void asp_pool_kernel(const float* __restrict__ logit, const float* __
 
 }  // namespace
 
+void ecapa_col_mean_std(idx_engine* e, const float* x, int ld, int T, int C, float* mean, float* std_out) {
+  col_mean_std_kernel<<<(C + 31) / 32, dim3(32, 8), 0, e->stream>>>(x, ld, T, C, mean, std_out);
+  KCHK(e);
+}
+void ecapa_asp_pool(idx_engine* e, const float* logit, const float* x, int T, int C, float* out) {
+  asp_pool_kernel<<<(C + 31) / 32, dim3(32, 8), 0, e->stream>>>(logit, x, T, C, out);
+  KCHK(e);
+}
+
 struct Tdnn {
   PackedW w;
   float *scale = nullptr, *shift = nullptr;   // BatchNorm(eval) after the ReLU
@@ -290,8 +299,7 @@ void ecapa_forward_dev(idx_engine* e, EcapaState* s, const float* d_mel, int T, 
     float* mean = sv;
     float* h1 = sv + Cm;
     float* sc = sv + 2 * Cm;
-    col_mean_std_kernel<<<(C + 31) / 32, dim3(32, 8), 0, e->stream>>>(y2, C, T, C, mean, nullptr);
-    KCHK(e);
+    ecapa_col_mean_std(e, y2, C, T, C, mean, nullptr);
     { ConvGemm g = gemm_of(b.se1, mean, 1, 1, h1); g.act = ACT_RELU; conv_gemm(e, g); }
     conv_gemm(e, gemm_of(b.se2, h1, 1, 1, sc));
     sigmoid_kernel<<<(C + 127) / 128, 128, 0, e->stream>>>(sc, C);
@@ -310,8 +318,7 @@ void ecapa_forward_dev(idx_engine* e, EcapaState* s, const float* d_mel, int T, 
   float* stats = sv;                 // [mean | std] of xm, uniform weights
   float* bvec = sv + 2 * Cm;         // W_stats . [mean | std] + bias  -> per-utterance bias of the attention TDNN
   float* pooled = sv + 2 * Cm + s->att;   // needs 2*Cm floats: sv holds 4*Cm
-  col_mean_std_kernel<<<(Cm + 31) / 32, dim3(32, 8), 0, e->stream>>>(xm, Cm, T, Cm, stats, stats + Cm);
-  KCHK(e);
+  ecapa_col_mean_std(e, xm, Cm, T, Cm, stats, stats + Cm);
   conv_gemm(e, gemm_of(s->asp_stats, stats, 1, 1, bvec));
   {
     ConvGemm g = gemm_of(s->asp_tdnn_x.w, xm, 1, T, att);
@@ -325,8 +332,7 @@ void ecapa_forward_dev(idx_engine* e, EcapaState* s, const float* d_mel, int T, 
     KCHK(e);
   }
   conv_gemm(e, gemm_of(s->asp_conv, att, 1, T, lg));
-  asp_pool_kernel<<<(Cm + 31) / 32, dim3(32, 8), 0, e->stream>>>(lg, xm, T, Cm, pooled);
-  KCHK(e);
+  ecapa_asp_pool(e, lg, xm, T, Cm, pooled);
   col_affine_kernel<<<(2 * Cm + 255) / 256, 256, 0, e->stream>>>(pooled, 2 * Cm, s->bn_scale, s->bn_shift, 1, 2 * Cm);
   KCHK(e);
   conv_gemm(e, gemm_of(s->fc, pooled, 1, 1, d_emb));

@@ -10,6 +10,7 @@
 // result per (speaker, emotion, alpha), so it runs once per reference audio.  All GEMMs go through
 // conv_gemm (wgmma tf32 where the shape allows); lengths follow the reference's all-valid mask (P10).
 #include "ops.h"
+#include "stages.h"
 #include <cmath>
 
 namespace {
@@ -132,6 +133,80 @@ __global__ void lerp_kernel(const float* base, const float* emo, float alpha, fl
 
 }  // namespace
 
+#define KCHECK(e)                  \
+  do {                             \
+    IDX_CUDA(cudaGetLastError());  \
+    (e)->launches++;               \
+  } while (0)
+
+// ---- host launchers of the kernels above: the model and idx_debug_cond_op both go through them ----
+static void conv2d_sub2_relu(idx_engine* e, const float* x, const float* w, const float* b, float* y, int T, int F_, int C) {
+  const int T2 = (T - 3) / 2 + 1, Fs = (F_ - 3) / 2 + 1;
+  conv2d_sub2_relu_kernel<<<dim3((Fs + 127) / 128, T2, C), 128, 0, e->stream>>>(x, w, b, y, T, F_, T2, Fs, C);
+  KCHECK(e);
+}
+static void pos_table(idx_engine* e, float* pe, int T, int d) {
+  pos_table_kernel<<<T, 128, 0, e->stream>>>(pe, T, d);
+  KCHECK(e);
+}
+static void glu(idx_engine* e, const float* x, float* y, long long rows, int C) {
+  glu_kernel<<<(unsigned)((rows * C + 255) / 256), 256, 0, e->stream>>>(x, y, rows, C);
+  KCHECK(e);
+}
+// q [nl][H*dh], kv [n][2*H*dh] (k | v) -> out [nl][H*dh]; the n scores of one (head, latent) live in shared memory
+static void latent_attention(idx_engine* e, const float* q, const float* kv, float* out, int nl, int n, int H, int dh) {
+  IDX_CHECK((size_t)n * 4 <= 48 * 1024, IDX_ERR_ARG, "latent attention: more than 12288 context rows");
+  latent_attn_kernel<<<dim3(H, nl), 128, (size_t)n * 4, e->stream>>>(q, kv, out, n, H, dh);
+  KCHECK(e);
+}
+// x [rows][2N] (x | gate per row) -> y [rows][N]
+static void geglu_rows(idx_engine* e, const float* x, float* y, int rows, int N) {
+  for (int r = 0; r < rows; ++r) {
+    geglu_kernel<<<(N + 127) / 128, 128, 0, e->stream>>>(x + (size_t)r * 2 * N, y + (size_t)r * N, N);
+    KCHECK(e);
+  }
+}
+static void l2norm_scale_rows(idx_engine* e, const float* x, const float* gamma, float* y, int rows, int d) {
+  for (int r = 0; r < rows; ++r) {
+    l2norm_scale_kernel<<<1, 256, 0, e->stream>>>(x + (size_t)r * d, gamma, y + (size_t)r * d, d);
+    KCHECK(e);
+  }
+}
+
+// Scratch of relpos_attention over T rows: A' [H][T][2dk], B' [H][T][2dk], Vt [H][dk][Tp] (its columns >= T stay zero:
+// the K padding of the P V GEMM), S [H][T][Tp], O [H][T][dk]; Tp = T rounded up to 4
+struct RelposBufs { float *Ap, *Bp, *Vt, *S, *O; };
+static RelposBufs relpos_bufs(idx_engine* e, int T, int H, int dk) {
+  const int Tp = (T + 3) & ~3;
+  RelposBufs r;
+  r.Ap = e->arena.get<float>((size_t)H * T * 2 * dk);
+  r.Bp = e->arena.get<float>((size_t)H * T * 2 * dk);
+  r.Vt = e->arena.get<float>((size_t)H * dk * Tp);
+  r.S = e->arena.get<float>((size_t)H * T * Tp);
+  r.O = e->arena.get<float>((size_t)H * T * dk);
+  fill_zero(e, r.Vt, (long long)H * dk * Tp);
+  return r;
+}
+// RelPositionMultiHeadedAttention without rel_shift (attention.py:189-312): qkv [T][3*H*dk] (q | k | v), pp = linear_pos(pe)
+// [T][H*dk], pos_bias_u / pos_bias_v [H*dk] -> att [T][H*dk] = softmax((q+u) k^T + (q+v) p^T) / sqrt(dk)) v per head
+static void relpos_attention(idx_engine* e, const RelposBufs& r, const float* qkv, const float* pp, const float* u,
+                             const float* v, float* att, int T, int H, int dk) {
+  const int Tp = (T + 3) & ~3;
+  relpos_split_kernel<<<dim3(T, H), 128, 0, e->stream>>>(qkv, pp, u, v, r.Ap, r.Bp, r.Vt, T, Tp, H, dk);
+  KCHECK(e);
+  ConvGemm g1;
+  g1.A = r.Ap; g1.B = H; g1.Tin = T; g1.K = 2 * dk; g1.Wk = r.Bp; g1.w_batch_stride = (long long)T * 2 * dk;
+  g1.M = T; g1.N = T; g1.out = r.S; g1.ldo = Tp; g1.out_batch_stride = (long long)T * Tp;
+  g1.scale = 1.0f / sqrtf((float)dk);               // (ac + bd) / sqrt(d_k)  (attention.py:307-308)
+  conv_gemm(e, g1);
+  softmax_rows_exact(e, r.S, (long long)H * T, T, Tp);
+  ConvGemm g2;
+  g2.A = r.S; g2.B = H; g2.Tin = T; g2.K = Tp; g2.Wk = r.Vt; g2.w_batch_stride = (long long)dk * Tp;
+  g2.M = T; g2.N = dk; g2.out = r.O;
+  conv_gemm(e, g2);
+  heads_merge(e, r.O, att, 1, T, H, dk);
+}
+
 struct EmoBlock {
   PackedW qkv, pos, out, w1, w2, pw1, pw2;
   const float *u, *v, *dw_w, *dw_b;
@@ -150,12 +225,6 @@ struct EmoState {
   bool has_heads = true;        // emovec_layer / emo_layer (v2.5 emotion path); the v1 prompt encoder has none
 };
 static EmoState* g_emo_of(idx_engine* e);
-
-#define KCHECK(e)                  \
-  do {                             \
-    IDX_CUDA(cudaGetLastError());  \
-    (e)->launches++;               \
-  } while (0)
 
 static EmoState* g_emo_of(idx_engine* e) { return e->emo; }
 
@@ -288,52 +357,31 @@ static void cond_encode_dev(idx_engine* e, EmoState* s, const float* d_x, int T,
   const int od = c.odim, H = c.heads, dk = od / H;
   const int T2 = (T - 3) / 2 + 1, Fs = (c.idim - 3) / 2 + 1;
   IDX_CHECK(T >= 3 && T2 >= 1, IDX_ERR_ARG, "emotion features too short");
-  const int Tp = (T2 + 3) & ~3;
   float* sub = e->arena.get<float>((size_t)T2 * od * Fs);
   float* y = e->arena.get<float>((size_t)T2 * od);
   float* hbuf = e->arena.get<float>((size_t)T2 * od);
   float* big = e->arena.get<float>((size_t)T2 * std::max(3 * od, std::max(2 * od, c.linear_units)));
   float* pe = e->arena.get<float>((size_t)T2 * od);
   float* pp = e->arena.get<float>((size_t)T2 * od);
-  float* Ap = e->arena.get<float>((size_t)H * T2 * 2 * dk);
-  float* Bp = e->arena.get<float>((size_t)H * T2 * 2 * dk);
-  float* Vt = e->arena.get<float>((size_t)H * dk * Tp);
-  float* S = e->arena.get<float>((size_t)H * T2 * Tp);
-  float* O = e->arena.get<float>((size_t)H * T2 * dk);
   float* att = e->arena.get<float>((size_t)T2 * od);
-  conv2d_sub2_relu_kernel<<<dim3((Fs + 127) / 128, T2, od), 128, 0, e->stream>>>(d_x, s->conv_w, s->conv_b, sub, T, c.idim, T2, Fs, od);
-  KCHECK(e);
+  conv2d_sub2_relu(e, d_x, s->conv_w, s->conv_b, sub, T, c.idim, od);
   {
     ConvGemm g = gemm_of(s->embed_out, sub, 1, T2, y);
     g.scale = sqrtf((float)od);                       // x * xscale (embedding.py:139)
     conv_gemm(e, g);
   }
-  pos_table_kernel<<<T2, 128, 0, e->stream>>>(pe, T2, od);
-  KCHECK(e);
-  fill_zero(e, Vt, (long long)H * dk * Tp);
+  pos_table(e, pe, T2, od);
+  const RelposBufs rb = relpos_bufs(e, T2, H, dk);
   for (auto& b : s->blocks) {
     layernorm(e, y, hbuf, 1, T2, od, b.n_mha_w, b.n_mha_b, 1e-5f, nullptr, nullptr, 0);
     conv_gemm(e, gemm_of(b.qkv, hbuf, 1, T2, big));
     conv_gemm(e, gemm_of(b.pos, pe, 1, T2, pp));
-    relpos_split_kernel<<<dim3(T2, H), 128, 0, e->stream>>>(big, pp, b.u, b.v, Ap, Bp, Vt, T2, Tp, H, dk);
-    KCHECK(e);
-    ConvGemm g1;
-    g1.A = Ap; g1.B = H; g1.Tin = T2; g1.K = 2 * dk; g1.Wk = Bp; g1.w_batch_stride = (long long)T2 * 2 * dk;
-    g1.M = T2; g1.N = T2; g1.out = S; g1.ldo = Tp; g1.out_batch_stride = (long long)T2 * Tp;
-    g1.scale = 1.0f / sqrtf((float)dk);               // (ac + bd) / sqrt(d_k)  (attention.py:307-308)
-    conv_gemm(e, g1);
-    softmax_rows_exact(e, S, (long long)H * T2, T2, Tp);
-    ConvGemm g2;
-    g2.A = S; g2.B = H; g2.Tin = T2; g2.K = Tp; g2.Wk = Vt; g2.w_batch_stride = (long long)dk * Tp;
-    g2.M = T2; g2.N = dk; g2.out = O;
-    conv_gemm(e, g2);
-    heads_merge(e, O, att, 1, T2, H, dk);
+    relpos_attention(e, rb, big, pp, b.u, b.v, att, T2, H, dk);
     { ConvGemm g = gemm_of(b.out, att, 1, T2, y); g.res = y; conv_gemm(e, g); }
     // convolution module (conformer_encoder.py:113-167)
     layernorm(e, y, hbuf, 1, T2, od, b.n_conv_w, b.n_conv_b, 1e-5f, nullptr, nullptr, 0);
     conv_gemm(e, gemm_of(b.pw1, hbuf, 1, T2, big));
-    glu_kernel<<<(unsigned)(((long long)T2 * od + 255) / 256), 256, 0, e->stream>>>(big, hbuf, T2, od);
-    KCHECK(e);
+    glu(e, big, hbuf, T2, od);
     dwconv1d(e, hbuf, att, 1, T2, od, b.dw_w, b.dw_b, c.cnn_kernel);
     layernorm(e, att, hbuf, 1, T2, od, b.cn_w, b.cn_b, 1e-5f, nullptr, nullptr, 0);
     silu_inplace(e, hbuf, (long long)T2 * od);
@@ -361,20 +409,13 @@ static void cond_encode_dev(idx_engine* e, EmoState* s, const float* d_x, int T,
   for (auto& l : s->pl) {
     conv_gemm(e, gemm_of(l.to_q, lat, 1, nl, q));
     conv_gemm(e, gemm_of(l.to_kv, ctx, 1, nl + T2, kv));
-    latent_attn_kernel<<<dim3(c.p_heads, nl), 128, (size_t)(nl + T2) * 4, e->stream>>>(q, kv, ao, nl + T2, c.p_heads, c.p_dim_head);
-    KCHECK(e);
+    latent_attention(e, q, kv, ao, nl, nl + T2, c.p_heads, c.p_dim_head);
     { ConvGemm g = gemm_of(l.to_out, ao, 1, nl, lat); g.res = lat; conv_gemm(e, g); }
     conv_gemm(e, gemm_of(l.ff0, lat, 1, nl, ff));
-    for (int r = 0; r < nl; ++r) {
-      geglu_kernel<<<(di + 127) / 128, 128, 0, e->stream>>>(ff + (size_t)r * 2 * di, fg + (size_t)r * di, di);
-      KCHECK(e);
-    }
+    geglu_rows(e, ff, fg, nl, di);
     { ConvGemm g = gemm_of(l.ff2, fg, 1, nl, lat); g.res = lat; conv_gemm(e, g); }
   }
-  for (int r = 0; r < nl; ++r) {
-    l2norm_scale_kernel<<<1, 256, 0, e->stream>>>(lat + (size_t)r * pd, s->gamma, d_lat_out + (size_t)r * pd, pd);
-    KCHECK(e);
-  }
+  l2norm_scale_rows(e, lat, s->gamma, d_lat_out, nl, pd);
 }
 
 // feats (device [T][idim]) -> emovec (device [model_dim])
@@ -428,6 +469,92 @@ extern "C" int idx_merge_emovec(idx_engine* e, const float* spk_feats, int Ts, c
     KCHECK(e);
   }
   idx_from_device(e, emo_vec_out, out, (size_t)c.model_dim * 4);
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  IDX_API_END(e)
+}
+
+// Diagnostic entry (tests): one kernel of the prompt encoders through the host function the model calls (include/idxtts.h,
+// idx_debug_cond).  Row-indexed inputs sit between NaN guard rows; the output travels with its guard bands.
+extern "C" int idx_debug_cond_op(idx_engine* e, const idx_debug_cond* d) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && d && d->out, IDX_ERR_ARG, "null argument");
+  IDX_CHECK(d->op >= 0 && d->op <= 8, IDX_ERR_ARG, "idx_debug_cond_op: unknown op");
+  IDX_CHECK(d->T > 0 && d->C > 0, IDX_ERR_ARG, "idx_debug_cond_op: bad shape");
+  IDX_CHECK(d->guard >= 0 && d->guard % 8 == 0, IDX_ERR_ARG, "idx_debug_cond_op: guard must be a non-negative multiple of 8");
+  IDX_CHECK(d->backend >= 0 && d->backend <= 2 && (d->op == 2 || d->backend == 0), IDX_ERR_ARG,
+            "idx_debug_cond_op: backend is 0, 1 or 2, and only relpos_attention takes one");
+  const int op = d->op, T = d->T, C = d->C, n2 = d->n2, H = d->heads;
+  // rows and widths of x, x2 and out; sizes of w and b
+  size_t xr = T, xc = C, x2r = 0, x2c = 0, orows = T, ocols = C, nw = 0, nb = 0;
+  switch (op) {
+    case 0:
+      IDX_CHECK(T >= 3 && C >= 3 && n2 > 0, IDX_ERR_ARG, "idx_debug_cond_op: conv2d_sub2 needs T, C >= 3 and n2 channels");
+      orows = (T - 3) / 2 + 1; ocols = (size_t)n2 * ((C - 3) / 2 + 1); nw = 9 * (size_t)n2; nb = n2;
+      break;
+    case 1: IDX_CHECK(C % 2 == 0, IDX_ERR_ARG, "idx_debug_cond_op: pos_table needs an even C"); xr = 0; break;
+    case 2:
+      IDX_CHECK(H > 0 && C % H == 0, IDX_ERR_ARG, "idx_debug_cond_op: C must be heads * dk");
+      xc = 3 * (size_t)C; x2r = T; x2c = C; nw = C; nb = C;
+      break;
+    case 3: case 5: xc = 2 * (size_t)C; break;
+    case 4:
+      IDX_CHECK(H > 0 && C % H == 0 && n2 > 0, IDX_ERR_ARG, "idx_debug_cond_op: latent_attention needs C = heads * dh and n2 rows");
+      x2r = n2; x2c = 2 * (size_t)C;
+      break;
+    case 6: nw = C; break;
+    case 7: IDX_CHECK(n2 == 0 || n2 == 1, IDX_ERR_ARG, "idx_debug_cond_op: col_mean_std takes n2 = 0 or 1"); orows = 1; ocols = n2 ? 2 * (size_t)C : C; break;
+    case 8: x2r = T; x2c = C; orows = 1; ocols = 2 * (size_t)C; break;
+  }
+  IDX_CHECK((xr == 0 || d->x) && (x2r == 0 || d->x2) && (nw == 0 || d->w) && (nb == 0 || d->b), IDX_ERR_ARG,
+            "idx_debug_cond_op: input missing");
+  IDX_CUDA(cudaSetDevice(e->device));
+  constexpr size_t G = 8;                           // NaN guard rows on each side of a row-indexed input
+  const size_t nx = xr * xc, nx2 = x2r * x2c, no = orows * ocols, g2 = 2 * (size_t)d->guard;
+  size_t scratch = 0;
+  if (op == 2) {
+    const size_t dk = C / H, Tp = (T + 3) & ~3;
+    scratch = 4 * ((size_t)H * T * 5 * dk + (size_t)H * dk * Tp + (size_t)H * T * Tp) + 5 * 256;
+  }
+  e->ensure_arena(4 * (nx + 2 * G * xc + nx2 + 2 * G * x2c + nw + nb + no + g2) + scratch + (16 << 20));
+  e->arena.reset();
+  auto stage_rows = [&](const float* src, size_t rows, size_t cols) -> const float* {     // [G NaN rows][rows][G NaN rows]
+    if (!rows) return nullptr;
+    float* p = e->arena.get<float>((rows + 2 * G) * cols);
+    IDX_CUDA(cudaMemsetAsync(p, 0xFF, (rows + 2 * G) * cols * 4, e->stream));        // all-ones: NaN
+    idx_to_device(e, p + G * cols, src, rows * cols * 4);
+    return p + G * cols;
+  };
+  auto stage = [&](const float* src, size_t n) -> const float* {
+    if (!n) return nullptr;
+    float* p = e->arena.get<float>(n);
+    idx_to_device(e, p, src, n * 4);
+    return p;
+  };
+  const float* dx = stage_rows(d->x, xr, xc);
+  const float* dx2 = stage_rows(d->x2, x2r, x2c);
+  const float* dw = stage(d->w, nw);
+  const float* db = stage(d->b, nb);
+  float* dOut = e->arena.get<float>(no + g2);
+  idx_to_device(e, dOut, d->out - d->guard, (no + g2) * 4);
+  float* y = dOut + d->guard;
+  DebugOverrides restore{e};
+  switch (op) {
+    case 0: conv2d_sub2_relu(e, dx, dw, db, y, T, C, n2); break;
+    case 1: pos_table(e, y, T, C); break;
+    case 2: {
+      e->force_backend = d->backend;
+      const RelposBufs r = relpos_bufs(e, T, H, C / H);
+      relpos_attention(e, r, dx, dx2, dw, db, y, T, H, C / H);
+      break;
+    }
+    case 3: glu(e, dx, y, T, C); break;
+    case 4: latent_attention(e, dx, dx2, y, T, n2, H, C / H); break;
+    case 5: geglu_rows(e, dx, y, T, C); break;
+    case 6: l2norm_scale_rows(e, dx, dw, y, T, C); break;
+    case 7: ecapa_col_mean_std(e, dx, C, T, C, y, n2 ? y + C : nullptr); break;
+    case 8: ecapa_asp_pool(e, dx2, dx, T, C, y); break;
+  }
+  idx_from_device(e, d->out - d->guard, dOut, (no + g2) * 4);
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   IDX_API_END(e)
 }

@@ -348,14 +348,6 @@ __global__ void kmajor_to_simt_kernel(const float* wk, float* ws, int N, int KT)
 }
 }  // namespace
 
-namespace {
-// restores the engine's diagnostic overrides however the debug entry leaves
-struct DebugOverrides {
-  idx_engine* e;
-  ~DebugOverrides() { e->force_backend = 0; e->force_tile_n = 0; }
-};
-}  // namespace
-
 // Diagnostic entry (tests): run one multi-tap GEMM through a chosen back end, operand format and tile width
 // (include/idxtts.h, idx_debug_gemm).  Every operand is staged into the arena; out / out16 travel with their guard bands.
 extern "C" int idx_debug_conv_gemm(idx_engine* e, const idx_debug_gemm* d) {

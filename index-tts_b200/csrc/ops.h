@@ -122,6 +122,11 @@ void attention_rope(idx_engine* e, const float* qkv, float* out, int B, int T, i
 void cfg_euler(idx_engine* e, float* x, const float* v_cond, const float* v_uncond, float dt, float rate,
                int T, int C, int P);
 void fill_zero(idx_engine* e, float* x, long long n);
+// restores the engine's diagnostic overrides (force_backend, force_tile_n) however a debug entry leaves
+struct DebugOverrides {
+  idx_engine* e;
+  ~DebugOverrides() { e->force_backend = 0; e->force_tile_n = 0; }
+};
 // y[b][i][:] = x[b][reflect(i - left)][:], i in [0, T + left + right)   (encodec.py pad1d mode='reflect': F.pad's reflection,
 // with an input no longer than max(left, right) zero-extended to max(left, right) + 1 rows first)
 void reflect_pad_rows(idx_engine* e, const float* x, float* y, int B, int T, int C, int left, int right, __half* y16 = nullptr);

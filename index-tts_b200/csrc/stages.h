@@ -54,3 +54,9 @@ void ecapa_destroy(EcapaState* s);
 size_t ecapa_arena_bytes(const EcapaState* s, int T);
 // d_mel [T][n_mels] -> d_emb [emb]
 void ecapa_forward_dev(idx_engine* e, EcapaState* s, const float* d_mel, int T, float* d_emb);
+// per-channel statistics over the T rows of x [T][ld] (columns < C): mean [C] and, when std_out is given,
+// std = sqrt(max(E[(x - mean)^2], 1e-12)) [C]
+void ecapa_col_mean_std(idx_engine* e, const float* x, int ld, int T, int C, float* mean, float* std_out);
+// attentive statistics pooling: per channel c, a = softmax over t of logit[t][c]; out [2C] = sum_t a x | sqrt(max(sum_t a (x -
+// mean)^2, 1e-12)); logit, x [T][C]
+void ecapa_asp_pool(idx_engine* e, const float* logit, const float* x, int T, int C, float* out);

@@ -195,10 +195,17 @@ def attach(tts, engine: Engine = None, device: int = 0):
     if getattr(engine, "emo_cfg", None) is not None:
         def merge_emovec(self, speech_condition, emo_speech_condition, cond_lengths=None, emo_cond_lengths=None, alpha=1.0):
             # model_v2.py:827-838; features [1, T, 1024] (or [1, 1024, T], transposed like get_emo_conditioning :588-593)
-            def feats(x):
+            def feats(x, lengths, what):
                 x = x[0].float()
-                return (x.t() if x.shape[0] == engine.emo_cfg.idim and x.shape[1] != engine.emo_cfg.idim else x).contiguous()
-            v = engine.merge_emovec(feats(speech_condition), feats(emo_speech_condition), float(alpha))
+                x = (x.t() if x.shape[0] == engine.emo_cfg.idim and x.shape[1] != engine.emo_cfg.idim else x).contiguous()
+                # The conformer masks rows at or beyond the given length; the engine encodes every row.  infer_v2_5.py passes
+                # the feature dim (1024, trap P10), which masks nothing for T <= 1024.
+                if lengths is not None and int(torch.as_tensor(lengths).reshape(-1).min()) < x.shape[0]:
+                    raise RuntimeError(f"merge_emovec: {what} {torch.as_tensor(lengths).reshape(-1).tolist()} is below the "
+                                       f"{x.shape[0]} feature rows; the engine does not mask rows")
+                return x
+            v = engine.merge_emovec(feats(speech_condition, cond_lengths, "cond_lengths"),
+                                    feats(emo_speech_condition, emo_cond_lengths, "emo_cond_lengths"), float(alpha))
             return torch.as_tensor(v)[None].to(dev)
 
         gpt.merge_emovec = types.MethodType(merge_emovec, gpt)

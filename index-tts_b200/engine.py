@@ -107,11 +107,20 @@ class DebugTail(C.Structure):
                 ("out", C.c_void_p), ("out16", C.c_void_p)]
 
 
+class DebugCond(C.Structure):
+    """include/idxtts.h idx_debug_cond."""
+    _fields_ = [("op", C.c_int32), ("T", C.c_int32), ("C", C.c_int32), ("n2", C.c_int32), ("heads", C.c_int32),
+                ("backend", C.c_int32), ("x", C.c_void_p), ("x2", C.c_void_p), ("w", C.c_void_p), ("b", C.c_void_p),
+                ("guard", C.c_int64), ("out", C.c_void_p)]
+
+
 _byref = C.byref          # debug_tail_op takes a parameter named C
 
 TAIL_OPS = {"layernorm": 0, "rmsnorm_adaln": 1, "groupnorm1_mish": 2, "dwconv1d": 3, "nearest_interp": 4,
             "reflect_pad_rows": 5, "reflect_pad_segments": 6, "compact_segments16": 7, "cfg_euler": 8,
             "cfg_euler_rows": 9, "rope_table": 10, "snake_act": 11, "conv_post": 12}
+COND_OPS = {"conv2d_sub2": 0, "pos_table": 1, "relpos_attention": 2, "glu": 3, "latent_attention": 4, "geglu": 5,
+            "l2norm_scale": 6, "col_mean_std": 7, "asp_pool": 8}
 
 
 # Guard bands of the diagnostic entries: sentinel NaNs (a payload no kernel produces) on both sides of every output,
@@ -223,6 +232,7 @@ def load_library(path: str = None):
     lib.idx_debug_flash_attention_varlen.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                                      C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]
     lib.idx_debug_tail_op.argtypes = [C.c_void_p, C.POINTER(DebugTail)]
+    lib.idx_debug_cond_op.argtypes = [C.c_void_p, C.POINTER(DebugCond)]
     lib.idx_s2mel_init.argtypes = [C.c_void_p, C.POINTER(S2melConfig)]
     lib.idx_codec_init.argtypes = [C.c_void_p, C.POINTER(CodecConfig)]
     lib.idx_codec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
@@ -874,6 +884,34 @@ class Engine:
             dt_ = np.float32 if buf.dtype == np.uint32 else np.float16
             res.append(buf[guard:guard + n].view(dt_).reshape(shape).copy())
         return tuple(res)
+
+    def debug_cond_op(self, op, x=None, x2=None, w=None, b=None, T=None, C=None, n2=0, heads=0, backend=0):
+        """One kernel of the prompt encoders (include/idxtts.h idx_debug_cond; op is a name of COND_OPS) through the host
+        function the model calls.  x is [T][width] fp32; T defaults to its rows, C to the op's channel count read from
+        its width.  Returns out float32, shaped [rows][cols] ([cols] for col_mean_std and asp_pool); raises AssertionError
+        when the kernel wrote outside it."""
+        code = COND_OPS[op]
+        f32 = lambda v: None if v is None else np.ascontiguousarray(v, dtype=np.float32)   # noqa: E731
+        keep = [f32(x), f32(x2), f32(w), f32(b)]
+        if x is not None:
+            T = keep[0].shape[0] if T is None else T
+            if C is None:
+                C = keep[0].shape[1] // {2: 3, 3: 2, 5: 2}.get(code, 1)
+        if code == 0:
+            rows, cols = (T - 3) // 2 + 1, n2 * ((C - 3) // 2 + 1)
+        elif code in (7, 8):
+            rows, cols = 1, (2 * C if (code == 8 or n2) else C)
+        else:
+            rows, cols = T, C
+        n, guard = rows * cols, _guard_len(cols)
+        buf = _guarded(n, guard, np.float32)
+        d = DebugCond(op=code, T=int(T), C=int(C), n2=int(n2), heads=int(heads), backend=int(backend), guard=guard,
+                      out=buf.ctypes.data + 4 * guard)
+        d.x, d.x2, d.w, d.b = (_ptr(v) for v in keep)
+        self._check(self.lib.idx_debug_cond_op(self.h, _byref(d)), "idx_debug_cond_op")
+        _check_guard(buf, guard, n, "idx_debug_cond_op")
+        out = buf[guard:guard + n].view(np.float32).copy()
+        return out if code in (7, 8) else out.reshape(rows, cols)
 
     # ------------------------------------------------------------------- emotion --
     def emo_init(self, c: dict):

@@ -29,13 +29,40 @@ def _lin(x, w, p):
     return F.linear(x, w[p + ".weight"], w.get(p + ".bias"))
 
 
-def pos_table(T, d):
+def pos_table(T, d, device=None, dtype=None):
+    """RelPositionalEncoding.pe (embedding.py:47-53), computed in fp32 on the CPU as the reference computes it, then moved
+    to `device` / `dtype` (the values do not change)."""
     pe = torch.zeros(T, d)
     position = torch.arange(0, T).unsqueeze(1)
     div = torch.exp(torch.arange(0, d, 2) * -(math.log(10000.0) / d))
     pe[:, 0::2] = torch.sin(position * div)
     pe[:, 1::2] = torch.cos(position * div)
-    return pe
+    return pe.to(device=device, dtype=dtype)
+
+
+def rel_attention(q, k, v, pp, pos_bias_u, pos_bias_v, H):
+    """RelPositionMultiHeadedAttention without rel_shift (attention.py:189-312) after its linears: q, k, v, pp (linear_pos of
+    the table) [T, od] -> [T, od]."""
+    T2, od = q.shape
+    dk = od // H
+    q = q.view(T2, H, dk)
+    k, v, pp = (t.view(T2, H, dk).transpose(0, 1) for t in (k, v, pp))
+    qu = (q + pos_bias_u).transpose(0, 1)
+    qv = (q + pos_bias_v).transpose(0, 1)
+    sc = (qu @ k.transpose(1, 2) + qv @ pp.transpose(1, 2)) / math.sqrt(dk)
+    return (torch.softmax(sc, -1) @ v).transpose(0, 1).reshape(T2, od)
+
+
+def latent_attention(q, kv, hh):
+    """The perceiver's Attention (perceiver.py:224-274) after to_q / to_kv: q [nl, inner], kv [n, 2 inner] -> [nl, inner]."""
+    nl, inner = q.shape
+    dh = inner // hh
+    k, v = kv.chunk(2, -1)
+    qq = q.view(nl, hh, dh).transpose(0, 1)
+    k = k.reshape(-1, hh, dh).transpose(0, 1)
+    v = v.reshape(-1, hh, dh).transpose(0, 1)
+    att = torch.softmax(qq @ k.transpose(1, 2) * dh ** -0.5, -1) @ v
+    return att.transpose(0, 1).reshape(nl, inner)
 
 
 @torch.no_grad()
@@ -43,24 +70,18 @@ def conformer_encode(w, c, x, prefix="emo_conditioning_encoder."):
     """x [T, idim] → [T', odim]  (ConformerEncoder with conv2d2 front-end, rel-pos attention)."""
     e = prefix
     od, H = c["odim"], c["heads"]
-    dk = od // H
     y = F.relu(F.conv2d(x[None, None], w[e + "embed.conv.0.weight"], w[e + "embed.conv.0.bias"], stride=2))
     _, C, T2, Fs = y.shape
     y = y.transpose(1, 2).contiguous().view(1, T2, C * Fs)
     y = _lin(y, w, e + "embed.out.0")[0]
     y = y * math.sqrt(od)
-    pe = pos_table(T2, od)
+    pe = pos_table(T2, od, device=x.device, dtype=x.dtype)
     for i in range(c["blocks"]):
         p = e + f"encoders.{i}."
         h = _ln(y, w, p + "norm_mha")
-        q = _lin(h, w, p + "self_attn.linear_q").view(T2, H, dk)
-        k = _lin(h, w, p + "self_attn.linear_k").view(T2, H, dk).transpose(0, 1)
-        v = _lin(h, w, p + "self_attn.linear_v").view(T2, H, dk).transpose(0, 1)
-        pp = F.linear(pe, w[p + "self_attn.linear_pos.weight"]).view(T2, H, dk).transpose(0, 1)
-        qu = (q + w[p + "self_attn.pos_bias_u"]).transpose(0, 1)
-        qv = (q + w[p + "self_attn.pos_bias_v"]).transpose(0, 1)
-        sc = (qu @ k.transpose(1, 2) + qv @ pp.transpose(1, 2)) / math.sqrt(dk)
-        a = (torch.softmax(sc, -1) @ v).transpose(0, 1).reshape(T2, od)
+        a = rel_attention(_lin(h, w, p + "self_attn.linear_q"), _lin(h, w, p + "self_attn.linear_k"),
+                          _lin(h, w, p + "self_attn.linear_v"), F.linear(pe, w[p + "self_attn.linear_pos.weight"]),
+                          w[p + "self_attn.pos_bias_u"], w[p + "self_attn.pos_bias_v"], H)
         y = y + _lin(a, w, p + "self_attn.linear_out")
         h = _ln(y, w, p + "norm_conv").t()[None]
         h = F.glu(F.conv1d(h, w[p + "conv_module.pointwise_conv1.weight"], w[p + "conv_module.pointwise_conv1.bias"]), dim=1)
@@ -79,20 +100,14 @@ def conformer_encode(w, c, x, prefix="emo_conditioning_encoder."):
 def perceiver_resample(w, c, ctx, prefix="emo_perceiver_encoder.", squeeze=True):
     """ctx [T', odim] → [p_dim] (1 latent; `squeeze=False`: [n_latents, p_dim], the v1 32-latent prompt)."""
     q = prefix
-    hh, dh = c["p_heads"], c["p_dim_head"]
+    hh = c["p_heads"]
     x = _lin(ctx, w, q + "proj_context")
     lat = w[q + "latents"].clone()
     for i in range(c["p_depth"]):
         a = q + f"layers.{i}.0."
         context = torch.cat([lat, x], 0)
-        nl = lat.shape[0]
-        qq = F.linear(lat, w[a + "to_q.weight"]).view(nl, hh, dh).transpose(0, 1)
-        kv = F.linear(context, w[a + "to_kv.weight"])
-        k, v = kv.chunk(2, -1)
-        k = k.view(-1, hh, dh).transpose(0, 1)
-        v = v.view(-1, hh, dh).transpose(0, 1)
-        att = torch.softmax(qq @ k.transpose(1, 2) * dh ** -0.5, -1) @ v
-        lat = F.linear(att.transpose(0, 1).reshape(nl, hh * dh), w[a + "to_out.weight"]) + lat
+        att = latent_attention(F.linear(lat, w[a + "to_q.weight"]), F.linear(context, w[a + "to_kv.weight"]), hh)
+        lat = F.linear(att, w[a + "to_out.weight"]) + lat
         f = q + f"layers.{i}.1."
         h = _lin(lat, w, f + "0")
         xg, gate = h.chunk(2, -1)

@@ -1,5 +1,8 @@
 """Pin oracle/emo.py against the reference ConformerEncoder / PerceiverResampler modules and mint
-tests/golden/emo_small.npz + emo_full.npz (build container only).   python -m oracle.make_goldens_emo"""
+tests/golden/emo_small.npz, emo_full.npz and emo_full_t750.npz (build container only).   python -m oracle.make_goldens_emo
+
+emo_full_t750 is a 15 s prompt (T = 750 feature rows, T' = 374 after the subsampling).  It stores the reference's outputs
+(ctx, latent, emovec) and the seed of the features, not the features: the test re-draws them from the seed."""
 import os
 import sys
 
@@ -13,7 +16,7 @@ from oracle.emo import EMO_CFG, conformer_encode, get_emovec, make_emo_weights, 
 
 
 @torch.no_grad()
-def check(c, T, seed, name):
+def check(c, T, seed, name, store_feats=True):
     refimport.setup()
     from indextts.gpt.conformer_encoder import ConformerEncoder
     from indextts.gpt.perceiver import PerceiverResampler
@@ -43,8 +46,12 @@ def check(c, T, seed, name):
     ev = get_emovec(w, c, feats)
     ev_ref = torch.nn.functional.linear(torch.nn.functional.linear(lat_ref[None], w["emovec_layer.weight"], w["emovec_layer.bias"]),
                                         w["emo_layer.weight"], w["emo_layer.bias"])[0]
-    np.savez_compressed(os.path.join(ROOT, "tests", "golden", name + ".npz"), feats=feats.numpy(), ctx=ctx_ref[0].numpy(),
-                        latent=lat_ref.numpy(), emovec=ev_ref.numpy(), seed=777)
+    out = dict(ctx=ctx_ref[0].numpy(), latent=lat_ref.numpy(), emovec=ev_ref.numpy(), seed=777)
+    if store_feats:
+        out.update(feats=feats.numpy())
+    else:
+        out.update(feats_seed=seed, T=T)
+    np.savez_compressed(os.path.join(ROOT, "tests", "golden", name + ".npz"), **out)
     assert (ev - ev_ref).abs().max() < 5e-4
 
 
@@ -52,4 +59,5 @@ if __name__ == "__main__":
     torch.set_num_threads(8)
     check(small_emo_cfg(), 37, 1, "emo_small")
     check(dict(EMO_CFG), 60, 2, "emo_full")
+    check(dict(EMO_CFG), 750, 3, "emo_full_t750", store_feats=False)
     print("wrote emo goldens")

@@ -40,6 +40,14 @@ def _tdnn(x, w, p, dilation=1):
     return _bn(F.relu(_conv_same(x, w[p + ".conv.conv.weight"], w[p + ".conv.conv.bias"], dilation)), w, p + ".norm")
 
 
+def weighted_stats(x, m):
+    """_compute_statistics of AttentiveStatisticsPooling (ECAPA_TDNN.py:299-304): x [B, C, L], weights m [B, 1 or C, L]
+    summing to 1 over L -> (mean, std) [B, C], std = sqrt(clamp(sum m (x - mean)^2, 1e-12))."""
+    mean = (m * x).sum(2)
+    std = torch.sqrt((m * (x - mean.unsqueeze(2)).pow(2)).sum(2).clamp(1e-12))
+    return mean, std
+
+
 @torch.no_grad()
 def ecapa_tdnn(w, mel, prefix="speaker_encoder.", channels=(512, 512, 512, 512, 1536), kernel_sizes=(5, 3, 3, 3, 1),
                dilations=(1, 2, 3, 4, 1), scale=8):
@@ -74,15 +82,11 @@ def ecapa_tdnn(w, mel, prefix="speaker_encoder.", channels=(512, 512, 512, 512, 
     x = _tdnn(torch.cat(xl[1:], dim=1), w, q + "mfa", dilations[-1])
     # AttentiveStatisticsPooling with global context (:282-338)
     L = x.shape[-1]
-    m = torch.full((x.shape[0], 1, L), 1.0 / L)
-    mean = (m * x).sum(2)
-    std = torch.sqrt((m * (x - mean.unsqueeze(2)).pow(2)).sum(2).clamp(1e-12))
+    mean, std = weighted_stats(x, torch.full((x.shape[0], 1, L), 1.0 / L, dtype=x.dtype, device=x.device))
     attn = torch.cat([x, mean.unsqueeze(2).repeat(1, 1, L), std.unsqueeze(2).repeat(1, 1, L)], dim=1)
     attn = torch.tanh(_tdnn(attn, w, q + "asp.tdnn"))
     attn = F.conv1d(attn, w[q + "asp.conv.conv.weight"], w[q + "asp.conv.conv.bias"])
-    attn = F.softmax(attn, dim=2)
-    mean = (attn * x).sum(2)
-    std = torch.sqrt((attn * (x - mean.unsqueeze(2)).pow(2)).sum(2).clamp(1e-12))
+    mean, std = weighted_stats(x, F.softmax(attn, dim=2))
     pooled = torch.cat((mean, std), dim=1).unsqueeze(2)
     pooled = F.batch_norm(pooled, w[q + "asp_bn.norm.running_mean"], w[q + "asp_bn.norm.running_var"],
                           w[q + "asp_bn.norm.weight"], w[q + "asp_bn.norm.bias"], training=False, eps=1e-5)

@@ -10,6 +10,7 @@ import json
 import os
 import types
 
+import pytest
 import torch
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -151,6 +152,37 @@ def test_rebound_seams_accept_the_reference_call_sites():
                 raise AssertionError(f"{name}: reference call ({npos} positional, keywords {kws}) does not bind to {sig}: {e}")
     # the rebound objects are the reference's own module objects: infer_generator reaches them unchanged
     assert tts.gpt is gpt and tts.bigvgan is bv and tts._b200_engine is eng
+
+
+def test_merge_emovec_refuses_lengths_below_the_feature_rows():
+    """The reference's conformer masks feature rows at or beyond cond_lengths / emo_cond_lengths; the engine encodes every
+    row.  The lengths infer_v2_5.py passes (the feature dim, 1024: trap P10) reach the engine unchanged; a length below
+    the number of rows is refused rather than silently computing something else."""
+    from indextts_b200.dropin import attach
+
+    _, tts = _tts_v2_5()
+
+    class Reached(Exception):
+        """raised by the stand-in engine: the call got through to the engine (no device to return a tensor to here)"""
+
+    class Rec(RecordingEngine):
+        def merge_emovec(self, spk, emo, alpha):
+            self.calls.setdefault("merge_emovec", []).append((tuple(spk.shape), tuple(emo.shape), alpha))
+            raise Reached
+
+    eng = Rec()
+    attach(tts, engine=eng)
+    spk, emo = torch.zeros(1, 64, 1024), torch.zeros(1, 90, 1024)
+    full = torch.tensor([1024])
+    for cl, el, alpha in ((full, full, 0.6), (torch.tensor([64]), torch.tensor([90]), 1.0), (None, None, 1.0)):
+        with pytest.raises(Reached):     # the .infer() lengths, exactly the rows, no lengths: nothing is masked
+            tts.gpt.merge_emovec(spk, emo, cl, el, alpha=alpha)
+    assert eng.calls["merge_emovec"] == [((64, 1024), (90, 1024), 0.6), ((64, 1024), (90, 1024), 1.0),
+                                         ((64, 1024), (90, 1024), 1.0)]
+    for cl, el, what in ((torch.tensor([63]), full, "cond_lengths"), (full, torch.tensor([89]), "emo_cond_lengths")):
+        with pytest.raises(RuntimeError, match=what):
+            tts.gpt.merge_emovec(spk, emo, cl, el)
+    assert len(eng.calls["merge_emovec"]) == 3
 
 
 def test_attach_v1_on_real_reference_v1_modules():

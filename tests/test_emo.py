@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 import torch
 
-from oracle.emo import EMO_CFG, get_emovec, make_emo_weights, merge_emovec, small_emo_cfg
+from oracle.emo import (EMO_CFG, conformer_encode, get_emovec, make_emo_weights, merge_emovec, perceiver_resample,
+                        small_emo_cfg)
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -15,6 +16,21 @@ def test_oracle_matches_reference_golden(name, cfg):
     g = np.load(os.path.join(GOLD, name + ".npz"))
     w = make_emo_weights(cfg, seed=int(g["seed"]))
     ev = get_emovec(w, cfg, torch.from_numpy(g["feats"]))
+    assert np.abs(ev.numpy() - g["emovec"]).max() < 5e-4
+
+
+def test_oracle_matches_reference_golden_at_a_15s_prompt():
+    """The oracle at T = 750 feature rows (T' = 374), where it is the yardstick of tests/test_emo_lengths_gpu.py: the
+    reference modules' ctx, latent and emo_vec, the features re-drawn from the stored seed."""
+    g = np.load(os.path.join(GOLD, "emo_full_t750.npz"))
+    cfg = dict(EMO_CFG)
+    w = make_emo_weights(cfg, seed=int(g["seed"]))
+    feats = torch.randn(int(g["T"]), cfg["idim"], generator=torch.Generator().manual_seed(int(g["feats_seed"])))
+    ctx = conformer_encode(w, cfg, feats)
+    lat = perceiver_resample(w, cfg, ctx)
+    ev = get_emovec(w, cfg, feats)
+    assert ctx.shape == g["ctx"].shape == (374, cfg["odim"])
+    assert np.abs(ctx.numpy() - g["ctx"]).max() < 2e-4 and np.abs(lat.numpy() - g["latent"]).max() < 2e-4
     assert np.abs(ev.numpy() - g["emovec"]).max() < 5e-4
 
 
