@@ -79,7 +79,8 @@ int idx_event_elapsed_ms(idx_engine* e, int slot_a, int slot_b, double* ms);
  * allows — the default), 1 = SIMT fp32 everywhere (strict-fp32 parity runs).  "tail_f16" (with gemm_backend 0): 1 = the
  * DiT / WaveNet / BigVGAN-resblock GEMMs read fp16 operands (kind::f16; activations written as fp16 by the kernel that
  * produces them, fp32 accumulate and fp32 residual streams — the default), 0 = tf32 over fp32 storage (round 1).
- * Options belong to the handle: another engine (another GPU, another thread) keeps its own.        */
+ * Options belong to the handle: another engine (another GPU, another thread) keeps its own.  idx_create starts an engine
+ * at gemm_backend 1 when IDX_NO_TC is set in the environment and at tail_f16 0 when IDX_TAIL_F16=0.        */
 int idx_set_option(idx_engine* e, const char* name, int value);
 
 /* -------------------------------------------------------------------- weights -- */
@@ -212,8 +213,8 @@ typedef struct {
 int idx_semantic_init(idx_engine* e, const idx_semantic_config* cfg);
 /* feats [B, T, feat_dim] f32 (input_features), lens [B] i32 (the number of ones of each prefix attention_mask row,
  * 1..T) -> out [B, T, hidden] f32.  Rows t >= lens[b] are masked as the HF encoder masks them; they are computed
- * like HF computes them.  Defaults: fp16 GEMM operands, fp32 accumulate and residual stream; gemm_backend 1 or
- * IDX_NO_TC: strict fp32.  The tail options (tail_f16, IDX_TAIL_F16, IDX_FA_WGMMA, IDX_ATTN_UNFUSED) do not apply.
+ * like HF computes them.  Defaults: fp16 GEMM operands, fp32 accumulate and residual stream; gemm_backend 1: strict
+ * fp32.  The tail option tail_f16 does not apply.
  * Errors: head size != 64, left_max + right_max + 1 > 80 (at init) or a length outside 1..T -> IDX_ERR_ARG.          */
 int idx_semantic_encode(idx_engine* e, const float* feats, const int32_t* lens, int B, int T, float* out);
 
@@ -366,10 +367,10 @@ typedef struct {
 } idx_debug_gemm;
 int idx_debug_conv_gemm(idx_engine* e, const idx_debug_gemm* g);
 
-/* Diagnostic (tests): one flash attention kernel on already rotated, split fp16 tensors q16 (already scaled: by 1/8
- * for kernel 1, by log2(e)/8 for kernel 2), k16, v16 [B*H][T][64].  kernel: 0 = the one the DiT uses, 1 = mma.sync
- * (softmax in e^x), 2 = wgmma (softmax in 2^x).  out [B][T][H*64] f32 and / or out16 (same layout, fp16), each with
- * `guard` caller elements on both sides (see idx_debug_gemm).                                                     */
+/* Diagnostic (tests): the DiT's flash attention (wgmma, softmax in 2^x) on already rotated, split fp16 tensors q16
+ * (already scaled by log2(e)/8), k16, v16 [B*H][T][64].  kernel: 0 or 2, both this kernel; any other value ->
+ * IDX_ERR_ARG.  out [B][T][H*64] f32 and / or out16 (same layout, fp16), each with `guard` caller elements on both sides
+ * (see idx_debug_gemm).                                                                                             */
 int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16, int B,
                               int T, int H, int kernel, long long guard, float* out, uint16_t* out16);
 
@@ -531,10 +532,10 @@ int idx_codes_to_wav(idx_engine* e, const idx_vocode_request* r, int n_steps, fl
  * Utterance u owns rows [o_u, o_u + P_u + F_u) of the packed solve (o_u = sum of the earlier P + F); attention, the RoPE
  * positions, the WaveNet reflect padding and the prompt-frame zeroing all stay inside each utterance's rows, so every
  * utterance gets the result of its own idx_codes_to_wav call.  The packed solve runs in the default tail mode (gemm_backend
- * 0, tail_f16 1, fused epilogues, the wgmma flash attention); in any other mode each request gets a solve of its own,
- * in the same call.  Errors: n < 1, a null reqs or a bad request (the message names its index) -> IDX_ERR_ARG, and no
- * output is written.  Afterwards idx_s2mel_last_ms reports the solves as the CFM time and the codec and length
- * regulator times summed over the requests; idx_bigvgan_last_ms the summed BigVGAN time.                             */
+ * 0, tail_f16 1); in any other mode each request gets a solve of its own, in the same call.  Errors: n < 1, a null reqs
+ * or a bad request (the message names its index) -> IDX_ERR_ARG, and no output is written.  Afterwards
+ * idx_s2mel_last_ms reports the solves as the CFM time and the codec and length regulator times summed over the
+ * requests; idx_bigvgan_last_ms the summed BigVGAN time.                                                             */
 int idx_codes_to_wav_batch(idx_engine* e, const idx_vocode_request* reqs, int n, int n_steps, float cfg_rate);
 
 /* Device ms of the last codec decode / length regulator / CFM solve (CUDA events).       */

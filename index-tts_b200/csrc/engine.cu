@@ -1,5 +1,6 @@
 // engine.cu — lifecycle, weight registry and host<->device staging of libidxtts.so.
 #include "engine.h"
+#include <cstdlib>
 #include <cstring>
 #include <mutex>
 
@@ -104,6 +105,9 @@ int idx_create(int device, idx_engine** out) {
     e = new idx_engine();
     e->device = device;
     e->num_sms = prop.multiProcessorCount;
+    // initial precision options; idx_set_option changes them afterwards
+    if (getenv("IDX_NO_TC")) e->gemm_backend = 1;
+    if (getenv("IDX_TAIL_F16") && atoi(getenv("IDX_TAIL_F16")) == 0) e->tail_f16 = 0;
     IDX_CUDA(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
     IDX_CUDA(cudaMalloc((void**)&e->dev_flag, 4));
     IDX_CUDA(cudaMemset(e->dev_flag, 0, 4));

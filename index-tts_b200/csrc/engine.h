@@ -88,10 +88,10 @@ struct idx_engine {
   size_t pinned_cap = 0;
   cudaEvent_t events[16] = {};
   cudaEvent_t order_ev = nullptr;   // idx_wait_stream: orders the engine stream after a caller stream
-  int gemm_backend = 0;         // idx_set_option("gemm_backend"): 0 auto (wgmma tf32 where applicable), 1 SIMT fp32
+  int gemm_backend = 0;         // idx_set_option("gemm_backend"): 0 auto (wgmma tf32 where applicable), 1 SIMT fp32 (IDX_NO_TC)
   int force_backend = 0;        // diagnostics (idx_debug_conv_gemm): 0 none, 1 SIMT, 2 tensor core
   int force_tile_n = 0;         // diagnostics (idx_debug_conv_gemm): tensor-core tile width, 0 automatic, 32 / 64 / 128
-  int tail_f16 = 1;             // idx_set_option("tail_f16"): 1 fp16 GEMM operands on the tensor-core path (default), 0 tf32 over fp32 storage
+  int tail_f16 = 1;             // idx_set_option("tail_f16"): 1 fp16 GEMM operands on the tensor-core path (default), 0 tf32 over fp32 storage (IDX_TAIL_F16=0)
   unsigned attr_done = 0;       // bit i: >48 KB dynamic-smem attribute of kernel family i set on this engine's device
   int* dev_flag = nullptr;      // device word set by kernels that meet invalid input (index out of range)
   GptState* gpt = nullptr;

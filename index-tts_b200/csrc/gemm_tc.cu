@@ -188,7 +188,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           uint32_t o[16];
           if (which < 2) {
             const float4* tab = (const float4*)(p.aux + ((size_t)row * (HD / 2) + (d0 >> 1)) * 2);   // (cos, sin) pairs
-            const float sc = (which == 0) ? p.scale : 1.0f;      // 1/8 (x log2 e when the wgmma flash kernel consumes q)
+            const float sc = (which == 0) ? p.scale : 1.0f;      // FLASH_Q_SCALE for the flash attention
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               const float4 t4 = __ldg(tab + i);
@@ -634,9 +634,8 @@ void flash_attention_wgmma_relkey(idx_engine* e, const __half* Qr, const __half*
 }
 
 bool gemm_tc_supported(const ConvGemm& g) {
-  static const bool off = getenv("IDX_NO_TC") != nullptr;
   const bool half = g.A16 && g.Wk16;
-  if (off || g.reflect || (!g.Wk && !half)) return false;
+  if (g.reflect || (!g.Wk && !half)) return false;
   const int al = half ? 8 : 4;                                // 16-byte global strides: 8 fp16 / 4 fp32 elements
   if (g.K % al != 0) return false;
   const int lda = g.lda ? g.lda : g.K;

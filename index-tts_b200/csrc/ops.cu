@@ -172,14 +172,12 @@ void conv_gemm(idx_engine* e, const ConvGemm& g) {
     return;
   }
   IDX_CHECK(g.A != nullptr, IDX_ERR_ARG, "conv_gemm: fp32 operand missing");
-  static const bool force_simt = getenv("IDX_FORCE_SIMT") != nullptr;
   if (e->force_backend == 2) {
     IDX_CHECK(g.Wk && !g.reflect, IDX_ERR_ARG, "conv_gemm: tensor-core path not applicable");
     gemm_tc_launch(e, g);
     return;
   }
-  if (!force_simt && e->force_backend != 1 && !(e->force_backend == 0 && e->gemm_backend == 1) && g.Wk &&
-      gemm_tc_supported(g)) {
+  if (e->force_backend != 1 && !(e->force_backend == 0 && e->gemm_backend == 1) && g.Wk && gemm_tc_supported(g)) {
     gemm_tc_launch(e, g);
     return;
   }
@@ -335,8 +333,7 @@ void pack_half(idx_engine* e, WeightPool& pool, PackedW& w) {
 }
 
 bool tail_half(const idx_engine* e) {
-  static const bool off = getenv("IDX_TAIL_F16") && atoi(getenv("IDX_TAIL_F16")) == 0;
-  return !off && e->tail_f16 && e->gemm_backend == 0 && e->force_backend == 0;
+  return e->tail_f16 && e->gemm_backend == 0 && e->force_backend == 0;
 }
 
 namespace {
@@ -443,7 +440,7 @@ extern "C" int idx_debug_conv_gemm(idx_engine* e, const idx_debug_gemm* d) {
     g.out16 = dOut16 ? dOut16 + d->guard : nullptr;
     g.aux = dAux;
     g.aux_stride = d->epi == EPI_ROPE ? d->heads : d->aux_stride;
-    if (d->epi == EPI_ROPE && d->scale == 0.f) g.scale = flash_attention_q_scale();
+    if (d->epi == EPI_ROPE && d->scale == 0.f) g.scale = FLASH_Q_SCALE;
   }
   DebugOverrides restore{e};
   e->force_backend = d->operands == 1 ? 0 : d->backend;
@@ -471,13 +468,14 @@ extern "C" int idx_debug_conv_gemm(idx_engine* e, const idx_debug_gemm* d) {
   IDX_API_END(e)
 }
 
-// Diagnostic entry (tests): one flash attention kernel on fp16 q / k / v [B*H][T][64] (include/idxtts.h).
+// Diagnostic entry (tests): the wgmma flash attention on fp16 q / k / v [B*H][T][64] (include/idxtts.h).
 extern "C" int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, const uint16_t* k16, const uint16_t* v16, int B,
                                          int T, int H, int kernel, long long guard, float* out, uint16_t* out16) {
   IDX_API_BEGIN
   IDX_CHECK(e && q16 && k16 && v16 && (out || out16), IDX_ERR_ARG, "null argument");
   IDX_CHECK(B > 0 && T > 0 && H > 0, IDX_ERR_ARG, "idx_debug_flash_attention: bad shape");
   IDX_CHECK(guard >= 0 && guard % 8 == 0, IDX_ERR_ARG, "idx_debug_flash_attention: guard must be a non-negative multiple of 8");
+  IDX_CHECK(kernel == 0 || kernel == 2, IDX_ERR_ARG, "idx_debug_flash_attention: kernel is 0 or 2 (the wgmma flash attention)");
   IDX_CUDA(cudaSetDevice(e->device));
   const size_t n = (size_t)B * H * T * 64, ng = n + 2 * (size_t)guard;
   e->ensure_arena(3 * 2 * n + 6 * ng + (16 << 20));
@@ -492,7 +490,7 @@ extern "C" int idx_debug_flash_attention(idx_engine* e, const uint16_t* q16, con
   __half* dOut16 = out16 ? (__half*)e->arena.alloc(2 * ng) : nullptr;
   if (dOut) idx_to_device(e, dOut, out - guard, 4 * ng);
   if (dOut16) idx_to_device(e, dOut16, out16 - guard, 2 * ng);
-  flash_attention_split(e, dq, dk, dv, dOut ? dOut + guard : nullptr, dOut16 ? dOut16 + guard : nullptr, B, T, H, kernel);
+  flash_attention_wgmma(e, dq, dk, dv, dOut ? dOut + guard : nullptr, dOut16 ? dOut16 + guard : nullptr, B, T, H);
   if (dOut) idx_from_device(e, out - guard, dOut, 4 * ng);
   if (dOut16) idx_from_device(e, out16 - guard, dOut16, 2 * ng);
   IDX_CUDA(cudaStreamSynchronize(e->stream));

@@ -11,6 +11,8 @@
 
 enum { EPI_NONE = 0, EPI_SWIGLU = 1, EPI_WNGATE = 2, EPI_ROPE = 3 };
 enum { ACT_NONE = 0, ACT_GELU_ERF = 1, ACT_SILU = 2, ACT_MISH = 3, ACT_GELU_TANH = 4, ACT_RELU = 5 };
+// the scale EPI_ROPE applies to q for the wgmma flash attention: 1/sqrt(64), times log2(e) because its softmax is in 2^x
+constexpr float FLASH_Q_SCALE = 0.125f * 1.4426950408889634f;
 
 // D[b][m][j] = epi( sum_{tap} sum_{k} A[b][m + tap*dil - pad][k] * W[tap][k][j] )
 // rows of A outside [0, Tin) read as zero (Conv1d zero padding) or are reflected (SConv1d).
@@ -29,7 +31,7 @@ struct ConvGemm {
   // fused pair epilogues of the tensor-core kernel (fp16 results straight into the operand of the next GEMM / the attention):
   //   EPI_SWIGLU : columns (2j, 2j+1) = (w1 x, w3 x)_j (weight rows interleaved at pack time) -> out16[row][j] = silu(a) * b
   //   EPI_WNGATE : columns (2j, 2j+1) = (a_j, c_j) of the WaveNet in_layer -> out16[row][j] = tanh(a + g[b][j]) * sigmoid(c + g[b][N/2 + j])
-  //   EPI_ROPE   : columns = q | k | v of the fused wqkv: interleaved-pair RoPE (table aux [T][32][2]) on q (x 1/8) and k, v as is,
+  //   EPI_ROPE   : columns = q | k | v of the fused wqkv: interleaved-pair RoPE (table aux [T][32][2]) on q (x scale) and k, v as is,
   //                written head-major as fp16 Qr | Kr | Vb [B*H][T][64] (out16 = Qr; the three tensors are contiguous)
   int epi = 0;
   __half* out16 = nullptr;
@@ -102,9 +104,9 @@ void nearest_interp(idx_engine* e, const float* x, float* y, int B, int Tin, int
 // out[t][:] = table[ids[t]][:]
 void embedding_rows(idx_engine* e, const float* table, const int* ids, float* out, int n, int C, int nrows);
 // y = silu(a) * b where ab [rows][2*N] holds a | b side by side
-void swiglu(idx_engine* e, const float* ab, float* y, long long rows, int N, __half* y16 = nullptr);
+void swiglu(idx_engine* e, const float* ab, float* y, long long rows, int N);
 // y = tanh(a + ga[b]) * sigmoid(c + gc[b]),  xin [B][T][2N] = a | c ; g [B][*] with stride
-void wn_gate(idx_engine* e, const float* xin, const float* g, int g_stride, float* y, int B, int T, int N, __half* y16 = nullptr);
+void wn_gate(idx_engine* e, const float* xin, const float* g, int g_stride, float* y, int B, int T, int N);
 // copy a [rows][C] block into columns [col0, col0+C) of a [rows][ldo] matrix (concat by columns)
 void copy_cols(idx_engine* e, const float* src, int lds, float* dst, int ldo, int col0, long long rows, int C, __half* dst16 = nullptr);
 // broadcast a per-batch vector [B][C] over T rows into columns of dst
@@ -113,11 +115,9 @@ void bcast_cols(idx_engine* e, const float* vec, float* dst, int ldo, int col0, 
 void silu_inplace(idx_engine* e, float* x, long long n);
 // RoPE table [T][hd/2][2] (cos, sin), base 1e4 (gpt_fast/model.py:336-346)
 void rope_table(idx_engine* e, float* tab, int T, int hd);
-// full (non-causal) attention with key-length mask and interleaved-pair RoPE on q,k.
-// qkv [B][T][3*H*64] (q | k | v), out [B][T][H*64]; lens [B] valid keys (device ints) or null
-// out16 (tensor-core flash path only): the result as fp16 (the operand of the output projection); out may then be null
-void attention_rope(idx_engine* e, const float* qkv, float* out, int B, int T, int H, const float* rope,
-                    const int* lens, __half* out16 = nullptr);
+// full (non-causal) attention with interleaved-pair RoPE on q,k: the wgmma flash attention on fp16 q / k / v (gemm_backend 0)
+// or the fp32 SIMT kernel (gemm_backend 1).  qkv [B][T][3*H*64] (q | k | v), out [B][T][H*64]
+void attention_rope(idx_engine* e, const float* qkv, float* out, int B, int T, int H, const float* rope);
 // x[b][t][c] (+)= ... CFG + Euler: x += dt * ((1+r) * v[0] - r * v[1]); rows t < P zeroed. x,v: [T][C]
 void cfg_euler(idx_engine* e, float* x, const float* v_cond, const float* v_uncond, float dt, float rate,
                int T, int C, int P);
@@ -159,14 +159,8 @@ void pack_half(idx_engine* e, WeightPool& pool, PackedW& w);
 // fp16 K-major copy of w.wk with the two halves of the output rows interleaved (row 2j = row j, row 2j+1 = row N/2 + j): the
 // weight layout of the EPI_SWIGLU / EPI_WNGATE pair epilogues; bias_out (optional) receives the bias interleaved the same way
 __half* pack_half_interleaved(idx_engine* e, WeightPool& pool, const PackedW& w, float** bias_out);
-// the fused flash attention on already rotated / split fp16 tensors Qr | Kr | Vb [B*H][T][64] (what EPI_ROPE writes);
-// kernel: 0 = the default (wgmma unless IDX_FA_WGMMA=0), 1 = mma.sync, 2 = wgmma
-enum { FA_KERNEL_DEFAULT = 0, FA_KERNEL_MMA = 1, FA_KERNEL_WGMMA = 2 };
-void flash_attention_split(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
-                           int B, int T, int H, int kernel = FA_KERNEL_DEFAULT);
-// scale EPI_ROPE must apply to q for flash_attention_split: 1/8, times log2(e) when the wgmma kernel (exp2 softmax) is on
-float flash_attention_q_scale();
-// the same on wgmma (gemm_tc.cu: S and O in registers, P fed back as a register operand)
+// the fused flash attention on already rotated / split fp16 tensors Qr | Kr | Vb [B*H][T][64] (what EPI_ROPE writes), on
+// wgmma (gemm_tc.cu: S and O in registers, P fed back as a register operand)
 void flash_attention_wgmma(idx_engine* e, const __half* Qr, const __half* Kr, const __half* Vb, float* out, __half* out16,
                            int B, int T, int H);
 // ------------------------------------------------------------------- packed sequences --
@@ -207,9 +201,7 @@ void flash_attention_wgmma_relkey(idx_engine* e, const __half* Qr, const __half*
                                   const int* lens, int rel_l, int rel_r, __half* out16, int B, int T, int H);
 // q | k | v Linears of one attention stacked into one [3*od][K] weight with its bias
 PackedW pack3(idx_engine* e, WeightPool& pool, const std::string& a, const std::string& b, const std::string& c);
-// true when the wgmma flash kernel is the default (IDX_FA_WGMMA unset or non-zero)
-bool fa_wgmma_on();
 // fp32 -> fp16 (round to nearest), n elements
 void to_half(idx_engine* e, const float* x, __half* y, long long n);
-// true when the engine runs the tail with fp16 GEMM operands (tensor-core back end and not disabled by IDX_TAIL_F16=0)
+// true when the engine runs the tail with fp16 GEMM operands (gemm_backend 0 and tail_f16 1)
 bool tail_half(const idx_engine* e);

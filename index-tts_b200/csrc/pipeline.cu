@@ -52,7 +52,7 @@ struct Solve {
 };
 
 // The tail of n requests: every request's codec decode and length regulator, then the CFM solves, then per request the
-// prompt-frame crop, BigVGAN and pcm16.  Where cfm_packed_supported() holds, ONE solve runs over the frames of all requests
+// prompt-frame crop, BigVGAN and pcm16.  Where cfm_half() holds, ONE solve runs over the frames of all requests
 // packed along T (request u owns rows [o_u, o_u + T_u) of both CFG batch entries; with one request that is the solo
 // layout); in the other tail modes each request gets a solve of its own.  Outputs are written only after every stage has
 // run and the codes have been checked.  batch: the error of a bad request names its index.
@@ -66,7 +66,7 @@ void codes_to_wav(idx_engine* e, const idx_vocode_request* reqs, int n, int n_st
   S2melState* s = e->s2mel;
   BigvganState* bv = e->bigvgan;
   const int Cd = s2mel_content_dim(s), Hs = s2mel_codec_hidden(s), C = 80, up = bigvgan_total_up(bv), Sd = s2mel_style_dim(s);
-  const bool packed = cfm_packed_supported(e, s);
+  const bool packed = cfm_half(e, s);
   std::vector<Solve> solves;
   for (int u = 0; u < n; ++u) {
     if (u == 0 || !packed) {

@@ -324,21 +324,11 @@ struct DitBuffers {
   // fp16 images of the GEMM operands (tail_half mode): written by the kernel that produces the operand
   __half *a16 = nullptr, *att16 = nullptr, *ffh16 = nullptr, *cat16 = nullptr, *xres16 = nullptr, *wpad16 = nullptr,
          *wacts16 = nullptr, *z16 = nullptr, *wy16 = nullptr, *qkv16 = nullptr;     // qkv16: Qr | Kr | Vb [B*H][T][64] each
-  int* lens;
   // packed solve (two or more segments; null otherwise): the utterances' segments along T, and the gapped WaveNet gate
   // output (see dit_eval)
   const Segments* sg = nullptr;
   __half* wacts16g = nullptr;
 };
-
-static bool tail_fused() {      // pair epilogues (A/B switch IDX_TAIL_FUSED=0)
-  static const bool fused = !(getenv("IDX_TAIL_FUSED") && atoi(getenv("IDX_TAIL_FUSED")) == 0);
-  return fused;
-}
-static bool attn_unfused() {
-  static const bool unfused = getenv("IDX_ATTN_UNFUSED") != nullptr;
-  return unfused;
-}
 
 // one DiT evaluation for batch Bn. x_t [T][80] (shared when x_bcast), C0 [Bn][T][H] constant part
 // of the merge linear, mod/wncond/flmod: rows of the per-timestep tables. out v [Bn][T][80].
@@ -352,8 +342,7 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
     g.a_bcast = x_bcast; g.res = C0;
     conv_gemm(e, g);
   }
-  const bool hf = b.a16 != nullptr;     // fp16 GEMM operands (alloc_dit decides; see ops.h tail_half)
-  const bool fused = tail_fused();
+  const bool hf = b.a16 != nullptr;     // fp16 GEMM operands and the fused pair epilogues (alloc_dit decides: cfm_half)
   auto G = [&](const PackedW& w, const float* A32, const __half* A16, int Bb, int Tt, float* out) {
     return hf ? gemm_of16(w, A16, Bb, Tt, out) : gemm_of(w, A32, Bb, Tt, out);
   };
@@ -371,18 +360,17 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
     }
     rmsnorm_adaln(e, h, hf ? nullptr : b.a, Bn, T, H, s->attn_norm[l].norm_w, mod + s->attn_norm[l].mod_off,
                   mod + s->attn_norm[l].mod_off + H, 0, 1e-5f, b.a16);
-    if (hf && fused) {
-      // wqkv with the RoPE / 1/8 scale / head split in its epilogue: fp16 Qr | Kr | Vb go straight to the flash attention
+    if (hf) {
+      // wqkv with the RoPE / q scale / head split in its epilogue: fp16 Qr | Kr | Vb go straight to the flash attention
       ConvGemm g = gemm_of16(s->wqkv[l], b.a16, Bn, T, nullptr);
-      g.epi = EPI_ROPE; g.out16 = b.qkv16; g.aux = b.rope; g.aux_stride = nh;
-      g.scale = flash_attention_q_scale();          // 1/sqrt(64), times log2(e) when the wgmma flash kernel takes q
+      g.epi = EPI_ROPE; g.out16 = b.qkv16; g.aux = b.rope; g.aux_stride = nh; g.scale = FLASH_Q_SCALE;
       conv_gemm(e, g);
       const size_t one = (size_t)Bn * nh * T * 64;
       if (b.sg) flash_attention_wgmma_varlen(e, b.qkv16, b.qkv16 + one, b.qkv16 + 2 * one, nullptr, b.att16, Bn, nh, *b.sg);
-      else flash_attention_split(e, b.qkv16, b.qkv16 + one, b.qkv16 + 2 * one, nullptr, b.att16, Bn, T, nh);
+      else flash_attention_wgmma(e, b.qkv16, b.qkv16 + one, b.qkv16 + 2 * one, nullptr, b.att16, Bn, T, nh);
     } else {
-      conv_gemm(e, G(s->wqkv[l], b.a, b.a16, Bn, T, b.qkv));
-      attention_rope(e, b.qkv, hf ? nullptr : b.att, Bn, T, nh, b.rope, b.lens, b.att16);
+      conv_gemm(e, gemm_of(s->wqkv[l], b.a, Bn, T, b.qkv));
+      attention_rope(e, b.qkv, b.att, Bn, T, nh, b.rope);
     }
     // layer output buffer: emitted skips (l < Dn/2) keep their own buffer
     float* hout = (l < Dn / 2) ? b.h[1 + l] : b.h[10 + (l & 1)];
@@ -393,13 +381,13 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
     }
     rmsnorm_adaln(e, hout, hf ? nullptr : b.a, Bn, T, H, s->ffn_norm[l].norm_w, mod + s->ffn_norm[l].mod_off,
                   mod + s->ffn_norm[l].mod_off + H, 0, 1e-5f, b.a16);
-    if (hf && fused) {
+    if (hf) {
       ConvGemm g = gemm_of16(s->w13[l], b.a16, Bn, T, nullptr);       // SwiGLU in the epilogue (w1 / w3 rows interleaved)
       g.Wk16 = s->w13_i16[l]; g.bias = nullptr; g.epi = EPI_SWIGLU; g.out16 = b.ffh16;
       conv_gemm(e, g);
     } else {
-      conv_gemm(e, G(s->w13[l], b.a, b.a16, Bn, T, b.ff));
-      swiglu(e, b.ff, hf ? nullptr : b.qkv, (long long)Bn * T, s->inter, b.ffh16);
+      conv_gemm(e, gemm_of(s->w13[l], b.a, Bn, T, b.ff));
+      swiglu(e, b.ff, b.qkv, (long long)Bn * T, s->inter);
     }
     {
       ConvGemm g = G(s->w2[l], b.qkv, b.ffh16, Bn, T, hout);
@@ -440,13 +428,13 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
       reflect_pad_rows(e, b.wy, hf ? nullptr : b.wpad, Bn, T, WH, pl, pr, b.wpad16);
       ConvGemm gi = G(s->wn_in[i], b.wpad, b.wpad16, Bn, T + kk - 1, b.wxin);
       gi.pad = 0; gi.M = T;
-      if (hf && fused) {        // the gate in the epilogue (tanh / sigmoid halves interleaved): fp16 acts, no [T][2 WH] round trip
+      if (hf) {                 // the gate in the epilogue (tanh / sigmoid halves interleaved): fp16 acts, no [T][2 WH] round trip
         gi.Wk16 = s->wn_in_i16[i]; gi.bias = s->wn_in_bias_i[i]; gi.out = nullptr;
         gi.epi = EPI_WNGATE; gi.out16 = b.wacts16; gi.aux = wncond + (size_t)i * 2 * WH; gi.aux_stride = 0;
         conv_gemm(e, gi);
       } else {
         conv_gemm(e, gi);
-        wn_gate(e, b.wxin, wncond + (size_t)i * 2 * WH, 0, hf ? nullptr : b.wacts, Bn, T, WH, b.wacts16);
+        wn_gate(e, b.wxin, wncond + (size_t)i * 2 * WH, 0, b.wacts, Bn, T, WH);
       }
     }
     if (i < NL - 1) {
@@ -470,7 +458,7 @@ static void dit_eval(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T,
   conv_gemm(e, G(s->conv2, b.wy, b.wy16, Bn, T, b.v));
 }
 
-// sg with more than one segment (packed solve, fp16 fused mode only): RoPE positions restart at every segment, room for the
+// sg with more than one segment (packed solve, fp16 mode only): RoPE positions restart at every segment, room for the
 // per-segment WaveNet frames.  One segment (or none) is the single-sequence layout.
 static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T, const Segments* sg = nullptr) {
   const idx_s2mel_config& c = s->cfg;
@@ -493,8 +481,7 @@ static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T
   b.z = e->arena.get<float>(bt * WH);
   b.v = e->arena.get<float>(bt * C);
   b.rope = e->arena.get<float>((size_t)T * 64);
-  b.lens = nullptr;
-  if (tail_half(e) && !attn_unfused() && H % 8 == 0 && WH % 8 == 0 && (H + C) % 8 == 0 && s->inter % 8 == 0) {
+  if (cfm_half(e, s)) {
     auto hb = [&](size_t n) { return (__half*)e->arena.alloc(n * sizeof(__half) + 16); };
     b.a16 = hb(bt * H); b.att16 = hb(bt * H); b.ffh16 = hb(bt * s->inter); b.cat16 = hb(bt * 2 * H);
     b.xres16 = hb(bt * H); b.wpad16 = hb((size_t)Bn * padT * WH); b.wacts16 = hb(bt * WH); b.z16 = hb(bt * WH);
@@ -503,20 +490,19 @@ static void alloc_dit(idx_engine* e, S2melState* s, DitBuffers& b, int Bn, int T
   }
   b.sg = sg;
   if (sg) {
-    IDX_CHECK(b.a16 && tail_fused() && fa_wgmma_on(), IDX_ERR_STATE, "packed solve outside the fp16 fused tail mode");
+    IDX_CHECK(b.a16, IDX_ERR_STATE, "packed solve outside the fp16 tail mode");
     b.wacts16g = (__half*)e->arena.alloc((size_t)Bn * padT * WH * sizeof(__half) + 16);
     rope_table_segments(e, b.rope, *sg, 64);
   } else {
     rope_table(e, b.rope, T, 64);
   }
 }
-// alloc_dit over nseg segments, plus the scratch attention_rope takes when the solve is not packed (the T x T scores only
-// on the unfused path): a packed solve is linear in its length
+// alloc_dit over nseg segments, plus the scratch attention_rope takes when the solve is not packed: linear in the length
 static size_t dit_arena_bytes(const S2melState* s, int Bn, int T, int nseg) {
   const idx_s2mel_config& c = s->cfg;
   const size_t bt = (size_t)Bn * T, pad = (size_t)Bn * (T + 8 * (size_t)nseg) * c.wn_hidden;
   const size_t Tp = (size_t)((T + 3) & ~3);
-  const size_t attn = nseg > 1 ? 0 : 4 * (size_t)Bn * c.heads * (3 * (size_t)T * 64 + 64 * Tp + (attn_unfused() ? (size_t)T * Tp : 0)) + 8 * 256;
+  const size_t attn = nseg > 1 ? 0 : 4 * (size_t)Bn * c.heads * (3 * (size_t)T * 64 + 64 * Tp) + 8 * 256;
   const size_t half_bytes = 2 * (bt * c.hidden * 8 + bt * s->inter + bt * c.wn_hidden * 3 + (nseg > 1 ? 2 : 1) * pad) + 16 * 512;
   return attn + half_bytes + 4 * (bt * c.hidden * 20 + bt * 3 * s->inter + bt * c.wn_hidden * 6 + pad + bt * c.in_channels +
                                   (size_t)T * 64) + 64 * 256;
@@ -659,10 +645,9 @@ size_t cfm_arena_bytes(const S2melState* s, const Segments& sg, int n_steps) {
          4 * (size_t)n_steps * (s->mod_width + 2 * c.wn_hidden * (c.wn_layers + 1) + 6 * c.hidden + 512) +
          (n > 1 ? (size_t)T + 16 * ((size_t)T / 128 + 2 * (size_t)n + 1) + 768 : 0) + (4 << 20);   // segment tables, zero_rows
 }
-bool cfm_packed_supported(const idx_engine* e, const S2melState* s) {
+bool cfm_half(const idx_engine* e, const S2melState* s) {
   const idx_s2mel_config& c = s->cfg;
-  return tail_half(e) && tail_fused() && !attn_unfused() && fa_wgmma_on() && getenv("IDX_NO_TC") == nullptr &&
-         c.hidden % 8 == 0 && c.wn_hidden % 8 == 0 && (c.hidden + c.in_channels) % 8 == 0 && s->inter % 8 == 0;
+  return tail_half(e) && c.hidden % 8 == 0 && c.wn_hidden % 8 == 0 && (c.hidden + c.in_channels) % 8 == 0 && s->inter % 8 == 0;
 }
 
 size_t codec_arena_bytes(const S2melState* s, int n) {

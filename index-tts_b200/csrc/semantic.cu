@@ -8,8 +8,8 @@
 //
 // Default path: fp16 GEMM operands (written by the producing kernel), fp32 accumulate, fp32 residual stream; the attention is
 // the wgmma flash kernel in its RELKEY mode (gemm_tc.cu), the conv module one fused kernel after pointwise_conv1.
-// Strict path (gemm_backend 1 or IDX_NO_TC): fp32 everywhere, the attention unfused (batched GEMMs + exact softmax).
-// The tail diagnostics tail_f16 / IDX_TAIL_F16, IDX_FA_WGMMA and IDX_ATTN_UNFUSED do not apply here.
+// Strict path (gemm_backend 1, the initial value under IDX_NO_TC): fp32 everywhere, the attention unfused (batched GEMMs +
+// exact softmax).  The tail option tail_f16 does not apply here.
 // Padding: rows t >= lens[b] are zeroed at entry and before the depthwise conv, and masked as keys — what the HF encoder
 // does with a prefix attention mask; those rows are still computed, as HF computes them.
 #include "ops.h"
@@ -145,8 +145,7 @@ namespace {
 
 // the encoder runs on fp16 tensor-core operands unless the engine is in strict fp32 mode
 bool sem_half(const idx_engine* e) {
-  static const bool no_tc = getenv("IDX_NO_TC") != nullptr;
-  return e->gemm_backend == 0 && e->force_backend == 0 && !no_tc;
+  return e->gemm_backend == 0 && e->force_backend == 0;
 }
 
 float* upload(WeightPool& pool, const std::vector<float>& h) {
@@ -245,7 +244,7 @@ void encode_dev(idx_engine* e, SemanticState* s, const float* feats, const int* 
       {
         ConvGemm g = gemm_of16(l.qkv, a16, B, T, nullptr);
         g.epi = EPI_ROPE; g.out16 = Qr; g.aux = s->ident; g.aux_stride = H;
-        g.scale = 0.125f * 1.4426950408889634f;              // 1/sqrt(64) and log2(e): the kernel's softmax is in 2^x
+        g.scale = FLASH_Q_SCALE;
         conv_gemm(e, g);
       }
       {

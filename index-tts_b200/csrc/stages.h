@@ -22,13 +22,13 @@ void cfm_stage(idx_engine* e, const S2melState* s, const CfmInputs& in, int u, i
 // The CFM solve of the utterances of sg as ONE solve over their frames packed along T: segment u owns rows
 // [off[u], off[u+1]) of both CFG batch entries and its first P[u] rows are prompt frames (include/idxtts.h
 // idx_codes_to_wav_batch).  One segment issues the launches of a single-utterance solve; two or more upload sg and take
-// the packed kernels, which exist only where cfm_packed_supported() holds.
+// the packed kernels, which exist only where cfm_half() holds.
 void cfm_solve_dev(idx_engine* e, S2melState* s, Segments& sg, const int* P, const CfmInputs& in, int n_steps, float rate);
-// arena of cfm_solve_dev over sg, with room for its staged inputs; the T x T attention scratch only where a one-segment
-// solve can take the unfused attention
+// arena of cfm_solve_dev over sg, with room for its staged inputs
 size_t cfm_arena_bytes(const S2melState* s, const Segments& sg, int n_steps);
-// true in the tail mode that has the packed solve (the default one)
-bool cfm_packed_supported(const idx_engine* e, const S2melState* s);
+// true when the CFM solve runs the DiT / WaveNet on fp16 GEMM operands with the fused pair epilogues: tail_half() and shapes
+// the fp16 kernels take.  The default mode, and the only one with the packed solve.
+bool cfm_half(const idx_engine* e, const S2melState* s);
 int s2mel_content_dim(const S2melState* s);
 int s2mel_style_dim(const S2melState* s);
 int s2mel_codec_hidden(const S2melState* s);

@@ -785,9 +785,9 @@ class Engine:
         return out.view(np.float32).reshape(B, per).copy()
 
     def debug_flash_attention(self, q16, k16, v16, B, H, kernel=0, out=True, out16=True):
-        """One flash attention kernel (include/idxtts.h idx_debug_flash_attention) on fp16 q (already scaled), k, v
-        [B*H][T][64].  Returns (out [B][T][H*64] f32 or None, out16 [B][T][H*64] fp16 or None); raises AssertionError
-        when the kernel wrote outside them."""
+        """The wgmma flash attention (include/idxtts.h idx_debug_flash_attention; kernel 0 or 2) on fp16 q (already scaled
+        by log2(e)/8), k, v [B*H][T][64].  Returns (out [B][T][H*64] f32 or None, out16 [B][T][H*64] fp16 or None);
+        raises AssertionError when the kernel wrote outside them."""
         q16, k16, v16 = (np.ascontiguousarray(x, dtype=np.float16) for x in (q16, k16, v16))
         BH, T, D = q16.shape
         assert D == 64 and BH == B * H and k16.shape == q16.shape and v16.shape == q16.shape

@@ -1,5 +1,6 @@
-"""GPU: both flash attention kernels (mma.sync, wgmma) on fp16 q / k / v against a float64 reference computed on the
-same fp16 values (tests/kernel_refs.py), fp32 and fp16 outputs.
+"""GPU: the wgmma flash attention on fp16 q / k / v against a float64 reference computed on the same fp16 values
+(tests/kernel_refs.py), fp32 and fp16 outputs, through both kernel values of idx_debug_flash_attention that select it
+(0, the one the DiT uses, and 2).
 
 Query rows come in five kinds (row index mod 5), so every tile meets each of them:
   0  plain random scores;
@@ -7,8 +8,7 @@ Query rows come in five kinds (row index mod 5), so every tile meets each of the
   2  large-magnitude scores (up to ~150: only a max-subtracted softmax stays finite);
   3  every real score strongly negative, so the zero-filled keys beyond T (score 0) would win if they were not masked;
   4  near-uniform scores.
-T crosses the key tiles of both kernels (64 and 128 keys) and, from T = 257 on, wraps the wgmma kernel's 2-stage K/V
-ring; T = 1741 is the benchmarked size.
+T crosses the 128-key tiles and, from T = 257 on, wraps the kernel's 2-stage K/V ring; T = 1741 is the benchmarked size.
 
 Bound per row and dimension: 1e-3 * sum_j p_ij |v_j| / sum_j p_ij (about twice the fp16 rounding of P, the dominant
 term), plus the worst-case fp32 summation error of the scores where they are large, plus 2^-11 |ref| for the fp16 output."""
@@ -22,7 +22,7 @@ from tests import kernel_refs as kr
 pytestmark = pytest.mark.gpu
 
 U = 2.0 ** -24
-KERNELS = {"mma": (1, math.e), "wgmma": (2, 2.0)}
+KERNELS = {"default": 0, "wgmma": 2}
 
 
 def make_qkv(B, H, T, seed):
@@ -62,12 +62,18 @@ def reference(B, H, T, base):
 @pytest.mark.parametrize("B,H", [(1, 1), (1, 3), (2, 8)])
 @pytest.mark.parametrize("T", [1, 7, 64, 65, 127, 128, 129, 256, 257, 385, 1741])
 def test_flash_attention(engine, T, B, H, kernel):
-    kid, base = KERNELS[kernel]
-    q, k, v, ref, bound = reference(B, H, T, base)
-    out, out16 = engine.debug_flash_attention(q, k, v, B, H, kernel=kid)
+    q, k, v, ref, bound = reference(B, H, T, 2.0)
+    out, out16 = engine.debug_flash_attention(q, k, v, B, H, kernel=KERNELS[kernel])
     for name, got, bd in (("out", out, bound), ("out16", out16.astype(np.float32), bound + 2.0 ** -11 * np.abs(ref))):
         assert np.all(np.isfinite(got)), name
         err = np.abs(got - ref)
         worst = (err / bd).max()
         print(f"{kernel} T={T} B={B} H={H} {name}: max err {err.max():.2e}, max err / bound {worst:.3f}")
         assert np.all(err <= bd), (name, float(err.max()), float(worst))
+
+
+@pytest.mark.parametrize("kernel", [1, 3, -1])
+def test_unknown_kernel_is_refused(engine, kernel):
+    q, k, v, _, _ = reference(1, 1, 7, 2.0)
+    with pytest.raises(RuntimeError, match=r"failed \(2\)"):
+        engine.debug_flash_attention(q, k, v, 1, 1, kernel=kernel)

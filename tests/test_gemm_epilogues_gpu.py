@@ -7,7 +7,6 @@ Operands are fp16-exact (rounded to fp16 on the host), so the products are exact
 summation error; what is left is the fp16 rounding of the result (2^-11 relative) and the fast intrinsics.  Bound per
 element: 2^-10 |ref| + the summation bound (K + 8) 2^-24 sum|a||w| carried through the epilogue's slope + 2^-24."""
 import math
-import os
 
 import numpy as np
 import pytest
@@ -34,9 +33,8 @@ def check(name, got, ref, bound):
 
 
 def q_scale():
-    """flash_attention_q_scale(): what EPI_ROPE multiplies q by for the default flash kernel."""
-    wgmma = not (os.environ.get("IDX_FA_WGMMA") and int(os.environ["IDX_FA_WGMMA"]) == 0)
-    return float(np.float32(0.125 * math.log2(math.e))) if wgmma else 0.125
+    """FLASH_Q_SCALE (ops.h): what EPI_ROPE multiplies q by for the wgmma flash attention."""
+    return float(np.float32(0.125 * math.log2(math.e)))
 
 
 _rope_cache = {}
@@ -70,7 +68,7 @@ def rope_case(B, H, T):
 @pytest.mark.parametrize("B,H", [(1, 2), (2, 2), (1, 8), (2, 8)])
 def test_rope_epilogue(engine, B, H, T, tile_n):
     A, wk, bias, ref, accb = rope_case(B, H, T)
-    # scale 0: the entry uses flash_attention_q_scale(), as the DiT does
+    # scale 0: the entry uses FLASH_Q_SCALE, as the DiT does
     out = engine.debug_conv_gemm(A, wk, bias=bias, operands=1, tile_n=tile_n, epi=3, heads=H, aux=kr.rope_table(T),
                                  scale=0.0)
     check(f"rope B={B} H={H} T={T} BN={tile_n}", out, ref, 2.0 ** -10 * np.abs(ref) + accb + U)
