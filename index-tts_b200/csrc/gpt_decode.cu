@@ -96,6 +96,7 @@ struct GptParams {
   const int* forced;    // [8][max_new] or null
   float* logits_dump;   // [8][max_new][V] or null
   int* done;            // [1] all sequences finished
+  int* flag;            // engine error word: set to step + 1 when more than CMAX tokens tie at the top-k boundary
   // prefill
   const float* prompt;  // [rows][D] f32
   float* hidden_out;    // prefill only, optional: [rows][D] residual stream after the last block (v1 latent pass)
@@ -1222,7 +1223,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
           FINE_STAMP(34);
           if (p.do_sample) {
             // top-k: extract candidates in descending order (ties at the k-th value are kept, like
-            // TopKLogitsWarper's `scores < kth` test, up to the CMAX slots); the host rejects top_k outside 1..CMAX
+            // TopKLogitsWarper's `scores < kth` test); the host rejects top_k outside 1..CMAX, and a tie that would
+            // need more than CMAX slots sets the error flag (the call is refused, never silently capped)
             float* cv = red + 32;                    // [CMAX] candidate scores
             int* ci = (int*)(red + 32 + CMAX);       // [CMAX] candidate ids
             const int kk = min(max(p.top_k, 1), CMAX);
@@ -1237,6 +1239,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
                 if (tid + j * NCT == besti) sv[j] = -INFINITY;
               block_argmax(best, besti);
             }
+            if (tid == 0 && nc == CMAX && best == kth && best > -INFINITY && !p.finished[b]) *p.flag = k + 1;
             ptx::named_bar_sync(1, NCT);
             if (tid == 0) {
               // softmax over the kept candidates, top-p filter (TopPLogitsWarper: drop while the
@@ -1485,7 +1488,7 @@ __global__ void strict_attn_kernel(const float* qkv, float* kc, float* vc, int p
 __global__ void strict_sample_kernel(const float* logits, unsigned* seen, int V, int k, int seq, float rep_penalty,
                                      int stop_tok, int forbid_stop_before, int do_sample, int top_k, float top_p,
                                      float temperature, unsigned long long seed, int* codes, int max_new, int* nout,
-                                     int* finished, int* tok, const int* forced, float* ldump) {
+                                     int* finished, int* tok, const int* forced, float* ldump, int* flag) {
   extern __shared__ float sv[];            // [V] processed scores
   __shared__ float rb[16];
   __shared__ int ri[16];
@@ -1532,6 +1535,8 @@ __global__ void strict_sample_kernel(const float* logits, unsigned* seen, int V,
       __syncthreads();
       block_argmax(best, besti);
     }
+    // more than CMAX tokens tie at the k-th score: TopKLogitsWarper would keep them all, so the call is refused
+    if (tid == 0 && nc == CMAX && best == kth && best > -INFINITY && !finished[0]) *flag = k + 1;
     __syncthreads();
     if (tid == 0) {
       const float mx = cv[0];
@@ -1600,7 +1605,8 @@ struct BeamParams {
   double* worst;      // [nutt]
   int* done_u;        // [nutt]
   float* ldump;       // [max_new][8][V] or null
-  int* trace_pt;      // [max_new][8][2] or null
+  int* flag;          // engine error word: set to step + 1 when more than CMAX tokens tie at the top-k boundary
+  int* trace_pt;     // [max_new][8][2] or null
   float* trace_sc;    // [max_new][8] or null
 };
 
@@ -1731,6 +1737,9 @@ __global__ void __launch_bounds__(256) beam_step_kernel(const BeamParams p) {
         if (tid + q * 256 == besti) sv[q] = -INFINITY;
       block_argmax(best, besti);
     }
+    // beam-sample top-k keeps every tie at the k-th score; more than CMAX of them is refused (plain beam search,
+    // top_k = 0, needs only the best 2m candidates and keeps no ties)
+    if (tid == 0 && p.top_k > 0 && nc == CMAX && best == kth && best > -INFINITY) *p.flag = k + 1;
     __syncthreads();
     if (tid == 0) {
       int keep = nc;
@@ -1957,6 +1966,9 @@ static T* galloc(GptState* g, size_t n) {
   return p;
 }
 
+// the samplers' error flag: a top-k boundary tie wider than the CMAX candidate slots
+static const char* const kTieOverflow = "more than 128 tokens tie at the top-k boundary";
+
 // ------------------------------------------------------------------ strict fp32 host path --
 struct StrictLayer {
   const float *ln1_w, *ln1_b, *wqkv, *bqkv, *wo, *bo, *ln2_w, *ln2_b, *wfc, *bfc, *wproj, *bproj;
@@ -2071,7 +2083,8 @@ static void strict_generate(idx_engine* e, GptState* g, const idx_gpt_request* r
       strict_sample_kernel<<<1, 256, (size_t)V * 4, st>>>(s->logits, g->seen, V, k, i + g->seq_base, sp->repetition_penalty, c.stop_mel_token,
                                                           sp->forbid_stop_before, sp->do_sample, sp->top_k, sp->top_p,
                                                           sp->temperature, sp->seed, d_codes, max_new, g->nout, g->finished,
-                                                          g->tok, d_forced, d_ldump ? d_ldump + (size_t)k * V : nullptr);
+                                                          g->tok, d_forced, d_ldump ? d_ldump + (size_t)k * V : nullptr,
+                                                          e->dev_flag);
       IDX_CUDA(cudaGetLastError());
       e->launches += 5;
       g->last_launches += 5;
@@ -2079,6 +2092,7 @@ static void strict_generate(idx_engine* e, GptState* g, const idx_gpt_request* r
       IDX_CUDA(cudaStreamSynchronize(st));
       if (*h_fin) break;
     }
+    e->check_flag(kTieOverflow);
     int h_nout = 0;
     IDX_CUDA(cudaMemcpyAsync(&h_nout, g->nout, 4, cudaMemcpyDeviceToHost, st));
     IDX_CUDA(cudaStreamSynchronize(st));
@@ -2472,7 +2486,7 @@ static void fill_common(idx_engine* e, GptState* g, GptParams& p) {
   p.kc = g->kc; p.vc = g->vc; p.nseq = c.max_batch; p.maxpos = g->maxpos;
   p.xg = g->xg; p.qg = g->qg; p.fg = g->fg; p.part = g->part; p.logits = g->logits;
   p.tok = g->tok; p.nout = g->nout; p.finished = g->finished; p.prompt_len = g->prompt_len;
-  p.seen = g->seen; p.done = g->done; p.barrier = g->barrier;
+  p.seen = g->seen; p.done = g->done; p.barrier = g->barrier; p.flag = e->dev_flag;
   p.wstream1 = g->wstream1; p.stream_off1 = g->stream_off1; p.ring_rows = g->ring_rows;
   p.dbg = getenv("IDX_GPT_DBG") ? atoi(getenv("IDX_GPT_DBG")) : 0;
   p.ot = g->ot; p.partt = g->partt; p.cand = g->cand; p.tokt = g->tokt;
@@ -2642,6 +2656,7 @@ static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* req
   bp.beam_scores = d_bscore; bp.tok = g->tok;
   bp.hyp_score = d_hscore; bp.hyp_len = d_hlen; bp.hyp_tok = d_htok; bp.hyp_order = d_horder; bp.nhyp = d_nhyp;
   bp.worst = d_worst; bp.done_u = d_done; bp.ldump = d_ldump; bp.trace_pt = d_trpt; bp.trace_sc = d_trsc;
+  bp.flag = e->dev_flag;
   int* h_done = (int*)e->pinned_buf(64);
   int steps = 0;
   for (int k = 0; k < max_new; ++k) {
@@ -2666,6 +2681,7 @@ static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* req
     }
   }
   IDX_CUDA(cudaEventRecord(g->ev2, st));
+  e->check_flag(kTieOverflow);
 
   // ---- BeamSearchScorer.finalize (transformers_beam_search.py:322-420) on the host ----
   const int fin = steps & 1;      // buffers written by the last beam step
@@ -2756,6 +2772,12 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   // than the device samplers hold, and capping them silently would change the support of the top-p / multinomial step
   IDX_CHECK(!sp->do_sample || (sp->top_k >= 1 && sp->top_k <= CMAX), IDX_ERR_ARG,
             "do_sample needs 1 <= top_k <= 128 (the reference default is 30; top_k = 0 / larger values are not built)");
+  // the values HF's processors refuse are refused here too (greedy ignores temperature and top_p, as HF does)
+  IDX_CHECK(std::isfinite(sp->repetition_penalty) && sp->repetition_penalty > 0.f, IDX_ERR_ARG,
+            "repetition_penalty must be a finite number > 0");
+  IDX_CHECK(!sp->do_sample || (std::isfinite(sp->temperature) && sp->temperature > 0.f), IDX_ERR_ARG,
+            "do_sample needs a finite temperature > 0");
+  IDX_CHECK(!sp->do_sample || (sp->top_p >= 0.f && sp->top_p <= 1.f), IDX_ERR_ARG, "do_sample needs 0 <= top_p <= 1");
   // an armed attention probe is consumed by this call, whatever its outcome
   const int probe_on = g->probe_armed, pprobe_on = g->pprobe_armed;
   g->probe_armed = g->pprobe_armed = 0;
@@ -2901,6 +2923,7 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
     if (*h_done) break;
   }
   IDX_CUDA(cudaEventRecord(g->ev2, e->stream));
+  e->check_flag(kTieOverflow);
 
   // ---- results ----
   int h_nout[8];

@@ -195,6 +195,7 @@ struct SampleArgs {
   int V, stop_tok, forbid_stop_before, top_k, seq_base;
   float rep_penalty, temperature, top_p;
   unsigned long long seed;
+  int* flag;    // set to k + 1 when more than CMAX tokens tie at the top-k boundary; null: the sequence has finished
 };
 __device__ __noinline__ int sample_block(const SampleArgs p, float* red, const unsigned* seen, const float* lg, int k, int b,
                                          int tid, int lane, int warp) {
@@ -257,6 +258,8 @@ __device__ __noinline__ int sample_block(const SampleArgs p, float* red, const u
       if (tid + j * NCT == besti) sv[j] = -INFINITY;
     block_argmax(best, besti);
   }
+  // more than CMAX tokens tie at the k-th score: TopKLogitsWarper would keep them all, so the call is refused
+  if (tid == 0 && p.flag && nc == CMAX && best == kth && best > -INFINITY) *p.flag = k + 1;
   ptx::named_bar_sync(1, NCT);
   if (tid == 0) {
     const float mx = cv[0];
@@ -958,7 +961,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
             SampleArgs sa;
             sa.V = V; sa.stop_tok = p.stop_tok; sa.forbid_stop_before = p.forbid_stop_before; sa.top_k = p.top_k;
             sa.seq_base = p.seq_base; sa.rep_penalty = p.rep_penalty; sa.temperature = p.temperature; sa.top_p = p.top_p;
-            sa.seed = p.seed;
+            sa.seed = p.seed; sa.flag = p.flag;
             const int tk = sample_block(sa, sm.red_att, sm.seen_s, p.logits + (size_t)b * V, k, b, tid, lane, warp);
             if (tid == 0) st_tagged(p.tokt, __int_as_float(tk), ep_head);
             token = tk;

@@ -657,8 +657,8 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
         SampleArgs sa;
         sa.V = V; sa.stop_tok = p.stop_tok; sa.forbid_stop_before = p.forbid_stop_before; sa.top_k = p.top_k;
         sa.seq_base = p.seq_base; sa.rep_penalty = p.rep_penalty; sa.temperature = p.temperature; sa.top_p = p.top_p;
-        sa.seed = p.seed;
-        tk = sample_block(sa, sm.red, sm.seen_s, p.logits + (size_t)b * V, k, b, tid, lane, warp);
+        sa.seed = p.seed; sa.flag = s_fin[b] ? nullptr : p.flag;
+        tk =sample_block(sa, sm.red, sm.seen_s, p.logits + (size_t)b * V, k, b, tid, lane, warp);
       } else {
         // greedy: RepetitionPenalty -> (forbid stop) -> argmax, lowest index among ties
         constexpr int VPT = 40;   // ceil(V / 256) for V <= 10240

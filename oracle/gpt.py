@@ -101,7 +101,8 @@ CMAX = 128     # candidate slots of the device samplers (csrc/gpt_decode.cu)
 
 
 def sample_token(scores, top_k, top_p, seed, step, seq):
-    """Temperature is already applied.  TopK (1 <= top_k <= CMAX = 128 — the device sampler refuses anything else; ties at the k-th value kept up to CMAX slots) → TopP → multinomial by
+    """Temperature is already applied.  TopK (1 <= top_k <= CMAX = 128 — the device sampler refuses anything else; ties at
+    the k-th value kept, and more than CMAX of them raise ValueError, as the device refuses them) → TopP → multinomial by
     inverse CDF over the descending candidates with one Philox draw (transformers logits_process order,
     transformers_generation_utils.py:1035-1047; RNG contract of the device sampler)."""
     s = np.asarray(scores, dtype=np.float32)
@@ -110,7 +111,11 @@ def sample_token(scores, top_k, top_p, seed, step, seq):
     cand = []
     kth = None
     for idx in order:
-        if not np.isfinite(s[idx]) or len(cand) >= CMAX:
+        if not np.isfinite(s[idx]):
+            break
+        if len(cand) >= CMAX:
+            if top_k > 0 and s[idx] == kth:
+                raise ValueError("more than 128 tokens tie at the top-k boundary")
             break
         if len(cand) < kk:
             cand.append(int(idx))
