@@ -1,5 +1,4 @@
-// gpt_decode.cu — the autoregressive speech-token path of UnifiedVoice as ONE persistent
-// sm_90a kernel per group of decode steps.
+// gpt_decode.cu — the autoregressive speech-token path of UnifiedVoice on the device.
 //
 // Replaces, for the v2/v2.5 GPT (SURVEY.md §8a rows a2–a6):
 //   GPT2InferenceModel.forward            indextts/gpt/model_v2.py:121-198
@@ -8,7 +7,17 @@
 //   GenerationMixin._sample greedy loop     transformers_generation_utils.py:3123-3297
 //   RepetitionPenaltyLogitsProcessor        (transformers.generation.logits_process)
 //
-// Design (batch-1 decode is pure weight streaming — 965.6 MB bf16 per token):
+// What the file holds:
+//   * pick_token: the one device token pick (penalty, stop ban, greedy argmax or the temperature / top-k / top-p /
+//     Philox draw, tie-overflow error word), shared by every decode kernel below;
+//   * gpt_fused_kernel: one persistent kernel per group of steps over tiles of 8 rows.  It runs the prefill (a "step"
+//     is a tile of up to 8 consecutive prompt positions of one sequence; causality falls out of the KV-cache position
+//     bound), the v1 latent pass, every beam-search step, and decode whenever the kernels below are not selected;
+//   * gpt_decode1_kernel (gpt_decode1.cuh): one-request decode without grid barriers, the default batch-1 path;
+//   * gpt_decode8_kernel (gpt_decode8.cuh): decode of 2-8 requests per group on the same weight-ring structure;
+//   * the strict fp32 per-op path (weights_bf16 = 0) and the beam-sample step, then the host side.
+//
+// gpt_fused_kernel design (decode is pure weight streaming — 965.6 MB bf16 per token):
 //   * one CTA per SM (cooperative launch), 8 compute warps + 1 producer warp;
 //   * every CTA owns a fixed slice of output columns of every GEMV phase; its weights for
 //     ALL layers/phases are pre-packed into one contiguous byte stream in consumption order,
@@ -16,10 +25,8 @@
 //     completely decoupled from the grid barriers — HBM stays busy while the SMs sit at a
 //     barrier or run the tiny attention / LayerNorm / sampling phases;
 //   * 5 grid barriers per layer (QKV | attention | O-proj+res | FC+gelu | proj+res), head,
-//     sampling; repetition penalty, argmax, stop check and the next-token embedding happen on
-//     the device, the host polls one flag per launch (no per-step D2H sync);
-//   * prefill reuses the same kernel: a "step" is then a tile of up to B_TILE consecutive
-//     prompt positions of one sequence (causality falls out of the KV-cache position bound).
+//     sampling; repetition penalty, the pick, stop check and the next-token embedding happen on
+//     the device, the host polls one flag per launch (no per-step D2H sync).
 //
 // Numerics follow the reference's bf16 path (infer_v2_5.py:143-146,758 — weights .bfloat16()
 // under autocast): bf16 weights, fp32 accumulation, and a round-to-bf16 at every point where
@@ -46,7 +53,9 @@ constexpr int MAXPL = 40;                   // max LayerNorm elements per lane (
 constexpr int HD = 64;                      // head dim (fixed)
 constexpr int PART_STRIDE = 66;             // attention partial: m, l, o[64]
 constexpr int CMAX = 128;                   // candidates the samplers keep after TopK (1 <= top_k <= CMAX, checked by the host)
-#define RED_FLOATS(BT) (((BT) == 1 ? 7 * NCW * 8 : 2 * NCW * 64) > (NCW * PART_STRIDE) ? ((BT) == 1 ? 7 * NCW * 8 : 2 * NCW * 64) : (NCW * PART_STRIDE))
+constexpr int BT = 8;                       // gpt_fused_kernel: rows per tile (decode rows / prompt positions)
+constexpr int RED_FLOATS = 2 * NCW * 8 * BT;   // GEMV K-split partials of 2 column groups; also the attention merge and the pick's scratch
+static_assert(RED_FLOATS >= NCW * PART_STRIDE && RED_FLOATS >= 32 + 2 * CMAX, "shared scratch too small");
 
 struct PrefillTile {
   int seq, pos0, nrows, src_row;
@@ -102,11 +111,10 @@ struct GptParams {
   float* hidden_out;    // prefill only, optional: [rows][D] residual stream after the last block (v1 latent pass)
   const PrefillTile* tiles;
   unsigned* barrier;    // grid barrier counter (zeroed before each launch)
-  // tag-in-data dataflow for the residual stream (batch-1 decode): x[c] travels as {value, epoch} in one 8-byte word
+  // tag-in-data hand-overs of gpt_decode1_kernel: x[c] travels as {value, epoch} in one 8-byte word
   // (the NCCL LL idea), consumers poll the words instead of waiting at a grid barrier
-  uint2* xt;            // [D] tagged residual stream, or null: grid barriers everywhere
-  unsigned* ft;         // [FF] gelu(fc) as {bf16 value, 16-bit tag} words (same mode)
-  unsigned* pflag;      // [B*H*nsplit] epoch of the attention partial of each (row, head, key split)
+  uint2* xt;            // [D] tagged residual stream
+  unsigned* ft;         // [FF] gelu(fc) as {bf16 value, 16-bit tag} words
   uint2* qt;            // [D] tagged q of the current layer
   uint2* kvt;           // [2][D] tagged k, v (bf16-valued) of the position being decoded
   unsigned epoch0;      // first epoch of this launch (2 per layer per step)
@@ -347,7 +355,6 @@ __device__ __forceinline__ float gelu_new(float x, int r) {
   return rnd(t7 * t6, r);
 }
 
-template <int BT>
 struct Smem {
   // carved from dynamic shared memory
   __nv_bfloat16* xs;    // [BT][FF]  GEMV input rows (bf16)
@@ -362,7 +369,7 @@ struct Smem {
   unsigned* seen_s;     // [(V+31)/32] repetition-penalty bitmap of the sequence being sampled
 };
 
-// Cooperative LayerNorm of ONE row by all 8 compute warps (batch-1 decode, where a warp-per-row
+// Cooperative LayerNorm of ONE row by all 8 compute warps (gpt_decode1_kernel, where a warp-per-row
 // LayerNorm would leave 7 warps idle on the critical path).  Shifted one-pass statistics with a
 // per-warp shift K_w = the warp's first element (a single global shift x[0] would make every thread of
 // every CTA poll the same word of the tagged stream): S1_w = sum(x-K_w), S2_w = sum((x-K_w)^2);
@@ -410,27 +417,26 @@ __device__ __forceinline__ void ln_block(float (&v)[NPL / 8], const float* w, co
 // One GEMV phase over this CTA's column slice on the tensor cores (mma.sync m16n8k16, bf16 in,
 // fp32 accumulate).  The slice is cut into groups of <= 8 columns; one ring chunk holds the 8 weight
 // rows of a group for one K-segment of D (pre-swizzled at pack time).  The MMA's M = 16 rows are the 8
-// weight rows (rows 8..15 alias them), N = 8 are the activation rows of the step (batch / prompt
-// positions; a 1-row step aliases row 0), K runs over the segment: warp w owns k-steps
+// weight rows (rows 8..15 alias them), N = 8 are the BT activation rows of the step (batch / prompt
+// positions), K runs over the segment: warp w owns k-steps
 // [w*KS, (w+1)*KS), so every warp issues KS x (ldmatrix A, ldmatrix B, mma) per chunk and the 8 partial
 // accumulators are summed through shared memory.  A tile of M = 8 weight rows per 20 KB stage is what
 // keeps the prefetch ring deep; wgmma's minimum M = 64 would need 160 KB stages.
 // EPI: 0 QKV, 1 O-proj(+residual), 2 FC(+gelu), 3 PROJ(+residual), 4 HEAD
-template <int BT, int EPI, int D>
-__device__ __forceinline__ void gemv_phase(const GptParams& p, const Smem<BT>& sm, int layer,
+template <int EPI, int D>
+__device__ __forceinline__ void gemv_phase(const GptParams& p, const Smem& sm, int layer,
                                            int col0, int ncols, int nseg, unsigned& cons_idx,
                                            const int* row_seq, const int* row_pos,
                                            const int* row_valid, int warp, int lane,
-                                           const float* bias_ph, int o0, long long* fine = nullptr,
-                                           unsigned x_epoch = 0) {
-  constexpr int GMAX = (BT == 1) ? 7 : 2;           // column groups in flight
+                                           const float* bias_ph, int o0) {
+  constexpr int GMAX = 2;                           // column groups in flight
   constexpr int KS = (D / 16) / NCW;                // k-steps per warp per segment
   constexpr int FFc = 4 * D;
   const int ngroups = (ncols + 7) >> 3;
   const int gpb = max(1, min(GMAX, (p.nst - 1) / nseg));
   // per-lane ldmatrix coordinates
   const int a_r = lane & 7, a_hi = (lane >> 4) & 1;            // A: row in tile, k-half (matrices 2,3)
-  const int b_n = min(lane & 7, BT - 1), b_hi = (lane >> 3) & 1;
+  const int b_n = lane & 7, b_hi = (lane >> 3) & 1;
   const uint32_t ring_base = ptx::smem_u32(sm.ring);
   const uint32_t xs_base = ptx::smem_u32(sm.xs) + (uint32_t)b_n * FFc * 2;
   const int g = lane >> 2, t4 = lane & 3;
@@ -446,7 +452,6 @@ __device__ __forceinline__ void gemv_phase(const GptParams& p, const Smem<BT>& s
           const unsigned n = cons_idx + gi * nseg + sgi;
           const int stage = n % p.nst;
           ptx::mbar_wait(&sm.full[stage], (n / p.nst) & 1u);
-          if (fine && threadIdx.x == 0 && g0 == 0 && gi == 0 && sgi == 0) fine[0] = gtimer();
           const uint32_t a_row = ring_base + (uint32_t)((stage * UPC + a_r) * D * 2);
           const uint32_t b_row = xs_base + (uint32_t)(sgi * D * 2);
 #pragma unroll
@@ -463,7 +468,6 @@ __device__ __forceinline__ void gemv_phase(const GptParams& p, const Smem<BT>& s
       }
     }
     // the weights of these chunks are consumed: hand the stages back to the producer
-    if (fine && threadIdx.x == 0 && g0 == 0) fine[1] = gtimer();
     __syncwarp();
     if (lane == 0)
       for (int i = 0; i < nb * nseg; ++i) ptx::mbar_arrive(&sm.empty[(cons_idx + i) % p.nst]);
@@ -474,17 +478,12 @@ __device__ __forceinline__ void gemv_phase(const GptParams& p, const Smem<BT>& s
 #pragma unroll
     for (int gi = 0; gi < GMAX; ++gi) {
       if (gi < nb) {
-        if (BT == 1) {
-          if (t4 == 0) red[(gi * NCW + warp) * 8 + g] = acc[gi][0];
-        } else {
-          float* rp = red + ((gi * NCW + warp) * 8 + g) * 8 + 2 * t4;
-          rp[0] = acc[gi][0];
-          rp[1] = acc[gi][1];
-        }
+        float* rp = red + ((gi * NCW + warp) * 8 + g) * 8 + 2 * t4;
+        rp[0] = acc[gi][0];
+        rp[1] = acc[gi][1];
       }
     }
     ptx::named_bar_sync(1, NCT);
-    if (fine && threadIdx.x == 0 && g0 == 0) fine[2] = gtimer();
     const int nout = nb * 8 * BT;
     for (int idx = threadIdx.x; idx < nout; idx += NCT) {
       const int gi = idx / (8 * BT), r = (idx / BT) & 7, b = idx % BT;
@@ -492,21 +491,18 @@ __device__ __forceinline__ void gemv_phase(const GptParams& p, const Smem<BT>& s
       if (cl >= ncols || !row_valid[b]) continue;
       float a = 0.f;
 #pragma unroll
-      for (int w = 0; w < NCW; ++w)
-        a += (BT == 1) ? red[(gi * NCW + w) * 8 + r] : red[((gi * NCW + w) * 8 + r) * 8 + b];
+      for (int w = 0; w < NCW; ++w) a += red[((gi * NCW + w) * 8 + r) * 8 + b];
       const int c = col0 + cl;
       const int rr = p.round_bf16;
       if (EPI == 0) {
         float v = rnd(a + bias_ph[cl], rr);
         if (c < D) {
           p.qg[(size_t)b * D + c] = v;
-          if (BT == 1 && x_epoch) st_tagged(p.qt + c, v, x_epoch);
         } else {
           size_t base = (((size_t)layer * p.nseq + row_seq[b]) * p.maxpos + row_pos[b]) * D;
           const __nv_bfloat16 kvb = __float2bfloat16_rn(v);
           if (c < 2 * D) p.kc[base + (c - D)] = kvb;
           else p.vc[base + (c - 2 * D)] = kvb;
-          if (BT == 1 && x_epoch) st_tagged(p.kvt + (c - D), __bfloat162float(kvb), x_epoch);
         }
       } else if (EPI == 1 || EPI == 3) {
         // the residual stream is fp32 even on the bf16 path (trap P12): only the branch is rounded
@@ -514,22 +510,132 @@ __device__ __forceinline__ void gemv_phase(const GptParams& p, const Smem<BT>& s
         float xn = sm.xres[b * p.ocap + (c - o0)] + o;
         sm.xres[b * p.ocap + (c - o0)] = xn;
         p.xg[(size_t)b * D + c] = xn;
-        if (BT == 1 && x_epoch) st_tagged(p.xt + c, xn, x_epoch);
       } else if (EPI == 2) {
         float f = rnd(a + bias_ph[cl], rr);
-        const __nv_bfloat16 fv = __float2bfloat16_rn(gelu_new(f, rr));
-        p.fg[(size_t)b * FFc + c] = fv;
-        if (BT == 1 && x_epoch)
-          asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p.ft + c),
-                       "r"((unsigned)__bfloat16_as_ushort(fv) | (x_epoch << 16)) : "memory");
+        p.fg[(size_t)b * FFc + c] = __float2bfloat16_rn(gelu_new(f, rr));
       } else {
         p.logits[(size_t)b * p.V + c] = rnd(a + bias_ph[cl], rr);
       }
     }
-    if (fine && threadIdx.x == 0 && g0 + gpb >= ngroups) fine[3] = gtimer();
     ptx::named_bar_sync(1, NCT);   // red is reused by the next batch of groups
   }
-  if (fine && threadIdx.x == 0) fine[4] = gtimer();
+}
+
+// The token pick of every decode path, in HF's processor order: RepetitionPenalty -> (forbid stop) -> either the argmax
+// (greedy; lowest index among ties) or Temperature -> TopK (every tie at the k-th score kept, like TopKLogitsWarper's
+// `scores < kth` test) -> TopP -> multinomial on the Philox stream at counter (step k, sequence seq_base + b).  The host
+// rejects top_k outside 1..CMAX; a tie that would need more than CMAX candidate slots sets *flag = k + 1, so the call is
+// refused, never silently capped.  Called by the NCT compute threads (threadIdx.x < NCT) of ONE CTA; `red` is
+// >= 32 + 2 * CMAX floats of shared scratch, `seen` the row's repetition-penalty bitmap, `lg` its V logits.  The pick is
+// valid in thread 0.
+struct SampleArgs {
+  int V, stop_tok, forbid_stop_before, do_sample, top_k, seq_base;
+  float rep_penalty, temperature, top_p;
+  unsigned long long seed;
+  int* flag;    // the engine's error word; null when the row has finished (its pick is not recorded)
+};
+__device__ __forceinline__ SampleArgs sample_args(const GptParams& p, bool finished) {
+  SampleArgs a;
+  a.V = p.V; a.stop_tok = p.stop_tok; a.forbid_stop_before = p.forbid_stop_before; a.do_sample = p.do_sample;
+  a.top_k = p.top_k; a.seq_base = p.seq_base; a.rep_penalty = p.rep_penalty; a.temperature = p.temperature;
+  a.top_p = p.top_p; a.seed = p.seed; a.flag = finished ? nullptr : p.flag;
+  return a;
+}
+__device__ __noinline__ int pick_token(const SampleArgs p, float* red, const unsigned* seen, const float* lg, int k, int b) {
+  constexpr int VPT = 40;   // ceil(V / 256) for V <= 10240 (checked by the host)
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int V = p.V;
+  // processed scores of this thread's slice stay in registers: s = rep_penalty(logit) [/ temperature]
+  float sv[VPT];
+  const float inv_temp = (p.do_sample && p.temperature > 0.f) ? 1.0f / p.temperature : 1.0f;
+  // two passes: all loads first (they then fly together: one L2 round trip instead of one per element —
+  // fused into one loop the compiler serialised load -> test -> next load)
+#pragma unroll
+  for (int j = 0; j < VPT; ++j) {
+    const int i = tid + j * NCT;
+    sv[j] = (i < V) ? __ldcg(lg + i) : -INFINITY;
+  }
+#pragma unroll
+  for (int j = 0; j < VPT; ++j) {
+    const int i = tid + j * NCT;
+    if (i < V) {
+      float sc = sv[j];
+      if ((seen[i >> 5] >> (i & 31)) & 1u) sc = (sc < 0.f) ? sc * p.rep_penalty : sc / p.rep_penalty;
+      if (i == p.stop_tok && k < p.forbid_stop_before) sc = -INFINITY;
+      if (p.do_sample) sc *= inv_temp;
+      sv[j] = sc;
+    }
+  }
+  // block argmax with lowest-index tie break, result in every thread
+  auto block_argmax = [&](float& bestv, int& besti) {
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+#pragma unroll
+    for (int j = 0; j < VPT; ++j) {
+      const int i = tid + j * NCT;
+      if (sv[j] > best || (sv[j] == best && i < bi && sv[j] > -INFINITY)) { best = sv[j]; bi = i; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float b2 = __shfl_xor_sync(0xffffffffu, best, o);
+      const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
+    }
+    ptx::named_bar_sync(1, NCT);
+    if (lane == 0) { red[warp * 2] = best; ((int*)red)[warp * 2 + 1] = bi; }
+    ptx::named_bar_sync(1, NCT);
+    for (int w = 0; w < NCW; ++w) {
+      const float b2 = red[w * 2];
+      const int i2 = ((int*)red)[w * 2 + 1];
+      if (w == 0 || b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
+    }
+    bestv = best; besti = bi;
+  };
+  float best; int besti;
+  block_argmax(best, besti);
+  if (!p.do_sample) return besti;
+  // top-k: extract candidates in descending order; the winner is removed from its owner's registers
+  float* cv = red + 32;                    // [CMAX] candidate scores
+  int* ci = (int*)(red + 32 + CMAX);       // [CMAX] candidate ids
+  const int kk = min(max(p.top_k, 1), CMAX);
+  int nc = 0;
+  float kth = best;
+  while (nc < CMAX && best > -INFINITY && (nc < kk || best == kth)) {
+    if (tid == 0) { cv[nc] = best; ci[nc] = besti; }
+    if (nc < kk) kth = best;
+    ++nc;
+#pragma unroll
+    for (int j = 0; j < VPT; ++j)
+      if (tid + j * NCT == besti) sv[j] = -INFINITY;
+    block_argmax(best, besti);
+  }
+  if (tid == 0 && p.flag && nc == CMAX && best == kth && best > -INFINITY) *p.flag = k + 1;
+  ptx::named_bar_sync(1, NCT);
+  if (tid == 0) {
+    // softmax over the kept candidates, top-p filter (TopPLogitsWarper: drop while the
+    // ascending cumulative probability <= 1 - top_p, keep at least one), multinomial
+    const float mx = cv[0];
+    float tot = 0.f;
+    for (int i = 0; i < nc; ++i) { cv[i] = expf(cv[i] - mx); tot += cv[i]; }
+    int keep = nc;
+    if (p.top_p < 1.0f) {
+      float tail = 0.f;
+      for (int i = nc - 1; i >= 1; --i) {
+        tail += cv[i] / tot;
+        if (tail <= 1.0f - p.top_p) keep = i; else break;
+      }
+    }
+    float kt = 0.f;
+    for (int i = 0; i < keep; ++i) kt += cv[i];
+    unsigned rnd4[4];
+    philox4x32_10(p.seed, (unsigned)k, (unsigned)(b + p.seq_base), rnd4);
+    const float u = (float)(rnd4[0] >> 8) * (1.0f / 16777216.0f) * kt;
+    float acc = 0.f;
+    int pick = keep - 1;
+    for (int i = 0; i < keep; ++i) { acc += cv[i]; if (u < acc) { pick = i; break; } }
+    besti = ci[pick];
+  }
+  return besti;
 }
 
 #define PROF_STAMP()                                                        \
@@ -543,7 +649,7 @@ __device__ __forceinline__ int col_begin(int N, int i, int G) {
 }
 
 // PROBE: the instantiation launched while an attention / prefill probe is armed (the other one has no probe code at all)
-template <int BT, int NPL, bool PROBE>
+template <int NPL, bool PROBE>
 __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int D = NPL * 32, FF = 4 * D;
@@ -551,12 +657,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
   const int cta = blockIdx.x;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-  Smem<BT> sm;
+  Smem sm;
   {
     unsigned char* q = smem_raw;
     sm.ring = (__nv_bfloat16*)q;  q += (size_t)p.nst * UPC * D * 2;
     sm.xs = (__nv_bfloat16*)q;    q += (size_t)BT * FF * 2;
-    sm.red = (float*)q;           q += sizeof(float) * RED_FLOATS(BT);
+    sm.red = (float*)q;           q += sizeof(float) * RED_FLOATS;
     sm.full = (uint64_t*)q;       q += sizeof(uint64_t) * p.nst;
     sm.empty = (uint64_t*)q;      q += sizeof(uint64_t) * p.nst;
     sm.flags = (int*)q;           q += 16;
@@ -691,7 +797,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
       // every CTA writes the input rows for its own O-proj column slice [o0,o1)
       for (int idx = tid; idx < BT * (o1 - o0); idx += NCT) {
         int b = idx / (o1 - o0), c = o0 + idx % (o1 - o0);
-        if (b < BT && row_valid[b]) {
+        if (row_valid[b]) {
           float v;
           if (p.mode == 0) {
             v = p.prompt[(size_t)row_posidx[b] * D + c];
@@ -709,57 +815,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
       PROF_STAMP();
 
       for (int l = 0; l < L; ++l) {
-        // Data-flow hand-overs (batch-1 decode): no grid barrier inside a layer.  Epochs are unique per (step, layer).
-        // Write-after-read safety without extra synchronisation — the next writer of every buffer transitively depends on
-        // data that all CTAs produce only after their own reads of it (program order + CTA barriers inside a CTA):
-        //   xt  (O-proj -> FC, PROJ -> next QKV): PROJ(l) starts on a CTA once it holds every ft word of FC(l), which each
-        //        CTA writes after its FC(l) read of xt; O-proj(l+1) needs the attention partials of all heads, hence
-        //        q/k/v columns from every CTA's QKV(l+1), each written after that CTA's read of xt;
-        //   ft  (FC -> PROJ): FC(l+1) needs every xt word of O-proj(l+1), which follows each CTA's PROJ(l) read of ft;
-        //   qt, kvt (QKV -> attention) and part/pflag (attention -> O-proj): QKV(l+1) needs every xt word of PROJ(l),
-        //        which follows each CTA's attention(l) and O-proj(l) reads.
-        // Steps are separated by the grid barriers around the head and the sampling phase.
-        // tagged residual stream (batch-1 decode): epochs of the two x hand-overs of this layer
-        const bool tagged = (BT == 1) && p.xt != nullptr;
-        long long* f2 = (p.prof2 && l == p.prof2_layer && step == p.nsteps - 1) ? p.prof2 + (size_t)cta * 64 : nullptr;
-#define F2(i) do { if (f2 && tid == 0) f2[(i)] = gtimer(); } while (0)
-        F2(0);
-        const unsigned ep_base = p.epoch0 + (unsigned)(step * L + l) * 2u;
-        const unsigned ep_oproj = ep_base + 1u;      // O-proj -> FC of this layer
-        const unsigned ep_proj = ep_base + 2u;       // PROJ -> QKV of the next layer (== ep_base of l + 1)
-        const unsigned f_tag = ((ep_base >> 1) % 65535u) + 1u;   // 16-bit tag of this layer's gelu(fc) words, never 0
         // ---------------- P1: LN1 -> QKV ----------------
         prefetch_ln(1, p.ln2_w + (size_t)l * D, p.ln2_b + (size_t)l * D);  // for P4
-        if constexpr (BT == 1) {
-          float v[NPL / 8];
-          if (tagged && l > 0) {
-            ld_tagged_slice<NPL / 8>(p.xt, warp * (NPL * 4) + lane, ep_base, v);
-            F2(1);
-          } else {
-#pragma unroll
-            for (int j = 0; j < NPL / 8; ++j) v[j] = __ldcg(p.xg + warp * (NPL * 4) + lane + 32 * j);
-          }
-          ln_block<NPL>(v, lnA, lnA + D, sm.red, warp, lane);
-          F2(2);
-#pragma unroll
-          for (int j = 0; j < NPL / 8; ++j)
-            sm.xs[warp * (NPL * 4) + lane + 32 * j] = __float2bfloat16_rn(v[j]);
-        } else {
-          for (int b = warp; b < BT; b += NCW) {
-            float v[NPL], o[NPL];
-            load_row<NPL>(v, p.xg + (size_t)b * D, lane);
-            ln_row<NPL>(v, o, lnA, lnA + D, lane);
-            store_row_bf16<NPL>(o, sm.xs + (size_t)b * FF, b, lane);
-          }
+        for (int b = warp; b < BT; b += NCW) {
+          float v[NPL], o[NPL];
+          load_row<NPL>(v, p.xg + (size_t)b * D, lane);
+          ln_row<NPL>(v, o, lnA, lnA + D, lane);
+          store_row_bf16<NPL>(o, sm.xs + (size_t)b * FF, b, lane);
         }
         ptx::named_bar_sync(1, NCT);
-        F2(3);
-        gemv_phase<BT, 0, D>(p, sm, l, q0, nq, 1, cons_idx, row_seq, row_pos, row_valid,
-                          warp, lane, sm.bias_s + l * bstride, o0,
-                          f2 ? f2 + 4 : nullptr, tagged ? ep_oproj : 0u);
-        F2(9);
+        gemv_phase<0, D>(p, sm, l, q0, nq, 1, cons_idx, row_seq, row_pos, row_valid,
+                         warp, lane, sm.bias_s + l * bstride, o0);
         PROF_STAMP();
-        if (!tagged) grid_sync(p.barrier, bar_target, G, p.bar_flavor);   // tagged: attention polls q and the new k, v
+        grid_sync(p.barrier, bar_target, G, p.bar_flavor);
         PROF_STAMP();
 
         // ---------------- P2: attention over the KV cache ----------------
@@ -776,27 +844,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
             const int k0 = (int)(((long long)ctx * sp) / nsplit);
             const int k1 = (int)(((long long)ctx * (sp + 1)) / nsplit);
             float qv[8];
-            if (tagged) {
-              const uint2* qp = p.qt + h * HD + sub * 8;
-              unsigned val[8], tg[8], spins = 0;
-              bool ok;
-              do {
+            const float* qp = p.qg + (size_t)b * D + h * HD + sub * 8;
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
-                  asm volatile("ld.relaxed.gpu.global.v2.u32 {%0, %1}, [%2];" : "=r"(val[i]), "=r"(tg[i]) : "l"(qp + i) : "memory");
-                ok = true;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) ok &= (tg[i] == ep_oproj);
-                if (++spins > (1u << 26)) __trap();
-              } while (!ok);
-              F2(10);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) qv[i] = __uint_as_float(val[i]);
-            } else {
-              const float* qp = p.qg + (size_t)b * D + h * HD + sub * 8;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) qv[i] = __ldcg(qp + i);
-            }
+            for (int i = 0; i < 8; ++i) qv[i] = __ldcg(qp + i);
             if (PROBE && sp == 0 && warp == 0 && g4 == 0) {
               float* const pr = prb_row[b];
               if (pr) {
@@ -806,8 +856,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
                   for (int i = 0; i < 8; ++i) pl[h * HD + sub * 8 + i] = qv[i];
               }
             }
-            // tagged mode: the position being decoded comes from the tagged words, not from the cache
-            const int kend = tagged ? min(k1, ctx - 1) : k1;
             float m = -INFINITY, lsum = 0.f, ov[8];
 #pragma unroll
             for (int i = 0; i < 8; ++i) ov[i] = 0.f;
@@ -823,9 +871,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
                 base_seq = (b / p.beams) * p.beams;
                 phys_b = p.phys + (size_t)b * p.phys_stride;
               }
-              for (int j0 = k0 + warp * 4; j0 < kend; j0 += NCW * 4) {
+              for (int j0 = k0 + warp * 4; j0 < k1; j0 += NCW * 4) {
                 const int j = j0 + g4;
-                const bool valid = j < kend;
+                const bool valid = j < k1;
                 float s = 0.f;
                 uint4 vv = make_uint4(0, 0, 0, 0);
                 if (valid) {
@@ -860,41 +908,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
               }
             };
             if (p.phys) key_loop(std::true_type{}); else key_loop(std::false_type{});
-            F2(11);
-            if (tagged && k1 == ctx && warp == 0 && g4 == 0) {
-              // the new position (owned by the last key split): k and v straight from the QKV epilogue's tagged words
-              const uint2* kp = p.kvt + h * HD + sub * 8;
-              const uint2* vp = p.kvt + D + h * HD + sub * 8;
-              unsigned kvv[16], tg[16], spins = 0;
-              bool ok;
-              do {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  asm volatile("ld.relaxed.gpu.global.v2.u32 {%0, %1}, [%2];" : "=r"(kvv[i]), "=r"(tg[i]) : "l"(kp + i) : "memory");
-                  asm volatile("ld.relaxed.gpu.global.v2.u32 {%0, %1}, [%2];" : "=r"(kvv[8 + i]), "=r"(tg[8 + i]) : "l"(vp + i) : "memory");
-                }
-                ok = true;
-#pragma unroll
-                for (int i = 0; i < 16; ++i) ok &= (tg[i] == ep_oproj);
-                if (++spins > (1u << 26)) __trap();
-              } while (!ok);
-              float s = 0.f;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) s += qv[i] * __uint_as_float(kvv[i]);
-              s += __shfl_xor_sync(0xffu, s, 1);
-              s += __shfl_xor_sync(0xffu, s, 2);
-              s += __shfl_xor_sync(0xffu, s, 4);
-              s *= 0.125f;
-              const float mn = fmaxf(m, s);
-              const float corr = __expf(m - mn);
-              const float pr = __expf(s - mn);
-              lsum = lsum * corr + pr;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) ov[i] = ov[i] * corr + pr * __uint_as_float(kvv[8 + i]);
-              m = mn;
-            }
             __syncwarp();
-            F2(12);
             // merge the 4 key groups of the warp
 #pragma unroll
             for (int xo = 8; xo <= 16; xo <<= 1) {
@@ -921,7 +935,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
               for (int i = 0; i < 8; ++i) rw[2 + lane * 8 + i] = ov[i];
             }
             ptx::named_bar_sync(1, NCT);
-            F2(13);
             if (warp == 0) {
               float mm = -INFINITY;
               for (int w = 0; w < NCW; ++w) mm = fmaxf(mm, red[w * PART_STRIDE]);
@@ -936,38 +949,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
               if (lane == 0) { pout[0] = mm; pout[1] = lt; }
               pout[2 + lane] = oa;
               pout[2 + 32 + lane] = ob;
-              if (tagged) {
-                // publish the partial: the release is cumulative over the warp's stores ordered by __syncwarp
-                __syncwarp();
-                if (lane == 0) st_release_gpu(p.pflag + (size_t)it * 32, ep_oproj);   // one 128-byte line per flag: no hot line
-              }
             }
           }
         }
-        F2(14);
         PROF_STAMP();
-        if (!tagged) grid_sync(p.barrier, bar_target, G, p.bar_flavor);   // tagged: O-proj polls the partials' flags
+        grid_sync(p.barrier, bar_target, G, p.bar_flavor);
         PROF_STAMP();
 
         // ---------------- P3: merge attention splits -> O-proj + residual ----------------
         // one warp per (row, head): the nsplit partials of a head are contiguous (66 floats
         // each); every load below is independent so they all fly together (one L2 round trip)
         for (int bh0 = warp; bh0 < BT * H; bh0 += 3 * NCW) {
-          if (tagged) {
-            // lanes 0..23 poll the flags of (head r3 = lane / 8, split lane % 8) of this round together
-            const int r3f = lane >> 3, sf = lane & 7;
-            const int bhf = bh0 + r3f * NCW;
-            const bool onf = r3f < 3 && bhf < BT * H && sf < nsplit && row_valid[bhf / H];
-            const unsigned* fp = p.pflag + ((size_t)bhf * nsplit + sf) * 32;
-            unsigned spins = 0;
-            for (;;) {
-              unsigned fv = ep_oproj;
-              if (onf) asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(fv) : "l"(fp) : "memory");
-              if (__all_sync(0xffffffffu, fv == ep_oproj)) break;
-              if (++spins > (1u << 26)) __trap();
-            }
-            if (bh0 == warp) F2(16);
-          }
           float ms[3][8], ls[3][8], oa[3][8], ob[3][8];
 #pragma unroll
           for (int r3 = 0; r3 < 3; ++r3) {
@@ -1011,12 +1003,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
           }
         }
         ptx::named_bar_sync(1, NCT);
-        F2(17);
-        gemv_phase<BT, 1, D>(p, sm, l, o0, no, 1, cons_idx, row_seq, row_pos, row_valid,
-                          warp, lane, sm.bias_s + l * bstride + nq, o0, f2 ? f2 + 18 : nullptr, tagged ? ep_oproj : 0u);
-        F2(23);
+        gemv_phase<1, D>(p, sm, l, o0, no, 1, cons_idx, row_seq, row_pos, row_valid,
+                         warp, lane, sm.bias_s + l * bstride + nq, o0);
         PROF_STAMP();
-        if (!tagged) grid_sync(p.barrier, bar_target, G, p.bar_flavor);   // tagged: FC polls the x words instead
+        grid_sync(p.barrier, bar_target, G, p.bar_flavor);
         PROF_STAMP();
 
         // ---------------- P4: LN2 -> FC + gelu_new ----------------
@@ -1024,96 +1014,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
         if (l + 1 < L) prefetch_ln(0, p.ln1_w + (size_t)(l + 1) * D, p.ln1_b + (size_t)(l + 1) * D);
         else if (p.mode == 1) prefetch_ln(0, p.lnf_w, p.lnf_b);
         else prefetch_ln(0, p.ln1_w, p.ln1_b);
-        if constexpr (BT == 1) {
-          float v[NPL / 8];
-          if (tagged) {
-            ld_tagged_slice<NPL / 8>(p.xt, warp * (NPL * 4) + lane, ep_oproj, v);
-            F2(24);
-            cp_async_wait_all();   // ln_2 parameters prefetched in P1 (ln_block's own CTA barrier publishes them)
-          } else {
-#pragma unroll
-            for (int j = 0; j < NPL / 8; ++j) v[j] = __ldcg(p.xg + warp * (NPL * 4) + lane + 32 * j);
-          }
-          ln_block<NPL>(v, lnB, lnB + D, sm.red, warp, lane);
-          F2(25);
-#pragma unroll
-          for (int j = 0; j < NPL / 8; ++j)
-            sm.xs[warp * (NPL * 4) + lane + 32 * j] = __float2bfloat16_rn(v[j]);
-        } else {
-          for (int b = warp; b < BT; b += NCW) {
-            float v[NPL], o[NPL];
-            load_row<NPL>(v, p.xg + (size_t)b * D, lane);
-            ln_row<NPL>(v, o, lnB, lnB + D, lane);
-            store_row_bf16<NPL>(o, sm.xs + (size_t)b * FF, b, lane);
-          }
+        for (int b = warp; b < BT; b += NCW) {
+          float v[NPL], o[NPL];
+          load_row<NPL>(v, p.xg + (size_t)b * D, lane);
+          ln_row<NPL>(v, o, lnB, lnB + D, lane);
+          store_row_bf16<NPL>(o, sm.xs + (size_t)b * FF, b, lane);
         }
         ptx::named_bar_sync(1, NCT);
-        F2(26);
-        gemv_phase<BT, 2, D>(p, sm, l, f0, nf, 1, cons_idx, row_seq, row_pos, row_valid,
-                          warp, lane, sm.bias_s + l * bstride + nq + no, o0,
-                          f2 ? f2 + 27 : nullptr, tagged ? f_tag : 0u);
-        F2(32);
+        gemv_phase<2, D>(p, sm, l, f0, nf, 1, cons_idx, row_seq, row_pos, row_valid,
+                         warp, lane, sm.bias_s + l * bstride + nq + no, o0);
         PROF_STAMP();
-        if (!tagged) grid_sync(p.barrier, bar_target, G, p.bar_flavor);   // tagged: PROJ polls the {value, tag} words
+        grid_sync(p.barrier, bar_target, G, p.bar_flavor);
         PROF_STAMP();
 
         // ---------------- P5: proj + residual ----------------
         if (l + 1 == L && p.mode == 1) prefetch_ln(1, p.fn_w, p.fn_b);  // final_norm for the head
-        if (tagged) {
-          // chunks of 8 words {bf16, tag}: all loads of a round in flight together, repeat until every tag matches
-          constexpr int CPR = FF / 8, NCH = (CPR + NCT - 1) / NCT;
-          uint4 lo[NCH], hi[NCH];
-          const unsigned want = f_tag << 16;
-          unsigned spins = 0;
-          bool ok;
-          do {
-            ok = true;
-#pragma unroll
-            for (int q = 0; q < NCH; ++q) {
-              const int c = tid + q * NCT;
-              if (c < CPR) {
-                const unsigned* src = p.ft + (size_t)c * 8;
-                asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];"
-                             : "=r"(lo[q].x), "=r"(lo[q].y), "=r"(lo[q].z), "=r"(lo[q].w) : "l"(src) : "memory");
-                asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];"
-                             : "=r"(hi[q].x), "=r"(hi[q].y), "=r"(hi[q].z), "=r"(hi[q].w) : "l"(src + 4) : "memory");
-              }
-            }
-#pragma unroll
-            for (int q = 0; q < NCH; ++q) {
-              if (tid + q * NCT < CPR)
-                ok &= ((lo[q].x & 0xffff0000u) == want) & ((lo[q].y & 0xffff0000u) == want) &
-                      ((lo[q].z & 0xffff0000u) == want) & ((lo[q].w & 0xffff0000u) == want) &
-                      ((hi[q].x & 0xffff0000u) == want) & ((hi[q].y & 0xffff0000u) == want) &
-                      ((hi[q].z & 0xffff0000u) == want) & ((hi[q].w & 0xffff0000u) == want);
-            }
-            if (++spins > (1u << 26)) __trap();
-          } while (!ok);
-          F2(33);
-#pragma unroll
-          for (int q = 0; q < NCH; ++q) {
-            const int c = tid + q * NCT;
-            if (c < CPR)
-              ((uint4*)sm.xs)[c] = make_uint4((lo[q].x & 0xffffu) | (lo[q].y << 16), (lo[q].z & 0xffffu) | (lo[q].w << 16),
-                                              (hi[q].x & 0xffffu) | (hi[q].y << 16), (hi[q].z & 0xffffu) | (hi[q].w << 16));
-          }
-          cp_async_wait_all();     // the LayerNorm parameters prefetched in P4 (the barrier used to drain them)
-        } else {
-          constexpr int CPR = FF / 8;   // 16-byte chunks per row
-          for (int idx = tid; idx < BT * CPR; idx += NCT) {
-            const int b = idx / CPR, c = idx % CPR;
-            ((uint4*)sm.xs)[b * CPR + (c ^ (b & 7))] = __ldcg(((const uint4*)p.fg) + idx);
-          }
+        constexpr int CPR = FF / 8;   // 16-byte chunks per row
+        for (int idx = tid; idx < BT * CPR; idx += NCT) {
+          const int b = idx / CPR, c = idx % CPR;
+          ((uint4*)sm.xs)[b * CPR + (c ^ (b & 7))] = __ldcg(((const uint4*)p.fg) + idx);
         }
         ptx::named_bar_sync(1, NCT);
-        F2(34);
-        const bool tag_proj = tagged && l + 1 < L;   // the last layer hands over to the head through a barrier
-        gemv_phase<BT, 3, D>(p, sm, l, o0, no, nseg_proj, cons_idx, row_seq, row_pos,
-                          row_valid, warp, lane, sm.bias_s + l * bstride + nq + no + nf, o0, f2 ? f2 + 35 : nullptr,
-                          tag_proj ? ep_proj : 0u);
-        F2(40);
+        gemv_phase<3, D>(p, sm, l, o0, no, nseg_proj, cons_idx, row_seq, row_pos,
+                         row_valid, warp, lane, sm.bias_s + l * bstride + nq + no + nf, o0);
         PROF_STAMP();
-        if (!tag_proj) grid_sync(p.barrier, bar_target, G, p.bar_flavor);
+        grid_sync(p.barrier, bar_target, G, p.bar_flavor);
         PROF_STAMP();
       }
 
@@ -1128,27 +1053,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
       }
       if (p.mode == 1) {
         // ---------------- head: ln_f -> final_norm -> mel_head ----------------
-        if constexpr (BT == 1) {
-          float v[NPL / 8];
-#pragma unroll
-          for (int j = 0; j < NPL / 8; ++j) v[j] = __ldcg(p.xg + warp * (NPL * 4) + lane + 32 * j);
-          ln_block<NPL>(v, lnA, lnA + D, sm.red, warp, lane);
-          ln_block<NPL>(v, lnB, lnB + D, sm.red + 3 * NCW, warp, lane);
-#pragma unroll
-          for (int j = 0; j < NPL / 8; ++j)
-            sm.xs[warp * (NPL * 4) + lane + 32 * j] = __float2bfloat16_rn(v[j]);
-        } else {
-          for (int b = warp; b < BT; b += NCW) {
-            float v[NPL], o[NPL];
-            load_row<NPL>(v, p.xg + (size_t)b * D, lane);
-            ln_row<NPL>(v, o, lnA, lnA + D, lane);
-            ln_row<NPL>(o, v, lnB, lnB + D, lane);
-            store_row_bf16<NPL>(v, sm.xs + (size_t)b * FF, b, lane);
-          }
+        for (int b = warp; b < BT; b += NCW) {
+          float v[NPL], o[NPL];
+          load_row<NPL>(v, p.xg + (size_t)b * D, lane);
+          ln_row<NPL>(v, o, lnA, lnA + D, lane);
+          ln_row<NPL>(o, v, lnB, lnB + D, lane);
+          store_row_bf16<NPL>(v, sm.xs + (size_t)b * FF, b, lane);
         }
         ptx::named_bar_sync(1, NCT);
-        gemv_phase<BT, 4, D>(p, sm, 0, h0, nh, 1, cons_idx, row_seq, row_pos, row_valid,
-                          warp, lane, sm.bias_s + L * bstride, o0);
+        gemv_phase<4, D>(p, sm, 0, h0, nh, 1, cons_idx, row_seq, row_pos, row_valid,
+                         warp, lane, sm.bias_s + L * bstride, o0);
         PROF_STAMP();
         grid_sync(p.barrier, bar_target, G, p.bar_flavor);
         PROF_STAMP();
@@ -1168,104 +1082,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
           ptx::named_bar_sync(1, NCT);
 #define FINE_STAMP(n) do { if (p.prof && cta == 0 && tid == 0 && step == p.nsteps - 1) p.prof[256 + (n)] = gtimer(); } while (0)
           FINE_STAMP(32);
-          const unsigned* seen = sm.seen_s;
-          // processed scores of this thread's slice stay in registers: s = rep_penalty(logit) [/ temperature]
-          constexpr int VPT = 40;   // ceil(V / 256) for V <= 10240
-          float sv[VPT];
-          const float inv_temp = (p.do_sample && p.temperature > 0.f) ? 1.0f / p.temperature : 1.0f;
-          // two passes: all loads first (they then fly together: one L2 round trip instead of one per element —
-          // fused into one loop the compiler serialised load -> test -> next load, 10.8 us of the 14 us of this phase)
-#pragma unroll
-          for (int j = 0; j < VPT; ++j) {
-            const int i = tid + j * NCT;
-            sv[j] = (i < V) ? __ldcg(lg + i) : -INFINITY;
-          }
-#pragma unroll
-          for (int j = 0; j < VPT; ++j) {
-            const int i = tid + j * NCT;
-            if (i < V) {
-              float sc = sv[j];
-              if ((seen[i >> 5] >> (i & 31)) & 1u) sc = (sc < 0.f) ? sc * p.rep_penalty : sc / p.rep_penalty;
-              if (i == p.stop_tok && k < p.forbid_stop_before) sc = -INFINITY;
-              if (p.do_sample) sc *= inv_temp;
-              sv[j] = sc;
-            }
-          }
-          float* red = sm.red;
-          // block argmax with lowest-index tie break; `extract` removes the winner from its owner's registers
-          auto block_argmax = [&](float& bestv, int& besti) {
-            float best = -INFINITY;
-            int bi = 0x7fffffff;
-#pragma unroll
-            for (int j = 0; j < VPT; ++j) {
-              const int i = tid + j * NCT;
-              if (sv[j] > best || (sv[j] == best && i < bi && sv[j] > -INFINITY)) { best = sv[j]; bi = i; }
-            }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-              const float b2 = __shfl_xor_sync(0xffffffffu, best, o);
-              const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-              if (b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
-            }
-            ptx::named_bar_sync(1, NCT);
-            if (lane == 0) { red[warp * 2] = best; ((int*)red)[warp * 2 + 1] = bi; }
-            ptx::named_bar_sync(1, NCT);
-            for (int w = 0; w < NCW; ++w) {
-              const float b2 = red[w * 2];
-              const int i2 = ((int*)red)[w * 2 + 1];
-              if (w == 0 || b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
-            }
-            bestv = best; besti = bi;
-          };
+          const int besti = pick_token(sample_args(p, p.finished[b]), sm.red, sm.seen_s, lg, k, b);
           FINE_STAMP(33);
-          float best; int besti;
-          block_argmax(best, besti);
-          FINE_STAMP(34);
-          if (p.do_sample) {
-            // top-k: extract candidates in descending order (ties at the k-th value are kept, like
-            // TopKLogitsWarper's `scores < kth` test); the host rejects top_k outside 1..CMAX, and a tie that would
-            // need more than CMAX slots sets the error flag (the call is refused, never silently capped)
-            float* cv = red + 32;                    // [CMAX] candidate scores
-            int* ci = (int*)(red + 32 + CMAX);       // [CMAX] candidate ids
-            const int kk = min(max(p.top_k, 1), CMAX);
-            int nc = 0;
-            float kth = best;
-            while (nc < CMAX && best > -INFINITY && (nc < kk || best == kth)) {
-              if (tid == 0) { cv[nc] = best; ci[nc] = besti; }
-              if (nc < kk) kth = best;
-              ++nc;
-#pragma unroll
-              for (int j = 0; j < VPT; ++j)
-                if (tid + j * NCT == besti) sv[j] = -INFINITY;
-              block_argmax(best, besti);
-            }
-            if (tid == 0 && nc == CMAX && best == kth && best > -INFINITY && !p.finished[b]) *p.flag = k + 1;
-            ptx::named_bar_sync(1, NCT);
-            if (tid == 0) {
-              // softmax over the kept candidates, top-p filter (TopPLogitsWarper: drop while the
-              // ascending cumulative probability <= 1 - top_p, keep at least one), multinomial
-              const float mx = cv[0];
-              float tot = 0.f;
-              for (int i = 0; i < nc; ++i) { cv[i] = expf(cv[i] - mx); tot += cv[i]; }
-              int keep = nc;
-              if (p.top_p < 1.0f) {
-                float tail = 0.f;
-                for (int i = nc - 1; i >= 1; --i) {
-                  tail += cv[i] / tot;
-                  if (tail <= 1.0f - p.top_p) keep = i; else break;
-                }
-              }
-              float kt = 0.f;
-              for (int i = 0; i < keep; ++i) kt += cv[i];
-              unsigned rnd4[4];
-              philox4x32_10(p.seed, (unsigned)k, (unsigned)(b + p.seq_base), rnd4);
-              const float u = (float)(rnd4[0] >> 8) * (1.0f / 16777216.0f) * kt;
-              float acc = 0.f;
-              int pick = keep - 1;
-              for (int i = 0; i < keep; ++i) { acc += cv[i]; if (u < acc) { pick = i; break; } }
-              besti = ci[pick];
-            }
-          }
           if (tid == 0) {
             const int fin = p.finished[b];
             if (!fin) {
@@ -1279,7 +1097,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) gpt_fused_kernel(const GptParams 
               p.seen[(size_t)b * ((V + 31) / 32) + (feed >> 5)] |= 1u << (feed & 31);
             }
           }
-          FINE_STAMP(35);
+          FINE_STAMP(34);
           ptx::named_bar_sync(1, NCT);
         }
         PROF_STAMP();
@@ -1483,90 +1301,23 @@ __global__ void strict_attn_kernel(const float* qkv, float* kc, float* vc, int p
   if (tid < HD) out[h * HD + tid] = (mg[tid] + mg[tid + HD]) / tot;
 }
 
-// RepetitionPenalty -> (forbid stop) -> [Temperature -> TopK -> TopP -> multinomial | argmax]; same order, tie rules
-// and Philox contract as the sampling phase of the fused kernel.
-__global__ void strict_sample_kernel(const float* logits, unsigned* seen, int V, int k, int seq, float rep_penalty,
-                                     int stop_tok, int forbid_stop_before, int do_sample, int top_k, float top_p,
-                                     float temperature, unsigned long long seed, int* codes, int max_new, int* nout,
-                                     int* finished, int* tok, const int* forced, float* ldump, int* flag) {
-  extern __shared__ float sv[];            // [V] processed scores
-  __shared__ float rb[16];
-  __shared__ int ri[16];
-  __shared__ float cv[CMAX];
-  __shared__ int ci[CMAX];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
-  const float inv_temp = (do_sample && temperature > 0.f) ? 1.0f / temperature : 1.0f;
-  for (int i = tid; i < V; i += blockDim.x) {
-    float s = logits[i];
-    if (ldump) ldump[i] = s;
-    if ((seen[i >> 5] >> (i & 31)) & 1u) s = (s < 0.f) ? s * rep_penalty : s / rep_penalty;
-    if (i == stop_tok && k < forbid_stop_before) s = -INFINITY;
-    if (do_sample) s *= inv_temp;
-    sv[i] = s;
-  }
-  __syncthreads();
-  auto block_argmax = [&](float& bestv, int& besti) {
-    float best = -INFINITY;
-    int bi = 0x7fffffff;
-    for (int i = tid; i < V; i += blockDim.x)
-      if (sv[i] > best || (sv[i] == best && i < bi && sv[i] > -INFINITY)) { best = sv[i]; bi = i; }
-    for (int o = 16; o > 0; o >>= 1) {
-      const float b2 = __shfl_xor_sync(0xffffffffu, best, o);
-      const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
-    }
-    __syncthreads();
-    if (lane == 0) { rb[warp] = best; ri[warp] = bi; }
-    __syncthreads();
-    for (int w = 0; w < nw; ++w)
-      if (w == 0 || rb[w] > best || (rb[w] == best && ri[w] < bi)) { best = rb[w]; bi = ri[w]; }
-    bestv = best; besti = bi;
-  };
-  float best; int besti;
-  block_argmax(best, besti);
-  if (do_sample) {
-    const int kk = min(max(top_k, 1), CMAX);
-    int nc = 0;
-    float kth = best;
-    while (nc < CMAX && best > -INFINITY && (nc < kk || best == kth)) {
-      if (tid == 0) { cv[nc] = best; ci[nc] = besti; sv[besti] = -INFINITY; }
-      if (nc < kk) kth = best;
-      ++nc;
-      __syncthreads();
-      block_argmax(best, besti);
-    }
-    // more than CMAX tokens tie at the k-th score: TopKLogitsWarper would keep them all, so the call is refused
-    if (tid == 0 && nc == CMAX && best == kth && best > -INFINITY && !finished[0]) *flag = k + 1;
-    __syncthreads();
-    if (tid == 0) {
-      const float mx = cv[0];
-      float tot = 0.f;
-      for (int i = 0; i < nc; ++i) { cv[i] = expf(cv[i] - mx); tot += cv[i]; }
-      int keep = nc;
-      if (top_p < 1.0f) {
-        float tail = 0.f;
-        for (int i = nc - 1; i >= 1; --i) {
-          tail += cv[i] / tot;
-          if (tail <= 1.0f - top_p) keep = i; else break;
-        }
-      }
-      float kt = 0.f;
-      for (int i = 0; i < keep; ++i) kt += cv[i];
-      unsigned rnd4[4];
-      philox4x32_10(seed, (unsigned)k, (unsigned)seq, rnd4);
-      const float u = (float)(rnd4[0] >> 8) * (1.0f / 16777216.0f) * kt;
-      float acc = 0.f;
-      int pick = keep - 1;
-      for (int i = 0; i < keep; ++i) { acc += cv[i]; if (u < acc) { pick = i; break; } }
-      besti = ci[pick];
-    }
-  }
+// The pick of one sequence (pick_token, one 256-thread block) and its bookkeeping, as in the sampling phase of the fused
+// kernel.
+__global__ void __launch_bounds__(NCT) strict_sample_kernel(const float* logits, unsigned* seen, int k, SampleArgs sa, int* codes,
+                                                           int max_new, int* nout, int* finished, int* tok, const int* forced,
+                                                           float* ldump) {
+  __shared__ float red[32 + 2 * CMAX];
+  const int tid = threadIdx.x;
+  if (ldump)
+    for (int i = tid; i < sa.V; i += NCT) ldump[i] = logits[i];
+  if (finished[0]) sa.flag = nullptr;
+  const int pick = pick_token(sa, red, seen, logits, k, 0);
   if (tid == 0 && !finished[0]) {
-    codes[k] = besti;
+    codes[k] = pick;
     nout[0] = k + 1;
-    int feed = besti;
+    int feed = pick;
     if (forced) feed = forced[k];
-    else if (besti == stop_tok) finished[0] = 1;
+    else if (pick == sa.stop_tok) finished[0] = 1;
     if (k + 1 >= max_new) finished[0] = 1;
     tok[0] = feed;
     seen[feed >> 5] |= 1u << (feed & 31);
@@ -1901,8 +1652,8 @@ struct GptState {
   GptStrict* strict = nullptr;   // fp32 per-op path (weights_bf16 = 0)
   struct BeamTrace* beam_trace = nullptr;
   int seq_base = 0;             // first request of the decode group being run (idx_gpt_generate splits large calls)
-  int G = 0, FF = 0, nst1 = 0, nst8 = 0, bias_cap = 0, ocap = 0, bar_flavor = 0;
-  size_t smem1 = 0, smem8 = 0;
+  int G = 0, FF = 0, nst = 0, bias_cap = 0, ocap = 0, bar_flavor = 0;
+  size_t smem = 0;                // gpt_fused_kernel: dynamic shared memory with an nst-stage ring
   __nv_bfloat16* wstream = nullptr;
   long long* stream_off = nullptr;
   float *ln1_w = nullptr, *ln1_b = nullptr, *ln2_w = nullptr, *ln2_b = nullptr;
@@ -1914,7 +1665,6 @@ struct GptState {
   uint2* xt = nullptr;          // tagged residual stream (batch-1 decode)
   unsigned* ft = nullptr;       // tagged gelu(fc) words
   uint2 *qt = nullptr, *kvt = nullptr;
-  unsigned* pflag = nullptr;
   // second-generation batch-1 decode kernel
   int v2 = 0, ring_rows = 0;
   int v8 = 0, ring_rows8 = 0;       // gpt_decode8_kernel (2..8 sequences per group)
@@ -1924,7 +1674,6 @@ struct GptState {
   long long* stream_off1 = nullptr;
   uint2 *ot = nullptr, *partt = nullptr, *cand = nullptr, *tokt = nullptr;
   unsigned epoch = 0;           // epochs handed out so far
-  int dataflow = 1;
   __nv_bfloat16* fg = nullptr;
   int *tok = nullptr, *nout = nullptr, *finished = nullptr, *prompt_len = nullptr, *done = nullptr;
   unsigned* seen = nullptr;
@@ -2073,6 +1822,10 @@ static void strict_generate(idx_engine* e, GptState* g, const idx_gpt_request* r
       strict_layers(e, g, pos);
     }
     int* h_fin = (int*)e->pinned_buf(64);
+    SampleArgs sa;
+    sa.V = V; sa.stop_tok = c.stop_mel_token; sa.forbid_stop_before = sp->forbid_stop_before; sa.do_sample = sp->do_sample;
+    sa.top_k = sp->top_k; sa.seq_base = i + g->seq_base; sa.rep_penalty = sp->repetition_penalty;
+    sa.temperature = sp->temperature; sa.top_p = sp->top_p; sa.seed = sp->seed; sa.flag = e->dev_flag;
     int k = 0;
     for (; k < max_new; ++k) {
       strict_embed_kernel<<<(D + 255) / 256, 256, 0, st>>>(s->x, nullptr, mel_emb, mel_pos, g->tok, (k == 0 || sp->mel_pos_mode == 1) ? k : k + 1, D);   // trap P1 / no-cache rule
@@ -2080,11 +1833,8 @@ static void strict_generate(idx_engine* e, GptState* g, const idx_gpt_request* r
       strict_ln_kernel<<<1, 256, 0, st>>>(s->x, e->Wf("gpt.gpt.ln_f.weight"), e->Wf("gpt.gpt.ln_f.bias"), s->h, D);
       strict_ln_kernel<<<1, 256, 0, st>>>(s->h, e->Wf("gpt.final_norm.weight"), e->Wf("gpt.final_norm.bias"), s->att, D);   // trap P3
       strict_gemv_nk_kernel<<<(V + 7) / 8, 256, 0, st>>>(s->att, e->Wf("gpt.mel_head.weight"), e->Wf("gpt.mel_head.bias"), s->logits, D, V);
-      strict_sample_kernel<<<1, 256, (size_t)V * 4, st>>>(s->logits, g->seen, V, k, i + g->seq_base, sp->repetition_penalty, c.stop_mel_token,
-                                                          sp->forbid_stop_before, sp->do_sample, sp->top_k, sp->top_p,
-                                                          sp->temperature, sp->seed, d_codes, max_new, g->nout, g->finished,
-                                                          g->tok, d_forced, d_ldump ? d_ldump + (size_t)k * V : nullptr,
-                                                          e->dev_flag);
+      strict_sample_kernel<<<1, NCT, 0, st>>>(s->logits, g->seen, k, sa, d_codes, max_new, g->nout, g->finished, g->tok, d_forced,
+                                              d_ldump ? d_ldump + (size_t)k * V : nullptr);
       IDX_CUDA(cudaGetLastError());
       e->launches += 5;
       g->last_launches += 5;
@@ -2111,50 +1861,30 @@ static void strict_generate(idx_engine* e, GptState* g, const idx_gpt_request* r
   g->last_steps = maxn;
 }
 
-static size_t smem_bytes(int BT, int D, int FF, int nst, int bias_cap, int ocap, int V) {
-  size_t red = sizeof(float) * (size_t)RED_FLOATS(BT);
-  return (size_t)nst * UPC * D * 2 + (size_t)BT * FF * 2 + red + 16 * (size_t)nst + 16 +
+static size_t smem_bytes(int D, int FF, int nst, int bias_cap, int ocap, int V) {
+  return (size_t)nst * UPC * D * 2 + (size_t)BT * FF * 2 + sizeof(float) * (size_t)RED_FLOATS + 16 * (size_t)nst + 16 +
          4 * (size_t)bias_cap + 4 * (size_t)BT * ocap + 4 * (size_t)((V + 31) / 32) + 16 +
          sizeof(float) * 4 * (size_t)D + 64;
 }
 
-static void reset_tagged_fwd(idx_engine* e, GptState* g, const GptParams& p);
-template <int BT, int NPL>
-static void launch_fused_t(idx_engine* e, GptState* g, GptParams& p) {
-  p.nst = (BT == 1) ? g->nst1 : g->nst8;
+static void launch_fused(idx_engine* e, GptState* g, GptParams& p) {
+  // instantiated geometries: model_dim 1280 (IndexTTS GPT) and 256 (unit-test size)
+  const int npl = p.D / 32;
+  if (npl != 40 && npl != 8) throw IdxError(IDX_ERR_ARG, "model_dim must be 1280 or 256 (instantiated kernel geometries)");
+  p.nst = g->nst;
   p.bias_cap = g->bias_cap;
   p.ocap = g->ocap;
   p.bar_flavor = g->bar_flavor;
-  size_t smem = smem_bytes(BT, p.D, p.FF, p.nst, g->bias_cap, g->ocap, p.V);
   IDX_CUDA(cudaMemsetAsync(g->barrier, 0, (32 + 256) * sizeof(unsigned), e->stream));
-  p.xt = nullptr;
-  if (BT == 1 && p.mode == 1 && g->dataflow) {
-    const unsigned need = (unsigned)p.nsteps * (unsigned)p.L * 2u + 2u;
-    if (g->epoch > 0xF0000000u - need) reset_tagged_fwd(e, g, p);   // epochs never repeat while a stale word could still carry them
-    p.xt = g->xt;
-    p.ft = g->ft;
-    p.qt = g->qt;
-    p.pflag = g->pflag;
-    p.kvt = g->kvt;
-    p.epoch0 = g->epoch;
-    g->epoch += need;
-  }
   void* args[] = {(void*)&p};
-  const void* fn = p.probe ? (const void*)gpt_fused_kernel<BT, NPL, true> : (const void*)gpt_fused_kernel<BT, NPL, false>;
-  IDX_CUDA(cudaLaunchCooperativeKernel(fn, dim3(g->G), dim3(NTHREADS),
-                                       args, smem, e->stream));
+  const void* fn = npl == 40 ? (p.probe ? (const void*)gpt_fused_kernel<40, true> : (const void*)gpt_fused_kernel<40, false>)
+                             : (p.probe ? (const void*)gpt_fused_kernel<8, true> : (const void*)gpt_fused_kernel<8, false>);
+  IDX_CUDA(cudaLaunchCooperativeKernel(fn, dim3(g->G), dim3(NTHREADS), args, g->smem, e->stream));
   e->launches++;
   g->last_launches++;
 }
-
-static void launch_fused_bt(idx_engine* e, GptState* g, GptParams& p, int BT) {
-  // instantiated geometries: model_dim 1280 (IndexTTS GPT) and 256 (unit-test size)
-  const int npl = p.D / 32;
-  if (npl == 40) { if (BT == 1) launch_fused_t<1, 40>(e, g, p); else launch_fused_t<8, 40>(e, g, p); }
-  else if (npl == 8) { if (BT == 1) launch_fused_t<1, 8>(e, g, p); else launch_fused_t<8, 8>(e, g, p); }
-  else throw IdxError(IDX_ERR_ARG, "model_dim must be 1280 or 256 (instantiated kernel geometries)");
-}
-// second-generation batch-1 decode launch (same epoch bookkeeping as the tagged mode of gpt_fused_kernel<1, .>)
+// batch-1 decode (gpt_decode1.cuh): the tagged hand-over words carry epochs that never repeat while a stale word could
+// still carry them
 static size_t smem_bytes_v2(int D, int FF, int R, int bias_cap, int ocap, int V) {
   return (size_t)R * D * 2 + (size_t)FF * 2 + sizeof(float) * (size_t)RED1_FLOATS + 8 * (size_t)NBAR + 5 * sizeof(Phase1) + 32 +
          4 * (size_t)bias_cap + 4 * (size_t)ocap + 4 * (size_t)((V + 31) / 32) + 16 + sizeof(float) * 4 * (size_t)D + 64;
@@ -2163,7 +1893,6 @@ static void reset_tagged(idx_engine* e, GptState* g, const GptParams& p) {
   IDX_CUDA(cudaMemsetAsync(g->xt, 0, (size_t)p.D * sizeof(uint2), e->stream));
   IDX_CUDA(cudaMemsetAsync(g->ft, 0, (size_t)p.FF * sizeof(unsigned), e->stream));
   IDX_CUDA(cudaMemsetAsync(g->qt, 0, (size_t)p.D * sizeof(uint2), e->stream));
-  IDX_CUDA(cudaMemsetAsync(g->pflag, 0, 32 * (size_t)(8 * p.H * std::max(1, p.G / p.H) + p.G) * sizeof(unsigned), e->stream));
   IDX_CUDA(cudaMemsetAsync(g->kvt, 0, 2 * (size_t)p.D * sizeof(uint2), e->stream));
   if (g->ot) {
     IDX_CUDA(cudaMemsetAsync(g->ot, 0, (size_t)p.D * sizeof(uint2), e->stream));
@@ -2173,11 +1902,10 @@ static void reset_tagged(idx_engine* e, GptState* g, const GptParams& p) {
   }
   g->epoch = 0;
 }
-static void reset_tagged_fwd(idx_engine* e, GptState* g, const GptParams& p) { reset_tagged(e, g, p); }
 static void launch_decode1(idx_engine* e, GptState* g, GptParams& p) {
   p.bias_cap = g->bias_cap;
   p.ocap = g->ocap;
-  p.xt = g->xt; p.ft = g->ft; p.qt = g->qt; p.pflag = g->pflag; p.kvt = g->kvt;
+  p.xt = g->xt; p.ft = g->ft; p.qt = g->qt; p.kvt = g->kvt;
   const unsigned need = (unsigned)p.nsteps * (unsigned)p.L * 2u + 2u;
   if (g->epoch > 0xF0000000u - need) reset_tagged(e, g, p);   // epochs never repeat while a stale word could still carry them
   p.epoch0 = g->epoch;
@@ -2205,17 +1933,6 @@ static void launch_decode8(idx_engine* e, GptState* g, GptParams& p) {
   IDX_CUDA(cudaLaunchCooperativeKernel(fn, dim3(g->G), dim3(NCT), args, g->smem_v8, e->stream));
   e->launches++;
   g->last_launches++;
-}
-
-template <int BT>
-static void set_smem_attr(int npl, size_t bytes) {
-  if (npl == 40) {
-    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 40, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 40, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  } else {
-    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<BT, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  }
 }
 
 extern "C" int idx_gpt_init(idx_engine* e, const idx_gpt_config* cfg) {
@@ -2256,18 +1973,17 @@ extern "C" int idx_gpt_init(idx_engine* e, const idx_gpt_config* cfg) {
   g->ocap = cdiv(D, G) + 1;
   g->bias_cap = L * (cdiv(3 * D, G) + 1 + 2 * g->ocap + cdiv(FF, G) + 1) + cdiv(V, G) + 1;
   g->bar_flavor = getenv("IDX_GPT_BAR_FLAVOR") ? atoi(getenv("IDX_GPT_BAR_FLAVOR")) : 1;   // flavor 2 (per-CTA flags) measured slower: 839 vs 683 us/step
-  auto pick_nst = [&](int BT) {
-    int nst = 2;
-    while (nst < 32 && smem_bytes(BT, D, FF, nst + 1, g->bias_cap, g->ocap, V) <= (size_t)dev_smem - 1024) ++nst;
-    return nst;
-  };
-  g->nst1 = pick_nst(1);
-  g->nst8 = pick_nst(8);
-  g->smem1 = smem_bytes(1, D, FF, g->nst1, g->bias_cap, g->ocap, V);
-  g->smem8 = smem_bytes(8, D, FF, g->nst8, g->bias_cap, g->ocap, V);
-  IDX_CHECK(g->smem8 <= (size_t)dev_smem, IDX_ERR_ARG, "shared memory budget exceeded");
-  set_smem_attr<1>(D / 32, g->smem1);
-  set_smem_attr<8>(D / 32, g->smem8);
+  g->nst = 2;
+  while (g->nst < 32 && smem_bytes(D, FF, g->nst + 1, g->bias_cap, g->ocap, V) <= (size_t)dev_smem - 1024) ++g->nst;
+  g->smem = smem_bytes(D, FF, g->nst, g->bias_cap, g->ocap, V);
+  IDX_CHECK(g->smem <= (size_t)dev_smem, IDX_ERR_ARG, "shared memory budget exceeded");
+  if (D / 32 == 40) {
+    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<40, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->smem));
+    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<40, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->smem));
+  } else {
+    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->smem));
+    IDX_CUDA(cudaFuncSetAttribute(gpt_fused_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->smem));
+  }
 
   // ---- build the per-CTA unit table in consumption order ----
   std::vector<PackUnit> units;
@@ -2446,9 +2162,7 @@ extern "C" int idx_gpt_init(idx_engine* e, const idx_gpt_config* cfg) {
   g->xt = galloc<uint2>(g, (size_t)D);
   g->ft = galloc<unsigned>(g, (size_t)FF);
   g->qt = galloc<uint2>(g, (size_t)D);
-  g->pflag = galloc<unsigned>(g, 32 * (size_t)(8 * H * std::max(1, G / H) + G));
   g->kvt = galloc<uint2>(g, 2 * (size_t)D);
-  g->dataflow = getenv("IDX_GPT_DATAFLOW") ? atoi(getenv("IDX_GPT_DATAFLOW")) : 1;
   g->qg = galloc<float>(g, 8 * (size_t)D);
   g->fg = galloc<__nv_bfloat16>(g, 8 * (size_t)FF);
   g->part = galloc<float>(g, (size_t)(8 * H * std::max(1, G / H) + G) * PART_STRIDE);
@@ -2636,7 +2350,7 @@ static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* req
   p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
   p.beams = m;                                   // the prefill probe's request index is the tile's slot / m
   if (pprobe_on) probe_arm_prefill(e, g, p, pb);
-  launch_fused_bt(e, g, p, 8);
+  launch_fused(e, g, p);
   IDX_CUDA(cudaEventRecord(g->ev1, st));
 
   fill_common(e, g, p);
@@ -2662,7 +2376,7 @@ static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* req
   for (int k = 0; k < max_new; ++k) {
     const int cur = k & 1, nxt = cur ^ 1;
     p.step0 = k; p.nsteps = 1; p.phys = d_phys[cur];
-    launch_fused_bt(e, g, p, 8);
+    launch_fused(e, g, p);
     bp.k = k;
     bp.seen_cur = d_seen[cur]; bp.seen_nxt = d_seen[nxt];
     bp.hist_cur = d_hist[cur]; bp.hist_nxt = d_hist[nxt];
@@ -2820,7 +2534,6 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
             "max_new_tokens must satisfy k+1 <= mel_pos rows - 1 (SURVEY A.3)");
   IDX_CUDA(cudaSetDevice(e->device));
   const int D = c.model_dim, V = c.number_mel_codes, max_new = sp->max_new_tokens;
-  const int BT = (nreq == 1) ? 1 : 8;
   g->last_launches = 0;
   if (g->strict) {
     IDX_CHECK(sp->num_beams == 1, IDX_ERR_ARG, "the strict fp32 path decodes one sequence at a time (num_beams = 1)");
@@ -2895,7 +2608,7 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
   ProbeBufs pb;
   if (pprobe_on) probe_arm_prefill(e, g, p, pb);
-  launch_fused_bt(e, g, p, 8);
+  launch_fused(e, g, p);
   IDX_CUDA(cudaEventRecord(g->ev1, e->stream));
 
   // ---- decode ----
@@ -2908,15 +2621,16 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   p.pos_plain = sp->mel_pos_mode == 1;
   p.codes = d_codes; p.forced = d_forced; p.logits_dump = d_ldump;
   if (probe_on) probe_arm_decode(e, g, p, pb, max_new);
-  const int SPL = (BT == 1 && g->v2) ? 64 : 32;  // steps per launch: the host looks at one flag every SPL steps
+  const bool dec1 = nreq == 1 && g->v2, dec8 = nreq > 1 && g->v8;   // otherwise gpt_fused_kernel decodes the nreq rows
+  const int SPL = dec1 ? 64 : 32;  // steps per launch: the host looks at one flag every SPL steps
   int steps_done = 0;
   int* h_done = (int*)e->pinned_buf(64);
   while (steps_done < max_new) {
     p.step0 = steps_done;
     p.nsteps = std::min(SPL, max_new - steps_done);
-    if (BT == 1 && g->v2) launch_decode1(e, g, p);
-    else if (BT == 8 && g->v8) launch_decode8(e, g, p);
-    else launch_fused_bt(e, g, p, BT);
+    if (dec1) launch_decode1(e, g, p);
+    else if (dec8) launch_decode8(e, g, p);
+    else launch_fused(e, g, p);
     IDX_CUDA(cudaMemcpyAsync(h_done, g->done, 4, cudaMemcpyDeviceToHost, e->stream));
     IDX_CUDA(cudaStreamSynchronize(e->stream));
     steps_done += p.nsteps;
@@ -3191,7 +2905,7 @@ extern "C" int idx_gpt_latents_v1(idx_engine* e, const float* conds, int n_laten
     fill_common(e, g, p);
     p.B = 8; p.mode = 0; p.nsteps = (int)tiles.size(); p.prompt = d_rows; p.tiles = d_tiles; p.hidden_out = d_hid;
     p.max_new = 1; p.rep_penalty = 1.f;
-    launch_fused_bt(e, g, p, 8);
+    launch_fused(e, g, p);
     layernorm(e, d_hid + (size_t)first * D, d_tmp, 1, n_codes, D, e->Wf("gpt.gpt.ln_f.weight"), e->Wf("gpt.gpt.ln_f.bias"), 1e-5f,
               nullptr, nullptr, 0);
     layernorm(e, d_tmp, d_lat, 1, n_codes, D, e->Wf("gpt.final_norm.weight"), e->Wf("gpt.final_norm.bias"), 1e-5f, nullptr, nullptr, 0);

@@ -1,12 +1,11 @@
-// gpt_decode1.cuh — second-generation batch-1 decode kernel (round 2).  Included by gpt_decode.cu inside its
-// anonymous namespace: it reuses GptParams, the tagged-word helpers, ln_block, gelu_new and the Philox sampler.
+// gpt_decode1.cuh — the batch-1 decode kernel.  Included by gpt_decode.cu inside its anonymous namespace: it reuses
+// GptParams, the tagged-word helpers, ln_block, gelu_new and pick_token.
 //
-// What it replaces: the <1, NPL> instantiation of gpt_fused_kernel for `nreq == 1, num_beams == 1` decode (the
-// BASELINE config-2 hot loop).  Same arithmetic, same rounding points, same sampler contract, same KV-cache layout;
-// prefill, multi-row decode and beam search stay on gpt_fused_kernel<8, NPL>.
+// It decodes `nreq == 1, num_beams == 1` (the BASELINE config-2 hot loop) with the arithmetic, rounding points, pick and
+// KV-cache layout of gpt_fused_kernel, which keeps prefill, multi-row decode and beam search.
 //
-// Why: the per-CTA timeline of round 1 (profiles/r02_gpt_fine_timeline_before.txt; 26 us per layer against 6 us of
-// pure weight streaming) showed where the time of a layer went:
+// Why a kernel of its own: the per-CTA timeline of a fused-kernel decode of one row (profiles/r02_gpt_fine_timeline_before.txt;
+// 26 us per layer against 6 us of pure weight streaming) showed where the time of a layer went:
 //   * 6.9 us in the GEMV MMAs: one dependent ldmatrix -> mma chain per 8-row chunk, chunks processed one after
 //     the other, and the 9th column of the 1280-wide phases costing a whole second chain
 //       -> here a tile is 16 REAL weight rows (m16n8k16 with all 16 A rows used), every tile of a phase is in flight
@@ -186,104 +185,6 @@ __device__ __forceinline__ uint2 ld_tagged_word(const uint2* p) {
   uint2 v;
   asm volatile("ld.relaxed.gpu.global.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p) : "memory");
   return v;
-}
-
-// The sampling phase of gpt_fused_kernel as a function (same processor order, tie rules and Philox contract):
-// RepetitionPenalty -> (forbid stop) -> Temperature -> TopK (ties kept) -> TopP -> multinomial.  Called by the 8 compute
-// warps of ONE CTA; `red` is >= 32 + 2 * CMAX floats of scratch.  The pick is valid in thread 0.
-struct SampleArgs {
-  int V, stop_tok, forbid_stop_before, top_k, seq_base;
-  float rep_penalty, temperature, top_p;
-  unsigned long long seed;
-  int* flag;    // set to k + 1 when more than CMAX tokens tie at the top-k boundary; null: the sequence has finished
-};
-__device__ __noinline__ int sample_block(const SampleArgs p, float* red, const unsigned* seen, const float* lg, int k, int b,
-                                         int tid, int lane, int warp) {
-  constexpr int VPT = 40;   // ceil(V / 256) for V <= 10240
-  const int V = p.V;
-  float sv[VPT];
-  const float inv_temp = (p.temperature > 0.f) ? 1.0f / p.temperature : 1.0f;
-#pragma unroll
-  for (int j = 0; j < VPT; ++j) {
-    const int i = tid + j * NCT;
-    sv[j] = (i < V) ? __ldcg(lg + i) : -INFINITY;
-  }
-#pragma unroll
-  for (int j = 0; j < VPT; ++j) {
-    const int i = tid + j * NCT;
-    if (i < V) {
-      float sc = sv[j];
-      if ((seen[i >> 5] >> (i & 31)) & 1u) sc = (sc < 0.f) ? sc * p.rep_penalty : sc / p.rep_penalty;
-      if (i == p.stop_tok && k < p.forbid_stop_before) sc = -INFINITY;
-      sv[j] = sc * inv_temp;
-    }
-  }
-  auto block_argmax = [&](float& bestv, int& besti) {
-    float best = -INFINITY;
-    int bi = 0x7fffffff;
-#pragma unroll
-    for (int j = 0; j < VPT; ++j) {
-      const int i = tid + j * NCT;
-      if (sv[j] > best || (sv[j] == best && i < bi && sv[j] > -INFINITY)) { best = sv[j]; bi = i; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float b2 = __shfl_xor_sync(0xffffffffu, best, o);
-      const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
-    }
-    ptx::named_bar_sync(1, NCT);
-    if (lane == 0) { red[warp * 2] = best; ((int*)red)[warp * 2 + 1] = bi; }
-    ptx::named_bar_sync(1, NCT);
-    for (int w = 0; w < NCW; ++w) {
-      const float b2 = red[w * 2];
-      const int i2 = ((int*)red)[w * 2 + 1];
-      if (w == 0 || b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
-    }
-    bestv = best; besti = bi;
-  };
-  float best; int besti;
-  block_argmax(best, besti);
-  float* cv = red + 32;
-  int* ci = (int*)(red + 32 + CMAX);
-  const int kk = min(max(p.top_k, 1), CMAX);
-  int nc = 0;
-  float kth = best;
-  while (nc < CMAX && best > -INFINITY && (nc < kk || best == kth)) {
-    if (tid == 0) { cv[nc] = best; ci[nc] = besti; }
-    if (nc < kk) kth = best;
-    ++nc;
-#pragma unroll
-    for (int j = 0; j < VPT; ++j)
-      if (tid + j * NCT == besti) sv[j] = -INFINITY;
-    block_argmax(best, besti);
-  }
-  // more than CMAX tokens tie at the k-th score: TopKLogitsWarper would keep them all, so the call is refused
-  if (tid == 0 && p.flag && nc == CMAX && best == kth && best > -INFINITY) *p.flag = k + 1;
-  ptx::named_bar_sync(1, NCT);
-  if (tid == 0) {
-    const float mx = cv[0];
-    float tot = 0.f;
-    for (int i = 0; i < nc; ++i) { cv[i] = expf(cv[i] - mx); tot += cv[i]; }
-    int keep = nc;
-    if (p.top_p < 1.0f) {
-      float tail = 0.f;
-      for (int i = nc - 1; i >= 1; --i) {
-        tail += cv[i] / tot;
-        if (tail <= 1.0f - p.top_p) keep = i; else break;
-      }
-    }
-    float kt = 0.f;
-    for (int i = 0; i < keep; ++i) kt += cv[i];
-    unsigned rnd4[4];
-    philox4x32_10(p.seed, (unsigned)k, (unsigned)(b + p.seq_base), rnd4);
-    const float u = (float)(rnd4[0] >> 8) * (1.0f / 16777216.0f) * kt;
-    float acc = 0.f;
-    int pick = keep - 1;
-    for (int i = 0; i < keep; ++i) { acc += cv[i]; if (u < acc) { pick = i; break; } }
-    besti = ci[pick];
-  }
-  return besti;
 }
 
 template <int NPL>
@@ -958,11 +859,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
             }
             __threadfence();
             ptx::named_bar_sync(1, NCT);
-            SampleArgs sa;
-            sa.V = V; sa.stop_tok = p.stop_tok; sa.forbid_stop_before = p.forbid_stop_before; sa.top_k = p.top_k;
-            sa.seq_base = p.seq_base; sa.rep_penalty = p.rep_penalty; sa.temperature = p.temperature; sa.top_p = p.top_p;
-            sa.seed = p.seed; sa.flag = p.flag;
-            const int tk = sample_block(sa, sm.red_att, sm.seen_s, p.logits + (size_t)b * V, k, b, tid, lane, warp);
+            const int tk = pick_token(sample_args(p, false), sm.red_att, sm.seen_s, p.logits + (size_t)b * V, k, b);
             if (tid == 0) st_tagged(p.tokt, __int_as_float(tk), ep_head);
             token = tk;
           }

@@ -1,7 +1,7 @@
 // gpt_decode8.cuh — decode of 2..8 sequences per group on the round-2 tile / ring structure (included by gpt_decode.cu
 // after gpt_decode1.cuh, inside its anonymous namespace).
 //
-// Replaces `gpt_fused_kernel<8, NPL>` for plain (non-beam) multi-sequence decode — BASELINE configs 3 and 5 decode 8
+// Takes plain (non-beam) multi-sequence decode off `gpt_fused_kernel` — BASELINE configs 3 and 5 decode 8
 // utterances per group.  The round-1 kernel spent 47 us per layer (profile of round 2: O-proj 11.7 us merging key splits for
 // 8 x 20 (row, head) pairs, attention 8.6, FC 6.4, QKV 5.3, barriers 10.9): 1.1 ms per 8-row step.  Here:
 //   * the m16n8k16 MMA's N = 8 columns are the 8 sequences (they were 7/8 wasted at batch 1), 16 real weight rows per tile,
@@ -25,7 +25,7 @@ struct Smem8 {
   __nv_bfloat16* ring;  // [R][D]
   __nv_bfloat16* xs;    // [8][D] LayerNorm output rows (bf16, 16-byte chunks XOR-swizzled by the row)
   float* red;           // [RED8_FLOATS]
-  float* att;           // [NCW][66] attention merge / argmax scratch
+  float* att;           // [NCW][66] attention merge
   uint64_t* full;       // [NBAR]
   Phase1* pht;          // [5]
   float* bias_s;
@@ -652,50 +652,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
     // ---------------- sampling: CTA b decides for sequence b ----------------
     if (cta < B) {
       const int b = cta;
-      int tk;
-      if (p.do_sample) {
-        SampleArgs sa;
-        sa.V = V; sa.stop_tok = p.stop_tok; sa.forbid_stop_before = p.forbid_stop_before; sa.top_k = p.top_k;
-        sa.seq_base = p.seq_base; sa.rep_penalty = p.rep_penalty; sa.temperature = p.temperature; sa.top_p = p.top_p;
-        sa.seed = p.seed; sa.flag = s_fin[b] ? nullptr : p.flag;
-        tk =sample_block(sa, sm.red, sm.seen_s, p.logits + (size_t)b * V, k, b, tid, lane, warp);
-      } else {
-        // greedy: RepetitionPenalty -> (forbid stop) -> argmax, lowest index among ties
-        constexpr int VPT = 40;   // ceil(V / 256) for V <= 10240
-        const float* lg = p.logits + (size_t)b * V;
-        float sv[VPT];
-#pragma unroll
-        for (int j = 0; j < VPT; ++j) {
-          const int i = tid + j * NCT;
-          sv[j] = (i < V) ? __ldcg(lg + i) : -INFINITY;
-        }
-        float best = -INFINITY;
-        int bi = 0x7fffffff;
-#pragma unroll
-        for (int j = 0; j < VPT; ++j) {
-          const int i = tid + j * NCT;
-          if (i < V) {
-            float s = sv[j];
-            if ((sm.seen_s[i >> 5] >> (i & 31)) & 1u) s = (s < 0.f) ? s * p.rep_penalty : s / p.rep_penalty;
-            if (i == p.stop_tok && k < p.forbid_stop_before) s = -INFINITY;
-            if (s > best || (s == best && i < bi && s > -INFINITY)) { best = s; bi = i; }
-          }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float b2 = __shfl_xor_sync(0xffffffffu, best, o);
-          const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-          if (b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
-        }
-        if (lane == 0) { sm.att[warp * 2] = best; ((int*)sm.att)[warp * 2 + 1] = bi; }
-        ptx::named_bar_sync(1, NCT);
-        for (int w = 0; w < NCW; ++w) {
-          const float b2 = sm.att[w * 2];
-          const int i2 = ((int*)sm.att)[w * 2 + 1];
-          if (w == 0 || b2 > best || (b2 == best && i2 < bi)) { best = b2; bi = i2; }
-        }
-        tk = bi;
-      }
+      const int tk = pick_token(sample_args(p, s_fin[b]), sm.red, sm.seen_s, p.logits + (size_t)b * V, k, b);
       if (tid == 0 && !s_fin[b]) {
         p.codes[(size_t)b * p.max_new + k] = tk;
         p.nout[b] = k + 1;

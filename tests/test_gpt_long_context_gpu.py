@@ -13,7 +13,7 @@ Contexts run from the prompt (605 rows) to 605 + 1816 = 2421 keys, the model's l
 batch-1 kernel goes through one CTA per head (<= 640 keys) and every key-split count its grid allows (at most
 min(7, SMs / heads) splits), across the 64-step launch boundaries; the 8-sequence kernel through very ragged contexts
 inside one group.  Logits are also checked end to end against the bf16 oracle at the same lengths, and at full depth
-against the round-1 fused kernel."""
+against gpt_fused_kernel with one row, key splits bounded by the grid."""
 import os
 
 import numpy as np
@@ -159,8 +159,8 @@ def test_long_context_logits_vs_oracle(engine):
 
 def test_full_depth_decode1_above_1920_keys(engine):
     """4e. 24 layers, 605-row prompt, 1816 teacher-forced steps (ctx up to 2421, where an unbounded split count would
-    need more CTAs than the grid has): the batch-1 kernel's logits against gpt_fused_kernel<1, .> (IDX_GPT_V2=0 at init,
-    splits bounded by the grid), and its attention of the first and the last layer against the fp64 reference."""
+    need more CTAs than the grid has): the batch-1 kernel's logits against gpt_fused_kernel with one row (IDX_GPT_V2=0 at
+    init, key splits bounded by the grid), and its attention of the first and the last layer against the fp64 reference."""
     cfg = gpt_config()
     w = make_gpt_weights(cfg, seed=2025, bf16=True)
     load_gpt(engine, cfg, w, max_prompt=MAX_PROMPT)

@@ -1,7 +1,7 @@
 """Every GPT decode path's token pick, replayed in fp64 from the exact fp32 logits that path consumed.
 
-The paths: gpt_decode1_kernel (one request), gpt_decode8_kernel (2-8 requests), gpt_fused_kernel at BT = 1 / 8
-(IDX_GPT_V2=0 / IDX_GPT_V8=0 at init), the strict fp32 path (weights_bf16=False), and consecutive decode groups
+The paths: gpt_decode1_kernel (one request), gpt_decode8_kernel (2-8 requests), gpt_fused_kernel with one and with
+three rows (IDX_GPT_V2=0 / IDX_GPT_V8=0 at init), the strict fp32 path (weights_bf16=False), and consecutive decode groups
 (more requests than max_batch, so the Philox sequence index is the group base + row).  Each pick is checked against
 tests/pick_refs.py with zero model noise: greedy picks exactly, sampled picks exactly except where a decision lies
 within fp32 rounding of its boundary (counted, and bounded).  Rows of mel_head.weight set to zero with one bf16-exact
@@ -25,7 +25,7 @@ PATHS = {                     # requests, max_batch, bf16 weights, environment a
     "decode1": (1, 1, True, {}),
     "decode8_3": (3, 8, True, {}),
     "decode8_8": (8, 8, True, {}),
-    "fused_bt1": (1, 1, True, {"IDX_GPT_V2": "0"}),
+    "fused_1": (1, 1, True, {"IDX_GPT_V2": "0"}),
     "fused_bt8": (3, 8, True, {"IDX_GPT_V8": "0"}),
     "strict_1": (1, 1, False, {}),
     "strict_2": (2, 2, False, {}),
@@ -228,7 +228,7 @@ def full():
     return cfg, w, prompts
 
 
-@pytest.mark.parametrize("path", ["decode1", "decode8_3", "fused_bt1"])
+@pytest.mark.parametrize("path", ["decode1", "decode8_3", "fused_1"])
 def test_full_size_picks_replay_exactly(engine, full, path):
     """24 x 1280, V = 8194 (NPL = 40): a greedy and a sampled run of 64 steps, and a greedy tie group at stride 53 over
     V (with 1, start, stop = the V tail) that ties on every step across CTA, warp and thread-slot boundaries."""

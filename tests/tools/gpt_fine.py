@@ -2,7 +2,7 @@
 (middle layer, last step): %globaltimer for the cross-CTA picture, clock64 deltas for the per-CTA costs.
     python -m tests.tools.gpt_fine [steps]
 Environment switches of the library that make sense here: IDX_GPT_DBG (1 skip the MMA loops, 2 skip the attention key
-loop, 4 do not wait in polls), IDX_GPT_RING (ring rows), IDX_GPT_V2=0 (round-1 kernel, old stamp numbering)."""
+loop, 4 do not wait in polls), IDX_GPT_RING (ring rows)."""
 import os
 import sys
 
@@ -72,12 +72,12 @@ def main():
     text = torch.randint(2, 12000, (32,), generator=g)
     prompts = [prepare_gpt_inputs(w, style, emo, text, lang=1, bf16=True).numpy()]
     e.gpt_generate(prompts, 8, 10.0, forbid_stop_before=8)
-    tag = " ".join(f"{k}={os.environ[k]}" for k in ("IDX_GPT_DBG", "IDX_GPT_RING", "IDX_GPT_V2") if k in os.environ) or "default"
+    tag = " ".join(f"{k}={os.environ[k]}" for k in ("IDX_GPT_DBG", "IDX_GPT_RING") if k in os.environ) or "default"
     for rep in range(3):
         e.gpt_generate(prompts, steps, 10.0, forbid_stop_before=steps)
         t = e.gpt_last_timing()
         print(f"[{tag}] decode {t['decode_ms'] / max(1, t['steps']) * 1000:.1f} us/step ({t['steps']} steps)")
-    if os.environ.get("IDX_GPT_V2") == "0" or "-q" in sys.argv:
+    if "-q" in sys.argv:
         e.close()
         return
     e.gpt_profile(True)

@@ -32,16 +32,15 @@ def main():
               f"= {t['decode_ms'] / t['steps'] * 1000:.1f} us/step, launches {t['launches']}")
     st_all = e.gpt_profile(True, read=True)
     import os
-    if batch == 1 and os.environ.get("IDX_GPT_V2") != "0":      # the round-2 batch-1 kernel keeps its own per-CTA timeline: tests/tools/gpt_fine.py
+    if batch == 1 and os.environ.get("IDX_GPT_V2") != "0":      # gpt_decode1_kernel keeps its own per-CTA timeline: tests/tools/gpt_fine.py
         e.close()
         return
     fine = st_all[256:]
     print('fine QKV (ns deltas):', np.diff(fine[:12][fine[:12] > 0]).tolist())
     print('fine FC  (ns deltas):', np.diff(fine[16:28][fine[16:28] > 0]).tolist())
-    fs = fine[32:36]
+    fs = fine[32:35]
     if (fs > 0).all():
-        print('sampling phase (us): seen copy+sync -> logits/penalty', (fs[1] - fs[0]) / 1000, '-> argmax', (fs[2] - fs[1]) / 1000,
-              '-> bookkeeping', (fs[3] - fs[2]) / 1000)
+        print('sampling phase (us): seen copy+sync -> pick', (fs[1] - fs[0]) / 1000, '-> bookkeeping', (fs[2] - fs[1]) / 1000)
     st = st_all[:256]
     st = st[st > 0]
     d = np.diff(st)
