@@ -131,6 +131,7 @@ struct GptParams {
   const long long* stream_off1;   // [G] row offset of CTA i's stream
   int ring_rows;                  // R: rows of D bf16 in the shared-memory ring
   int dbg;                        // diagnostics (IDX_GPT_DBG): 1 skip the MMA loops, 2 skip the attention key loop, 4 do not wait in polls
+  int dbg_hi;                     // bits 32-63 of IDX_GPT_DBG: weight-ring pacing knobs of gpt_decode1_kernel
   uint2* ot;                      // [D] tagged normalised attention output (one CTA per head)
   uint2* partt;                   // [H * 7][66] tagged (m, l, o) partials (long contexts: key splits)
   uint2* cand;                    // [G][2] tagged per-CTA argmax candidate (score, index) / sampling flags
@@ -2202,7 +2203,11 @@ static void fill_common(idx_engine* e, GptState* g, GptParams& p) {
   p.tok = g->tok; p.nout = g->nout; p.finished = g->finished; p.prompt_len = g->prompt_len;
   p.seen = g->seen; p.done = g->done; p.barrier = g->barrier; p.flag = e->dev_flag;
   p.wstream1 = g->wstream1; p.stream_off1 = g->stream_off1; p.ring_rows = g->ring_rows;
-  p.dbg = getenv("IDX_GPT_DBG") ? atoi(getenv("IDX_GPT_DBG")) : 0;
+  {
+    const unsigned long long dbg = getenv("IDX_GPT_DBG") ? strtoull(getenv("IDX_GPT_DBG"), nullptr, 0) : 0ull;
+    p.dbg = (int)(unsigned)(dbg & 0xffffffffull);
+    p.dbg_hi = (int)(unsigned)(dbg >> 32);
+  }
   p.ot = g->ot; p.partt = g->partt; p.cand = g->cand; p.tokt = g->tokt;
   p.prof = g->prof_on ? g->prof : nullptr;
   p.prof2 = g->prof_on ? g->prof2 : nullptr;

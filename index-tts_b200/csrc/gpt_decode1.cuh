@@ -27,8 +27,9 @@
 // (per layer: QKV, O-proj, FC, PROJ; then the head), each a run of consecutive stream rows (its MMA tiles back to back).
 // Phase g lands in ring rows [row(g) mod R ...) with ONE bulk copy (two when it wraps) and completes full[g mod NBAR];
 // There is no producer warp and no "empty" barrier: a phase is free again once all 8 warps have passed the CTA barrier that
-// ends its MMAs, and right there ONE thread (the last one, never an epilogue thread) issues every following phase that
-// now fits (fewer than NBAR outstanding, rows fit behind the consumed ones).  8 warps = 256 threads also lifts the
+// ends its MMAs, and ONE thread (the last one, never an epilogue thread) issues the following phases as they fit (fewer
+// than NBAR outstanding, rows fit behind the consumed ones): right there when the next phase is incomplete, otherwise
+// from inside and after the next hand-over poll, paced by the rows in flight.  8 warps = 256 threads also lifts the
 // register cap from 168 (288 threads are allocated like 384) to 255 per thread.
 
 constexpr int TROWS = 16;       // weight rows per MMA tile
@@ -168,14 +169,17 @@ __device__ __forceinline__ float red_sum(const float* red, int item, int row) {
 // stored when all 256 threads of all CTAs re-read their whole slice in every round — CTAs x 4 sector reads per 128-byte
 // line per round queue at the L2 slice that holds the line, in front of the very stores the pollers wait for.  So a warp
 // first spins on ONE word (all lanes the same address = one request per warp per round, the word chosen per (CTA, warp)
-// so the spinners spread over the lines) and only then checks its whole slice.
-template <int N>
-__device__ __forceinline__ void poll_slice(const uint2* base, int first, unsigned epoch, float (&v)[N], int spin_idx, bool nowait) {
+// so the spinners spread over the lines) and only then checks its whole slice.  `on_spin` runs once per round while the
+// load is in flight (the weight producer issues ring rows from there).
+template <int N, class F>
+__device__ __forceinline__ void poll_slice(const uint2* base, int first, unsigned epoch, float (&v)[N], int spin_idx, bool nowait,
+                                           F&& on_spin) {
   if (!nowait) {
     unsigned spins = 0, tag;
     do {
       asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(tag) : "l"((const unsigned*)(base + spin_idx) + 1) : "memory");
       if (++spins > (1u << 26)) __trap();
+      on_spin();
     } while (tag != epoch);
   }
   ld_tagged_slice<N>(base, first, epoch, v, nowait);
@@ -262,7 +266,17 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
     // Measured over 256 steps (us / step): whole phases only 445.2; instalments, no cap 433.1; cap 24: 432.8; cap 18: 425.5; cap 12: 436.5.
     constexpr int MINPART = 4;
     const int cap = ((p.dbg >> 8) & 0xff) ? ((p.dbg >> 8) & 0xff) : 18;
+    // Paced issues (after a poll and while spinning in one) are also bounded by the rows IN FLIGHT — issued, phase not yet
+    // seen complete — so that the copies keep flowing through a hand-over wait without every CTA starting a large burst
+    // at once.  IDX_GPT_DBG bits 32-39: in-flight target in rows; bits 40-47: spin rounds between two issue attempts
+    // inside a poll; bit 4: no issues from inside the polls.
+    const int target = (p.dbg_hi & 0xff) ? (p.dbg_hi & 0xff) : 54;
+    const int spin_every = ((p.dbg_hi >> 8) & 0xff) ? ((p.dbg_hi >> 8) & 0xff) : 8;
+    const bool spin_issue = is_prod && !(p.dbg & 16);
     int part = 0;                     // rows of phase pidx already issued
+    unsigned landed = 0;              // phases known to be complete: every phase before `landed` (landed >= cons_tile)
+    int lpidx = 0;                    // phase inside the step of phase `landed`
+    int inflight = 0;                 // rows of phases [landed, tix) plus the issued part of phase tix
     auto issue_fitting = [&](int budget = 0) {
       if (!is_prod) return;
       if (budget <= 0) budget = cap;
@@ -281,6 +295,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
         wpos += m;
         if (wpos >= R) wpos -= R;
         fill += m;
+        inflight += m;
         uoff += m;
         budget -= m;
         if (!last) { part += m; break; }
@@ -288,6 +303,25 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
         ++tix;
         if (++pidx == pps) { pidx = 0; uoff = 0; ++pstep; }
       }
+    };
+    // Phases [landed, tix) are tested in order without blocking.  The parity test is unambiguous: phase n >= cons_tile
+    // is outstanding, so its slot has not been re-armed for phase n + NBAR (fewer than NBAR phases are outstanding).
+    auto note_landed = [&]() {
+      while (landed < tix && ptx::mbar_test_wait(&sm.full[landed % NBAR], (landed / NBAR) & 1u)) {
+        inflight -= sc.rows(lpidx);
+        ++landed;
+        if (++lpidx == pps) lpidx = 0;
+      }
+    };
+    auto issue_paced = [&]() {
+      if (!is_prod) return;
+      note_landed();
+      const int budget = min(cap, target - inflight);
+      if (budget > 0) issue_fitting(budget);
+    };
+    unsigned spin_n = 0;
+    auto on_spin = [&]() {            // inside a hand-over poll: the other threads only spin
+      if (spin_issue && ++spin_n >= (unsigned)spin_every) { spin_n = 0; issue_paced(); }
     };
     const int b = 0;                  // the one sequence
     const int plen = __ldg(p.prompt_len + b);
@@ -337,17 +371,25 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
     // called right after mma_items (which ends with a CTA barrier: every warp is done with the phase's rows)
     auto advance = [&](const Phase1& ph) {
       const int tot = ph.total;
+      if (landed == cons_tile) {      // a consumed phase has landed (keeps landed >= cons_tile)
+        inflight -= tot;
+        ++landed;
+        if (++lpidx == pps) lpidx = 0;
+      }
       cons_row += tot;
       if (cons_row >= R) cons_row -= R;
       ++cons_tile;
       fill -= tot;
       if ((p.dbg & 8) || tix == cons_tile) issue_fitting(max(cap, sc.rows(pidx) - part));   // the phase consumed next is not (completely) issued: all of it at once; dbg 8 = always
     };
-    // The freed rows are refilled a little later — right after this CTA's NEXT hand-over poll has completed: at the release
-    // point all CTAs would start their 60-90 KB bulk copies together, exactly when the epilogue stores and the polls of
-    // the hand-over (the latency-critical traffic) are in flight; the ring holds two to three phases, so the weights issued
-    // one poll later still arrive long before they are consumed.
-    auto refill = [&]() { if (!(p.dbg & 8)) issue_fitting(); };
+    // The freed rows are refilled a little later — from inside this CTA's NEXT hand-over poll (on_spin) and right after it
+    // has completed: at the release point all CTAs would start their 60-90 KB bulk copies together, exactly when the
+    // epilogue stores and the polls of the hand-over (the latency-critical traffic) are in flight.  Issuing only after the
+    // poll left HBM idle through the wait: on H100 the 112 CTAs that own no head wait ~9 us for the attention output with
+    // the QKV phase's rows free and nothing in flight.  H100 SXM (700 W), 256 steps, us per step: after the poll only 552;
+    // from inside the polls every 8 rounds (the default) 515, every round 543-573 (the early copies land on top of the
+    // attention's K/V reads), from every poll but the o poll 549 (the gain is the long o wait).
+    auto refill = [&]() { if (!(p.dbg & 8)) issue_paced(); };
     issue_fitting(R);                 // initial fill
 
     for (int step = 0; step < p.nsteps && !already_done; ++step) {
@@ -386,7 +428,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
         {
           float v[NPL / 8];
           if (l > 0) {
-            poll_slice<NPL / 8>(p.xt, warp * (NPL * 4) + lane, ep_base, v, spin_x, nowait);
+            poll_slice<NPL / 8>(p.xt, warp * (NPL * 4) + lane, ep_base, v, spin_x, nowait, on_spin);
           } else {
 #pragma unroll
             for (int j = 0; j < NPL / 8; ++j) v[j] = v0[j];
@@ -595,7 +637,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
         // ---------------- P3: attention output -> O-proj + residual ----------------
         if (nsplit == 1) {
           float v[NPL / 8];
-          poll_slice<NPL / 8>(p.ot, warp * (NPL * 4) + lane, ep_oproj, v, spin_x, nowait);
+          poll_slice<NPL / 8>(p.ot, warp * (NPL * 4) + lane, ep_oproj, v, spin_x, nowait, on_spin);
           G2(11);
           refill();
 #pragma unroll
@@ -618,6 +660,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
                   wa[s] = ld_tagged_word(pp + s * PART_STRIDE + 2 + lane);
                   wb[s] = ld_tagged_word(pp + s * PART_STRIDE + 34 + lane);
                 }
+              on_spin();
 #pragma unroll
               for (int s = 0; s < 7; ++s)
                 if (s < nsplit) ok &= (wm[s].y == ep_oproj) & (wl[s].y == ep_oproj) & (wa[s].y == ep_oproj) & (wb[s].y == ep_oproj);
@@ -664,7 +707,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
         else prefetch_ln(0, p.lnf_w, p.lnf_b);
         {
           float v[NPL / 8];
-          poll_slice<NPL / 8>(p.xt, warp * (NPL * 4) + lane, ep_oproj, v, spin_x, nowait);
+          poll_slice<NPL / 8>(p.xt, warp * (NPL * 4) + lane, ep_oproj, v, spin_x, nowait, on_spin);
           G2(16);
           refill();
           cp_async_wait_all();   // ln_2 parameters prefetched in P1 (ln_block's own CTA barrier publishes them)
@@ -712,6 +755,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
             do {
               asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(wv) : "l"(p.ft + spin_f) : "memory");
               if (++spins > (1u << 26)) __trap();
+              on_spin();
             } while ((wv & 0xffff0000u) != want);
           }
           do {
@@ -767,7 +811,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode1_kernel(const GptParams p) 
       const unsigned ep_head = p.epoch0 + (unsigned)(step * L + L - 1) * 2u + 2u;
       {
         float v[NPL / 8];
-        poll_slice<NPL / 8>(p.xt, warp * (NPL * 4) + lane, ep_head, v, spin_x, nowait);
+        poll_slice<NPL / 8>(p.xt, warp * (NPL * 4) + lane, ep_head, v, spin_x, nowait, on_spin);
         refill();
         ln_block<NPL>(v, lnA, lnA + D, sm.red_ln, warp, lane);
         ln_block<NPL>(v, lnB, lnB + D, sm.red_ln + 3 * NCW, warp, lane);

@@ -46,6 +46,21 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+// test_wait never suspends the thread (try_wait may, up to a system-dependent time limit): for a thread that only wants
+// to know whether a phase has completed and has other work to do either way
+__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+      "selp.b32 %0, 1, 0, p;\n"
+      "}\n"
+      : "=r"(ok)
+      : "r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
 // Bounded wait: a protocol bug must become a trapped kernel (reported as a CUDA error),
 // never a hung GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
