@@ -10,9 +10,10 @@
 // Layout: activations are channels-last fp32 [B][T][C] so that
 //   * every Conv1d is a multi-tap GEMM with M = time, N = C_out, K = C_in (ops.h), zero padding
 //     comes from the row bounds of the A operand (TMA out-of-bounds fill on the wgmma path);
-//   * ConvTranspose1d(k = 2u, stride u, pad u/2) is the SAME 2-tap GEMM with N = u*C_out: output
-//     phase r of frame q lands at flat offset (q*u + r - pad)*C_out + co, i.e. the GEMM's row q
-//     is a contiguous run of the upsampled signal (shifted by -pad*C_out) — no scatter;
+//   * ConvTranspose1d(k = n*u, stride u, pad (k - u)/2) is the SAME n-tap GEMM with N = u*C_out (n = 2
+//     in BigVGAN-v2; the v1.5 generator also has k = u, n = 1): output phase r of frame q lands at
+//     flat offset (q*u + r - pad)*C_out + co, i.e. the GEMM's row q is a contiguous run of the
+//     upsampled signal (shifted by -pad*C_out) — no scatter;
 //   * the anti-aliased SnakeBeta is ONE fused kernel (2x FIR upsample → snake → FIR downsample)
 //     that reads x once and writes once; threads map to channels (coalesced) and slide along
 //     time with a 6-sample input window and a 12-sample activated window in registers.
@@ -153,21 +154,21 @@ __global__ void pack_conv_kernel(const float* w, float* wsimt, float* wk, int Co
   wsimt[((long long)kk * Ci + ci) * Co + co] = v;
   wk[(long long)co * k * Ci + (long long)kk * Ci + ci] = v;
 }
-// ConvTranspose1d weight [Ci][Co][2u] -> 2-tap GEMM weights with N = u*Co:
-//   tap 0 (x[q])   : W[ci][co][r],   tap 1 (x[q-1]) : W[ci][co][r+u]
-//   Wsimt [2][Ci][u*Co],  Wk [u*Co][2*Ci]
-__global__ void pack_convT_kernel(const float* w, float* wsimt, float* wk, int Ci, int Co, int u) {
+// ConvTranspose1d weight [Ci][Co][nt*u] -> nt-tap GEMM weights with N = u*Co:
+//   tap t (x[q-t]) : W[ci][co][r + t*u]
+//   Wsimt [nt][Ci][u*Co],  Wk [u*Co][nt*Ci]
+__global__ void pack_convT_kernel(const float* w, float* wsimt, float* wk, int Ci, int Co, int u, int nt) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long n = (long long)Ci * Co * 2 * u;
+  long long n = (long long)Ci * Co * nt * u;
   if (i >= n) return;
-  int kk = i % (2 * u);
-  int co = (i / (2 * u)) % Co;
-  int ci = i / ((long long)2 * u * Co);
+  int kk = i % (nt * u);
+  int co = (i / (nt * u)) % Co;
+  int ci = i / ((long long)nt * u * Co);
   int tap = kk / u, r = kk % u;
   float v = w[i];
   int j = r * Co + co;
   wsimt[((long long)tap * Ci + ci) * ((long long)u * Co) + j] = v;
-  wk[(long long)j * 2 * Ci + (long long)tap * Ci + ci] = v;
+  wk[(long long)j * nt * Ci + (long long)tap * Ci + ci] = v;
 }
 
 }  // namespace
@@ -286,7 +287,8 @@ static void bigvgan_build(idx_engine* e, const idx_bigvgan_config* cfg, const st
   int ch = cfg->upsample_initial_channel;
   for (int i = 0; i < cfg->num_upsamples; ++i) {
     const int u = cfg->upsample_rates[i], k = cfg->upsample_kernel_sizes[i];
-    IDX_CHECK(k == 2 * u && u % 2 == 0, IDX_ERR_ARG, "ConvTranspose1d must have kernel = 2*stride, even stride");
+    IDX_CHECK(u >= 1 && k >= u && k % u == 0 && (k - u) % 2 == 0, IDX_ERR_ARG,
+              "ConvTranspose1d kernel must be a multiple of its stride, with an even difference (padding (k - u) / 2)");
     const std::string name = P + "ups." + std::to_string(i) + ".0";
     const DevTensor& w = e->W(name + ".weight");
     IDX_CHECK(w.shape.size() == 3 && w.shape[0] == ch && w.shape[1] == ch / 2 && w.shape[2] == k, IDX_ERR_ARG, name + ".weight shape");
@@ -295,7 +297,7 @@ static void bigvgan_build(idx_engine* e, const idx_bigvgan_config* cfg, const st
     size_t n = w.numel();
     c.wsimt = balloc(s, n);
     c.wk = balloc(s, n);
-    pack_convT_kernel<<<(unsigned)((n + 255) / 256), 256, 0, e->stream>>>((const float*)w.d, c.wsimt, c.wk, c.Ci, c.Co, u);
+    pack_convT_kernel<<<(unsigned)((n + 255) / 256), 256, 0, e->stream>>>((const float*)w.d, c.wsimt, c.wk, c.Ci, c.Co, u, k / u);
     IDX_CUDA(cudaGetLastError());
     c.bias = e->has(name + ".bias") ? e->Wf(name + ".bias") : nullptr;
     s->ups.push_back(c);
@@ -392,12 +394,13 @@ static void run_conv(idx_engine* e, const ConvW& c, const float* x, float* out, 
 }
 
 static void run_convT(idx_engine* e, const ConvW& c, int u, const float* x, float* out, int B, int T) {
-  // rows q = 0..T ; tap0 reads x[q] (zero at q = T), tap1 reads x[q-1] (zero at q = 0)
+  // nt = k / u taps; rows q = 0..T+nt-2, tap t reads x[q-t] (zero outside 0..T-1)
+  const int nt = c.k / u;
   ConvGemm g;
   g.A = x; g.B = B; g.Tin = T; g.K = c.Ci;
   g.W = c.wsimt; g.Wk = c.wk;
-  g.taps = 2; g.dil = -1; g.pad = 0;
-  g.M = T + 1; g.N = u * c.Co; g.bias = c.bias; g.biasN = c.Co;
+  g.taps = nt; g.dil = -1; g.pad = 0;
+  g.M = T + nt - 1; g.N = u * c.Co; g.bias = c.bias; g.biasN = c.Co;
   const int pad = (c.k - u) / 2;
   g.out = out;
   g.ldo = u * c.Co;

@@ -2497,6 +2497,9 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   IDX_CHECK(!sp->do_sample || (std::isfinite(sp->temperature) && sp->temperature > 0.f), IDX_ERR_ARG,
             "do_sample needs a finite temperature > 0");
   IDX_CHECK(!sp->do_sample || (sp->top_p >= 0.f && sp->top_p <= 1.f), IDX_ERR_ARG, "do_sample needs 0 <= top_p <= 1");
+  // the paths read the mode as `mel_pos_mode == 1`: any other value would silently decode with the KV-cache rule
+  IDX_CHECK(sp->mel_pos_mode == 0 || sp->mel_pos_mode == 1, IDX_ERR_ARG,
+            "mel_pos_mode must be 0 (mel position k + 1 at step k >= 1, KV cache) or 1 (position k, no cache)");
   // an armed attention probe is consumed by this call, whatever its outcome
   const int probe_on = g->probe_armed, pprobe_on = g->pprobe_armed;
   g->probe_armed = g->pprobe_armed = 0;
@@ -2881,7 +2884,6 @@ extern "C" int idx_gpt_latents_v1(idx_engine* e, const float* conds, int n_laten
   GptStrict* s = g->strict;
   const int D = g->cfg.model_dim, R = n_latents + n_text + 2 + n_codes + 2;
   IDX_CHECK(R <= g->maxpos, IDX_ERR_ARG, "sequence longer than the KV cache");
-  for (int i = 0; i < n_codes; ++i) (void)i;
   e->ensure_arena(4 * ((size_t)(2 * R + n_latents + 2 * n_codes + 2) * D + (size_t)n_text + n_codes + 32) +
                   (size_t)(R / 8 + 2) * sizeof(PrefillTile) + (1 << 16));
   e->arena.reset();

@@ -99,7 +99,7 @@ def kaiser_sinc_filter1d(cutoff=0.25, half_width=0.3, kernel_size=12):  # filter
     return filt.view(1, 1, kernel_size)
 
 
-def make_bigvgan_weights(h, seed=1234):
+def make_bigvgan_weights(h, seed=1234, post_gain=0.06):
     """Seeded synthetic generator weights under the reference state-dict names (weight norm
     already removed).  Conv weights are scaled to 1/sqrt(fan_in) so activations neither vanish
     nor explode through the 6 stages (the reference's std 0.01 init, bigvgan/utils.py:45-48,
@@ -135,7 +135,7 @@ def make_bigvgan_weights(h, seed=1234):
             for q in range(6):
                 act(f"resblocks.{rb}.activations.{q}", ch)
     act("activation_post", ch)
-    conv("conv_post", 1, ch, 7, bias=h.get("use_bias_at_final", True), gain=0.06)
+    conv("conv_post", 1, ch, 7, bias=h.get("use_bias_at_final", True), gain=post_gain)
     return w
 
 
@@ -367,6 +367,28 @@ def small_v1_config():
                 cond_d_vector_in_each_upsampling_layer=True, speaker_embedding_dim=24, num_mels=20)
 
 
+def v1_5_config():
+    """The IndexTTS-1.5 vocoder: 1280-d GPT latents -> 1536 channels, six upsamples (x1024, 24 kHz), AMPBlock1 with
+    kernels 3/7/11, snakebeta, the speaker embedding added after conv_pre and after every upsample.
+
+    [ASSUMED] from the published IndexTTS-1.5 checkpoints/config.yaml, which the reference checkout does not carry;
+    consistent with SURVEY section 8 row a13 (1280-d latents, x1024, 24 kHz).  Its GPT is
+    gpt_config(max_mel_tokens=605, max_text_tokens=402) with the V1_COND_CFG conditioning encoder, also [ASSUMED]."""
+    return dict(gpt_dim=1280, upsample_rates=[4, 4, 4, 4, 2, 2], upsample_kernel_sizes=[8, 8, 4, 4, 4, 4],
+                upsample_initial_channel=1536, resblock="1", resblock_kernel_sizes=[3, 7, 11],
+                resblock_dilation_sizes=[[1, 3, 5], [1, 3, 5], [1, 3, 5]], activation="snakebeta", snake_logscale=True,
+                feat_upsample=False, cond_d_vector_in_each_upsampling_layer=True, speaker_embedding_dim=512, num_mels=100)
+
+
+V1_5_POST_GAIN = 0.012      # conv_post gain of the v1.5 test weights (make_bigvgan_v1_weights)
+
+
+# v1 / v1.5 conditioning encoder (gpt/model.py:352-363): conformer over a 100-bin mel (512 dims, 2048 FF units, 8 heads,
+# 6 blocks) and a 32-latent perceiver at p_dim = model_dim = 1280
+V1_COND_CFG = dict(idim=100, odim=512, linear_units=2048, heads=8, blocks=6, cnn_kernel=15, p_dim=1280, p_heads=8,
+                   p_dim_head=64, p_depth=2, p_ff_mult=2, model_dim=1280)
+
+
 def make_ecapa_weights(n_mels, emb_dim, seed=99, prefix="speaker_encoder.", channels=(512, 512, 512, 512, 1536),
                        kernel_sizes=(5, 3, 3, 3, 1), scale=8, se_channels=128, attention_channels=128):
     """Seeded ECAPA-TDNN weights under the reference state-dict names (ECAPA_TDNN.py:470-541), BatchNorm running
@@ -408,10 +430,12 @@ def make_ecapa_weights(n_mels, emb_dim, seed=99, prefix="speaker_encoder.", chan
     return w
 
 
-def make_bigvgan_v1_weights(h, seed=4321):
-    """Seeded weights of the latent-conditioned v1 BigVGAN under the reference state-dict names (weight norm removed)."""
+def make_bigvgan_v1_weights(h, seed=4321, post_gain=0.06):
+    """Seeded weights of the latent-conditioned v1 BigVGAN under the reference state-dict names (weight norm removed).
+    `post_gain` scales conv_post: at the v1.5 geometry the default drives 1/3 of the samples into tanh saturation, where
+    the waveform hides the generator's errors; V1_5_POST_GAIN keeps it in the near-linear range."""
     h2 = dict(h, num_mels=h["gpt_dim"], use_bias_at_final=True)
-    w = make_bigvgan_weights(h2, seed=seed)                 # same generator layout: conv_pre takes gpt_dim channels
+    w = make_bigvgan_weights(h2, seed=seed, post_gain=post_gain)   # same generator layout: conv_pre takes gpt_dim channels
     g = torch.Generator().manual_seed(seed + 1)
     E, ch = h["speaker_embedding_dim"], h["upsample_initial_channel"]
     w["cond_layer.weight"] = torch.randn(ch, E, 1, generator=g) * (0.5 / math.sqrt(E))

@@ -182,8 +182,8 @@ class GptOracle:
             kh = K.view(S, H, hd).transpose(0, 1)
             vh = Vv.view(S, H, hd).transpose(0, 1)
             sc = (qh @ kh.transpose(1, 2)) / math.sqrt(hd)          # transformers_gpt2.py:199-203
-            qpos = torch.arange(S - T, S)[:, None]
-            mask = torch.arange(S)[None, :] <= qpos
+            qpos = torch.arange(S - T, S, device=x.device)[:, None]
+            mask = torch.arange(S, device=x.device)[None, :] <= qpos
             sc = sc.masked_fill(~mask[None], float("-inf"))
             a = rr((torch.softmax(sc, dim=-1) @ vh).transpose(0, 1).reshape(T, D))
             o = rr(a @ w[p + "attn.c_proj.weight"] + w[p + "attn.c_proj.bias"])
@@ -208,7 +208,7 @@ class GptOracle:
         cfg, w, rr = self.cfg, self.w, self.rr
         start, stop = cfg["start_mel_token"], cfg["stop_mel_token"]
         self.reset()
-        prompt_emb = torch.as_tensor(prompt_emb, dtype=torch.float32)
+        prompt_emb = torch.as_tensor(prompt_emb, dtype=torch.float32).to(w["mel_embedding.weight"])
         first = rr(w["mel_embedding.weight"][start] + w["mel_pos_embedding.emb.weight"][0])
         x = torch.cat([prompt_emb, first[None]], dim=0)                       # model_v2.py:146-156
         hidden = self.forward_rows(x)[-1:]
@@ -218,13 +218,13 @@ class GptOracle:
             lg = self.logits(hidden)[0]
             all_logits.append(lg.clone())
             s = lg.clone()
-            idx = torch.tensor(sorted(seen))
+            idx = torch.tensor(sorted(seen), device=s.device)
             sv = s[idx]
             s[idx] = torch.where(sv < 0, sv * repetition_penalty, sv / repetition_penalty)
             if k < forbid_stop_before:
                 s[stop] = float("-inf")
             if do_sample:
-                sc = (s.numpy().astype(np.float32) * np.float32(1.0 / temperature)).astype(np.float32)
+                sc = (s.cpu().numpy().astype(np.float32) * np.float32(1.0 / temperature)).astype(np.float32)
                 tok, _ = sample_token(sc, top_k, top_p, seed, k, seq)
             else:
                 tok = int(torch.argmax(s))  # first maximal index on CPU
@@ -237,4 +237,4 @@ class GptOracle:
             seen.add(feed)
             emb = rr(w["mel_embedding.weight"][feed] + w["mel_pos_embedding.emb.weight"][k + 2])
             hidden = self.forward_rows(emb[None])                             # position k+2 (P1)
-        return np.array(codes, dtype=np.int32), torch.stack(all_logits).numpy()
+        return np.array(codes, dtype=np.int32), torch.stack(all_logits).cpu().numpy()

@@ -1,6 +1,7 @@
-"""Mint tests/golden/v1_vocoder_small.npz from the reference's own v1 `BigVGAN` (indextts/BigVGAN/models.py:129-249, which
-owns the ECAPA-TDNN speaker encoder, ECAPA_TDNN.py:429-582) with the seeded weights of index-tts_b200/synth.py loaded into
-it.  Build container only.
+"""Mint tests/golden/v1_vocoder_small.npz and (at the IndexTTS-1.5 geometry, synth.v1_5_config) v1_vocoder_full.npz from
+the reference's own v1 `BigVGAN` (indextts/BigVGAN/models.py:129-249, which owns the ECAPA-TDNN speaker encoder,
+ECAPA_TDNN.py:429-582) with the seeded weights of index-tts_b200/synth.py loaded into it, and v1_gpt_small.npz from its v1
+UnifiedVoice.  Needs the reference checkout.
     python -m oracle.make_goldens_v1"""
 import os
 
@@ -45,6 +46,32 @@ def main():
     assert e1 < 1e-4 and e2 < 1e-5
     out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "v1_vocoder_small.npz")
     np.savez_compressed(out, seed=seed, latent=latent.numpy(), mel_ref=mel_ref.numpy(), spk=spk_ref.numpy(), wav=wav_ref.numpy())
+    print("wrote", out)
+
+
+FULL_SEED = 1515
+
+
+def main_full():
+    """The real v1.5 vocoder (1536 channels, x1024, conv_pre K = 7 * 1280) on T = 4 latents (4096 samples) and a 61-frame
+    reference mel.  Only the inputs and outputs are stored: the weights are regenerated from the seed."""
+    h = synth.v1_5_config()
+    w = synth.make_bigvgan_v1_weights(h, seed=FULL_SEED, post_gain=synth.V1_5_POST_GAIN)
+    m = reference_module(h, w)
+    g = torch.Generator().manual_seed(8)
+    latent = torch.randn(1, 4, h["gpt_dim"], generator=g)
+    mel_ref = torch.randn(1, 61, h["num_mels"], generator=g) * 1.5 - 4.0
+    with torch.no_grad():
+        spk_ref = m.speaker_encoder(mel_ref, torch.tensor([1.0]))
+        wav_ref, _ = m(latent, mel_ref, torch.tensor([1.0]))
+    wav = v1.bigvgan_v1_forward(h, w, latent, mel_ref)
+    e = float((wav - wav_ref).abs().max())
+    print(f"v1.5 vocoder: wav [{tuple(wav_ref.shape)}] max |diff| vs reference {e:.2e} "
+          f"(rms {float(wav_ref.pow(2).mean().sqrt()):.3f})")
+    assert wav_ref.shape == (1, 1, 4 * 1024) and e < 1e-5
+    out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "v1_vocoder_full.npz")
+    np.savez_compressed(out, seed=FULL_SEED, latent=latent.numpy(), mel_ref=mel_ref.numpy(), spk=spk_ref.numpy(),
+                        wav=wav_ref.numpy())
     print("wrote", out)
 
 
@@ -111,4 +138,5 @@ def main_gpt():
 
 if __name__ == "__main__":
     main()
+    main_full()
     main_gpt()

@@ -13,8 +13,10 @@ BASELINE config 1): the ECAPA-TDNN speaker encoder and the latent-conditioned Bi
                                      oracle/bigvgan.py)
 
 Pinned against the reference's own `indextts.BigVGAN.models.BigVGAN` (which owns the ECAPA encoder) by
-oracle/make_goldens_v1.py -> tests/golden/v1_vocoder_small.npz.  The CUDA side of row a13 is NOT built yet
-(DESIGN.md section 1): this file and its goldens are the checker it will be built against."""
+oracle/make_goldens_v1.py -> tests/golden/v1_vocoder_small.npz and, at the IndexTTS-1.5 geometry,
+tests/golden/v1_vocoder_full.npz.  The CUDA side (csrc/bigvgan.cu, csrc/ecapa.cu) is checked against it by
+tests/test_v1_gpu.py and, at full size in float64 on the GPU, tests/test_v1_full_gpu.py.  The GPT-side functions below
+run on whatever device and dtype the weights are on."""
 import numpy as np
 import torch
 import torch.nn.functional as F
@@ -167,18 +169,18 @@ def generate_v1(oracle, prompt, max_new, repetition_penalty=10.0, kv_cache=False
         return oracle.generate(prompt, max_new, repetition_penalty, 0)
     w, cfg = oracle.w, oracle.cfg
     start, stop = cfg["start_mel_token"], cfg["stop_mel_token"]
-    prompt = torch.as_tensor(prompt, dtype=torch.float32)
+    prompt = torch.as_tensor(prompt, dtype=torch.float32).to(w["mel_embedding.weight"])
     toks, codes, logits = [start], [], []
     seen = {1, start}
     for k in range(max_new):
         oracle.reset()
-        t = torch.tensor(toks)
+        t = torch.tensor(toks, device=prompt.device)
         emb = w["mel_embedding.weight"][t] + w["mel_pos_embedding.emb.weight"][: len(toks)]
         hidden = oracle.forward_rows(torch.cat([prompt, emb], 0))[-1:]
         lg = oracle.logits(hidden)[0]
         logits.append(lg.clone())
         s = lg.clone()
-        idx = torch.tensor(sorted(seen))
+        idx = torch.tensor(sorted(seen), device=s.device)
         sv = s[idx]
         s[idx] = torch.where(sv < 0, sv * repetition_penalty, sv / repetition_penalty)
         tok = int(torch.argmax(s))
@@ -187,7 +189,7 @@ def generate_v1(oracle, prompt, max_new, repetition_penalty=10.0, kv_cache=False
             break
         toks.append(tok)
         seen.add(tok)
-    return np.array(codes, dtype=np.int32), torch.stack(logits).numpy()
+    return np.array(codes, dtype=np.int32), torch.stack(logits).cpu().numpy()
 
 
 @torch.no_grad()
@@ -195,10 +197,11 @@ def latents_v1(oracle, conds, text_ids, codes):
     """UnifiedVoice.forward(..., return_latent=True) (model.py:526-589) for one utterance: final_norm(ln_f(hidden)) at the
     mel positions [start_mel, codes..., stop_mel] minus the last two -> [len(codes), D]  (what BigVGAN v1 consumes)."""
     w, cfg = oracle.w, oracle.cfg
-    ids = torch.as_tensor(text_ids, dtype=torch.long)
+    dev = w["mel_embedding.weight"].device
+    ids = torch.as_tensor(np.asarray(text_ids), dtype=torch.long, device=dev)
     ids = F.pad(F.pad(ids, (0, 1), value=1), (1, 0), value=0)            # stop appended, then start prepended (:565-569)
     text_emb = w["text_embedding.weight"][ids] + w["text_pos_embedding.emb.weight"][: ids.shape[0]]
-    mel = torch.as_tensor(np.asarray(codes), dtype=torch.long)
+    mel = torch.as_tensor(np.asarray(codes), dtype=torch.long, device=dev)
     mel = F.pad(F.pad(mel, (0, 1), value=cfg["stop_mel_token"]), (1, 0), value=cfg["start_mel_token"])
     mel_emb = w["mel_embedding.weight"][mel] + w["mel_pos_embedding.emb.weight"][: mel.shape[0]]
     oracle.reset()

@@ -13,6 +13,7 @@ import pytest
 import torch
 
 from indextts_b200 import synth
+from indextts_b200.synth import V1_COND_CFG
 from oracle import v1
 from oracle.emo import EMO_CFG, get_emovec, make_emo_weights
 
@@ -20,8 +21,6 @@ pytestmark = pytest.mark.gpu
 
 U = 2.0 ** -24
 LENGTHS = [3, 4, 64, 65, 91, 129, 750]
-V1_COND_CFG = dict(idim=100, odim=512, linear_units=2048, heads=8, blocks=6, cnn_kernel=15, p_dim=1280, p_heads=8,
-                   p_dim_head=64, p_depth=2, p_ff_mult=2, model_dim=1280)
 
 
 def _on_gpu(w):

@@ -1,6 +1,8 @@
 """CPU: the v1 / v1.5 vocoder-side restatement (oracle/v1.py: ECAPA-TDNN speaker encoder + latent-conditioned BigVGAN,
 SURVEY section 8 row a13) against outputs of the reference's own `indextts.BigVGAN.models.BigVGAN`
-(tests/golden/v1_vocoder_small.npz, oracle/make_goldens_v1.py).  The CUDA side of a13 is not built yet."""
+(tests/golden/v1_vocoder_small.npz and, at the IndexTTS-1.5 geometry, v1_vocoder_full.npz; oracle/make_goldens_v1.py)
+and of the v1 UnifiedVoice (v1_gpt_small.npz).  The CUDA side is checked against this restatement by tests/test_v1_gpu.py
+and tests/test_v1_full_gpu.py."""
 import os
 
 import numpy as np
@@ -27,6 +29,23 @@ def test_ecapa_and_bigvgan_v1_match_reference_module():
     # the speaker embedding really conditions the waveform
     wav2 = v1.bigvgan_v1_forward(h, w, latent, mel_ref.flip(1) * 0.5).numpy()
     assert np.abs(wav2 - wav).max() > 1e-3
+
+
+def test_bigvgan_v1_5_geometry_matches_reference_module():
+    """The real v1.5 generator (synth.v1_5_config: 1280 -> 1536 channels, six upsamples, x1024, kernels 3/7/11, speaker
+    embedding folded in after conv_pre and after each upsample) on 4 latents and a 61-frame reference mel."""
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "v1_vocoder_full.npz"))
+    h = synth.v1_5_config()
+    w = synth.make_bigvgan_v1_weights(h, seed=int(g["seed"]), post_gain=synth.V1_5_POST_GAIN)
+    latent, mel_ref = torch.from_numpy(g["latent"]), torch.from_numpy(g["mel_ref"])
+    assert latent.shape == (1, 4, 1280) and mel_ref.shape == (1, 61, 100)
+    spk = v1.ecapa_tdnn(w, mel_ref).numpy()
+    assert spk.shape == g["spk"].shape == (1, 1, 512)
+    assert np.abs(spk - g["spk"]).max() <= 1e-4 * max(1.0, float(np.abs(g["spk"]).max()))
+    wav = v1.bigvgan_v1_forward(h, w, latent, mel_ref).numpy()
+    assert wav.shape == g["wav"].shape == (1, 1, 4 * 1024)
+    assert np.abs(wav - g["wav"]).max() <= 1e-5
+    assert np.abs(wav).max() < 1.0
 
 
 def test_v1_gpt_side_matches_reference_unifiedvoice():
