@@ -123,7 +123,10 @@ typedef struct {
   int32_t do_sample;            /* 0: greedy argmax                                  */
   int32_t num_beams;            /* 1, or 2..4: beam search (do_sample = 1: beam-sample,
                                    the reference default num_beams = 3); each request
-                                   then occupies num_beams rows: nreq * num_beams <= 8 */
+                                   then occupies num_beams rows: nreq * num_beams <= 8.
+                                   Strict fp32 path (weights_bf16 = 0): requests run one
+                                   at a time, num_beams <= max_batch (one KV slot per
+                                   beam); forced_codes is refused with beams          */
   int32_t top_k;                /* 0 = off                                           */
   float top_p;                  /* 1.0 = off                                         */
   float temperature;            /* 1.0 = off                                         */
@@ -239,7 +242,8 @@ int idx_gpt_latents_v1(idx_engine* e, const float* conds, int n_latents, const i
  * beam slot the (parent beam, token) chosen by BeamSearchScorer.process
  * (gpt/transformers_beam_search.py:215-320) and the running beam score; the score of the returned hypothesis
  * (BeamSearchScorer.finalize :322-420).  Steps run after an utterance is done record the identity reorder: parent j
- * for beam j, the stop token, the unchanged beam score.
+ * for beam j, the stop token, the unchanged beam score.  steps_out is the utterance's own step count (on the strict
+ * path each request of a call runs, and may stop, on its own).
  *   parents_tokens [max_steps][num_beams][2] i32, scores [max_steps][num_beams] f32 (either may be NULL)    */
 int idx_gpt_beam_trace(const idx_engine* e, int utterance, int32_t* parents_tokens, float* scores,
                        int max_steps, int32_t* steps_out, double* final_score);

@@ -1189,21 +1189,24 @@ __global__ void prepare_inputs_kernel(const float* style, const float* emo_vec,
 
 // ============================================================================================
 // Strict fp32 path (idx_gpt_config.weights_bf16 = 0): the reference's default `use_bf16=False`
-// arithmetic (fp32 weights, fp32 activations, fp32 KV cache) as plain per-op kernels, one sequence
-// at a time.  It exists for token-for-token parity against the fp32 oracle (DESIGN.md section 5); the
+// arithmetic (fp32 weights, fp32 activations, fp32 KV cache) as plain per-op kernels, one request
+// at a time (with beam search its beams are the R <= 4 rows of each launch).  It exists for token-for-token parity against the fp32 oracle (DESIGN.md section 5); the
 // fused persistent kernel above is the performance path.  Same call sites, same sampler contract.
 // ============================================================================================
+// Row r = blockIdx.y of an R-row launch: the prompt row (prefill, R = 1) or mel_emb[tok[r]] + mel_pos[posidx].
 __global__ void strict_embed_kernel(float* x, const float* prompt_row, const float* mel_emb, const float* mel_pos,
                                     const int* tok, int posidx, int D) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
   if (c >= D) return;
-  x[c] = prompt_row ? prompt_row[c] : mel_emb[(size_t)tok[0] * D + c] + mel_pos[(size_t)posidx * D + c];
+  x[(size_t)r * D + c] = prompt_row ? prompt_row[c] : mel_emb[(size_t)tok[r] * D + c] + mel_pos[(size_t)posidx * D + c];
 }
 
-// LayerNorm(eps 1e-5) of one row, statistics accumulated in double
+// LayerNorm(eps 1e-5) of row blockIdx.y, statistics accumulated in double
 __global__ void strict_ln_kernel(const float* x, const float* w, const float* b, float* y, int D) {
   __shared__ double sh[64];
   const int tid = threadIdx.x;
+  x += (size_t)blockIdx.y * D;
+  y += (size_t)blockIdx.y * D;
   double s = 0.0;
   for (int i = tid; i < D; i += blockDim.x) s += (double)x[i];
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
@@ -1225,54 +1228,81 @@ __global__ void strict_ln_kernel(const float* x, const float* w, const float* b,
   for (int i = tid; i < D; i += blockDim.x) y[i] = (x[i] - mf) * rstd * w[i] + b[i];
 }
 
-// y[c] = act(sum_k x[k] W[k][c] + bias[c]) (+ res[c]);  W is HF Conv1D [K][N] (trap P4).  Block (32, 32):
-// warp ty owns k = ty, ty + 32, ...; a warp reads one 128-byte row segment per k.
+// y[r][c] = act(sum_k x[r][k] W[k][c] + bias[c]) (+ res[r][c]) for R rows;  W is HF Conv1D [K][N] (trap P4).  Block (32, 32):
+// warp ty owns k = ty, ty + 32, ...; a warp reads one 128-byte row segment per k, once for all R rows.  Every row runs the
+// one-row FMA and summation order, so row r is bitwise what an R = 1 launch computes on that row.
+template <int R>
 __global__ void strict_gemv_kn_kernel(const float* __restrict__ x, const float* __restrict__ W,
                                       const float* __restrict__ bias, const float* res, float* y, int K, int N, int act) {
-  __shared__ float part[32][33];
+  __shared__ float part[R][32][33];
   const int tx = threadIdx.x, ty = threadIdx.y;
   const int c = blockIdx.x * 32 + tx;
-  float acc = 0.f;
+  float acc[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) acc[r] = 0.f;
   if (c < N)
-    for (int k = ty; k < K; k += 32) acc = fmaf(x[k], W[(size_t)k * N + c], acc);
-  part[ty][tx] = acc;
+    for (int k = ty; k < K; k += 32) {
+      const float wk = W[(size_t)k * N + c];
+#pragma unroll
+      for (int r = 0; r < R; ++r) acc[r] = fmaf(x[(size_t)r * K + k], wk, acc[r]);
+    }
+#pragma unroll
+  for (int r = 0; r < R; ++r) part[r][ty][tx] = acc[r];
   __syncthreads();
-  if (ty == 0 && c < N) {
+  if (ty < R && c < N) {          // warp r finishes row r
     float s = 0.f;
 #pragma unroll
-    for (int q = 0; q < 32; ++q) s += part[q][tx];
+    for (int q = 0; q < 32; ++q) s += part[ty][q][tx];
     s += bias[c];
     if (act == 1) s = gelu_new(s, 0);
-    if (res) s += res[c];
-    y[c] = s;
+    if (res) s += res[(size_t)ty * N + c];
+    y[(size_t)ty * N + c] = s;
   }
 }
 
-// nn.Linear [N][K]: one warp per output row
+// nn.Linear [N][K] for R rows: one warp per output row, each weight read once for all R rows
+template <int R>
 __global__ void strict_gemv_nk_kernel(const float* __restrict__ x, const float* __restrict__ W,
                                       const float* __restrict__ bias, float* y, int K, int N) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= N) return;
-  float acc = 0.f;
-  for (int k = lane; k < K; k += 32) acc = fmaf(x[k], W[(size_t)row * K + k], acc);
-  acc = warp_sum(acc);
-  if (lane == 0) y[row] = acc + bias[row];
+  float acc[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) acc[r] = 0.f;
+  for (int k = lane; k < K; k += 32) {
+    const float wk = W[(size_t)row * K + k];
+#pragma unroll
+    for (int r = 0; r < R; ++r) acc[r] = fmaf(x[(size_t)r * K + k], wk, acc[r]);
+  }
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    acc[r] = warp_sum(acc[r]);
+    if (lane == 0) y[(size_t)r * N + row] = acc[r] + bias[row];
+  }
 }
 
-// one head per block: append (k, v) of this position to the fp32 cache, softmax(q k^T / 8) v over positions 0..pos
-__global__ void strict_attn_kernel(const float* qkv, float* kc, float* vc, int pos, float* out, int D) {
+// One (head, row) per block: append (k, v) of this position to the row's fp32 cache slot, softmax(q k^T / 8) v over
+// positions 0..pos.  kc / vc point at slot 0 of the layer; slots are `sstride` floats apart.  Without a map (phys = null,
+// one row) every position is in slot 0.  With one (beam rows, the fused path's convention) prompt positions j < plen live
+// once in slot 0, generated position t of row r lives in slot phys[r * phys_stride + t], and row r writes pos in its own
+// slot r (phys[r][pos - plen] = r).
+__global__ void strict_attn_kernel(const float* qkv, float* kc, float* vc, int pos, float* out, int D,
+                                   const unsigned char* phys, int phys_stride, int plen, size_t sstride) {
   extern __shared__ float sc[];           // [pos + 1] scores, then [128] merge buffer
   __shared__ float redv[8];
-  const int h = blockIdx.x, tid = threadIdx.x;
+  const int h = blockIdx.x, r = blockIdx.y, tid = threadIdx.x;
+  qkv += (size_t)r * 3 * D;
+  const unsigned char* map = phys ? phys + (size_t)r * phys_stride : nullptr;
+  auto slot = [&](int j) -> size_t { return (map && j >= plen) ? (size_t)map[j - plen] * sstride : 0; };
   if (tid < HD) {
-    kc[(size_t)pos * D + h * HD + tid] = qkv[D + h * HD + tid];
-    vc[(size_t)pos * D + h * HD + tid] = qkv[2 * D + h * HD + tid];
+    kc[(size_t)r * sstride + (size_t)pos * D + h * HD + tid] = qkv[D + h * HD + tid];
+    vc[(size_t)r * sstride + (size_t)pos * D + h * HD + tid] = qkv[2 * D + h * HD + tid];
   }
   __syncthreads();
   const float* q = qkv + h * HD;
   float mx = -INFINITY;
   for (int j = tid; j <= pos; j += blockDim.x) {
-    const float* kr = kc + (size_t)j * D + h * HD;
+    const float* kr = kc + slot(j) + (size_t)j * D + h * HD;
     float s = 0.f;
 #pragma unroll 8
     for (int d = 0; d < HD; ++d) s = fmaf(q[d], kr[d], s);
@@ -1295,11 +1325,11 @@ __global__ void strict_attn_kernel(const float* qkv, float* kc, float* vc, int p
   for (int q2 = 0; q2 < (int)(blockDim.x >> 5); ++q2) tot += redv[4 + q2];
   const int d = tid & (HD - 1), half = tid / HD;      // 128 threads: two interleaved halves of the positions
   float acc = 0.f;
-  for (int j = half; j <= pos; j += 2) acc = fmaf(sc[j], vc[(size_t)j * D + h * HD + d], acc);
+  for (int j = half; j <= pos; j += 2) acc = fmaf(sc[j], vc[slot(j) + (size_t)j * D + h * HD + d], acc);
   float* mg = sc + pos + 1;
   mg[tid] = acc;
   __syncthreads();
-  if (tid < HD) out[h * HD + tid] = (mg[tid] + mg[tid + HD]) / tot;
+  if (tid < HD) out[(size_t)r * D + h * HD + tid] = (mg[tid] + mg[tid + HD]) / tot;
 }
 
 // The pick of one sequence (pick_token, one 256-thread block) and its bookkeeping, as in the sampling phase of the fused
@@ -1725,8 +1755,10 @@ struct StrictLayer {
 };
 struct GptStrict {
   std::vector<StrictLayer> layers;
-  float *kc = nullptr, *vc = nullptr;                 // [L][maxpos][D] fp32, one sequence at a time
-  float *x = nullptr, *h = nullptr, *qkv = nullptr, *att = nullptr, *f = nullptr, *logits = nullptr;
+  int nslot = 0;                                      // sequence slots: one per beam row of the request being decoded
+  size_t sstride = 0;                                 // floats per slot: L * maxpos * D
+  float *kc = nullptr, *vc = nullptr;                 // [nslot][L][maxpos][D] fp32
+  float *x = nullptr, *h = nullptr, *qkv = nullptr, *att = nullptr, *f = nullptr, *logits = nullptr;   // [nslot][...]
 };
 
 static void strict_init(idx_engine* e, GptState* g) {
@@ -1749,37 +1781,75 @@ static void strict_init(idx_engine* e, GptState* g) {
   }
   IDX_CHECK(e->W("gpt.mel_head.weight").numel() == (size_t)V * D, IDX_ERR_ARG, "mel_head.weight shape");
   g->maxpos = c.max_prompt + c.max_mel_positions + 8;
-  s->kc = galloc<float>(g, (size_t)L * g->maxpos * D);
-  s->vc = galloc<float>(g, (size_t)L * g->maxpos * D);
-  s->x = galloc<float>(g, D); s->h = galloc<float>(g, D); s->qkv = galloc<float>(g, 3 * (size_t)D);
-  s->att = galloc<float>(g, D); s->f = galloc<float>(g, FF); s->logits = galloc<float>(g, V);
+  s->nslot = std::min(c.max_batch, BEAM_MAX);
+  s->sstride = (size_t)L * g->maxpos * D;
+  const int R = s->nslot;
+  s->kc = galloc<float>(g, R * s->sstride);
+  s->vc = galloc<float>(g, R * s->sstride);
+  s->x = galloc<float>(g, (size_t)R * D); s->h = galloc<float>(g, (size_t)R * D); s->qkv = galloc<float>(g, (size_t)R * 3 * D);
+  s->att = galloc<float>(g, (size_t)R * D); s->f = galloc<float>(g, (size_t)R * FF); s->logits = galloc<float>(g, (size_t)R * V);
   g->tok = galloc<int>(g, 8); g->nout = galloc<int>(g, 8); g->finished = galloc<int>(g, 8);
   g->seen = galloc<unsigned>(g, (size_t)((V + 31) / 32));
   IDX_CUDA(cudaFuncSetAttribute(strict_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   IDX_CHECK((size_t)(g->maxpos + 129) * 4 <= 96 * 1024, IDX_ERR_ARG, "context too long for the strict attention kernel");
 }
 
-// one position through the 24 blocks (x in s->x, updated in place); pos = its index in the KV cache
-static void strict_layers(idx_engine* e, GptState* g, int pos) {
+// R-row launches of the strict GEMVs (R <= BEAM_MAX sequence slots)
+static void strict_gemv_kn(cudaStream_t st, int R, const float* x, const float* W, const float* b, const float* res, float* y,
+                           int K, int N, int act) {
+  const dim3 grid((N + 31) / 32), blk(32, 32);
+  switch (R) {
+    case 1: strict_gemv_kn_kernel<1><<<grid, blk, 0, st>>>(x, W, b, res, y, K, N, act); break;
+    case 2: strict_gemv_kn_kernel<2><<<grid, blk, 0, st>>>(x, W, b, res, y, K, N, act); break;
+    case 3: strict_gemv_kn_kernel<3><<<grid, blk, 0, st>>>(x, W, b, res, y, K, N, act); break;
+    case 4: strict_gemv_kn_kernel<4><<<grid, blk, 0, st>>>(x, W, b, res, y, K, N, act); break;
+    default: throw IdxError(IDX_ERR_ARG, "the strict path runs 1..4 rows");
+  }
+}
+static void strict_gemv_nk(cudaStream_t st, int R, const float* x, const float* W, const float* b, float* y, int K, int N) {
+  const int grid = (N + 7) / 8;
+  switch (R) {
+    case 1: strict_gemv_nk_kernel<1><<<grid, 256, 0, st>>>(x, W, b, y, K, N); break;
+    case 2: strict_gemv_nk_kernel<2><<<grid, 256, 0, st>>>(x, W, b, y, K, N); break;
+    case 3: strict_gemv_nk_kernel<3><<<grid, 256, 0, st>>>(x, W, b, y, K, N); break;
+    case 4: strict_gemv_nk_kernel<4><<<grid, 256, 0, st>>>(x, W, b, y, K, N); break;
+    default: throw IdxError(IDX_ERR_ARG, "the strict path runs 1..4 rows");
+  }
+}
+
+// R rows at position pos through the 24 blocks (rows in s->x, updated in place).  One row (phys = null) uses slot 0; beam
+// rows read their lineage through phys (see strict_attn_kernel), the prompt being the first plen positions of slot 0.
+static void strict_layers(idx_engine* e, GptState* g, int pos, int R = 1, const unsigned char* phys = nullptr,
+                          int phys_stride = 0, int plen = 0) {
   GptStrict* s = g->strict;
   const int D = g->cfg.model_dim, H = g->cfg.heads, FF = 4 * D;
   cudaStream_t st = e->stream;
-  const dim3 blk(32, 32);
   for (int l = 0; l < g->cfg.layers; ++l) {
     const StrictLayer& y = s->layers[l];
     float* kc = s->kc + (size_t)l * g->maxpos * D;
     float* vc = s->vc + (size_t)l * g->maxpos * D;
-    strict_ln_kernel<<<1, 256, 0, st>>>(s->x, y.ln1_w, y.ln1_b, s->h, D);
-    strict_gemv_kn_kernel<<<(3 * D + 31) / 32, blk, 0, st>>>(s->h, y.wqkv, y.bqkv, nullptr, s->qkv, D, 3 * D, 0);
-    strict_attn_kernel<<<H, 128, (size_t)(pos + 1 + 128) * 4, st>>>(s->qkv, kc, vc, pos, s->att, D);
-    strict_gemv_kn_kernel<<<(D + 31) / 32, blk, 0, st>>>(s->att, y.wo, y.bo, s->x, s->x, D, D, 0);
-    strict_ln_kernel<<<1, 256, 0, st>>>(s->x, y.ln2_w, y.ln2_b, s->h, D);
-    strict_gemv_kn_kernel<<<(FF + 31) / 32, blk, 0, st>>>(s->h, y.wfc, y.bfc, nullptr, s->f, D, FF, 1);
-    strict_gemv_kn_kernel<<<(D + 31) / 32, blk, 0, st>>>(s->f, y.wproj, y.bproj, s->x, s->x, FF, D, 0);
+    strict_ln_kernel<<<dim3(1, R), 256, 0, st>>>(s->x, y.ln1_w, y.ln1_b, s->h, D);
+    strict_gemv_kn(st, R, s->h, y.wqkv, y.bqkv, nullptr, s->qkv, D, 3 * D, 0);
+    strict_attn_kernel<<<dim3(H, R), 128, (size_t)(pos + 1 + 128) * 4, st>>>(s->qkv, kc, vc, pos, s->att, D, phys, phys_stride,
+                                                                             plen, s->sstride);
+    strict_gemv_kn(st, R, s->att, y.wo, y.bo, s->x, s->x, D, D, 0);
+    strict_ln_kernel<<<dim3(1, R), 256, 0, st>>>(s->x, y.ln2_w, y.ln2_b, s->h, D);
+    strict_gemv_kn(st, R, s->h, y.wfc, y.bfc, nullptr, s->f, D, FF, 1);
+    strict_gemv_kn(st, R, s->f, y.wproj, y.bproj, s->x, s->x, FF, D, 0);
     e->launches += 7;
     g->last_launches += 7;
   }
   IDX_CUDA(cudaGetLastError());
+}
+
+// ln_f, final_norm and mel_head of R rows: logits [R][V] in s->logits
+static void strict_head(idx_engine* e, GptState* g, int R) {
+  GptStrict* s = g->strict;
+  const int D = g->cfg.model_dim, V = g->cfg.number_mel_codes;
+  cudaStream_t st = e->stream;
+  strict_ln_kernel<<<dim3(1, R), 256, 0, st>>>(s->x, e->Wf("gpt.gpt.ln_f.weight"), e->Wf("gpt.gpt.ln_f.bias"), s->h, D);
+  strict_ln_kernel<<<dim3(1, R), 256, 0, st>>>(s->h, e->Wf("gpt.final_norm.weight"), e->Wf("gpt.final_norm.bias"), s->att, D);   // trap P3
+  strict_gemv_nk(st, R, s->att, e->Wf("gpt.mel_head.weight"), e->Wf("gpt.mel_head.bias"), s->logits, D, V);
 }
 
 static void strict_generate(idx_engine* e, GptState* g, const idx_gpt_request* reqs, int nreq, const idx_sampling* sp) {
@@ -1831,9 +1901,7 @@ static void strict_generate(idx_engine* e, GptState* g, const idx_gpt_request* r
     for (; k < max_new; ++k) {
       strict_embed_kernel<<<(D + 255) / 256, 256, 0, st>>>(s->x, nullptr, mel_emb, mel_pos, g->tok, (k == 0 || sp->mel_pos_mode == 1) ? k : k + 1, D);   // trap P1 / no-cache rule
       strict_layers(e, g, plen + k);
-      strict_ln_kernel<<<1, 256, 0, st>>>(s->x, e->Wf("gpt.gpt.ln_f.weight"), e->Wf("gpt.gpt.ln_f.bias"), s->h, D);
-      strict_ln_kernel<<<1, 256, 0, st>>>(s->h, e->Wf("gpt.final_norm.weight"), e->Wf("gpt.final_norm.bias"), s->att, D);   // trap P3
-      strict_gemv_nk_kernel<<<(V + 7) / 8, 256, 0, st>>>(s->att, e->Wf("gpt.mel_head.weight"), e->Wf("gpt.mel_head.bias"), s->logits, D, V);
+      strict_head(e, g, 1);
       strict_sample_kernel<<<1, NCT, 0, st>>>(s->logits, g->seen, k, sa, d_codes, max_new, g->nout, g->finished, g->tok, d_forced,
                                               d_ldump ? d_ldump + (size_t)k * V : nullptr);
       IDX_CUDA(cudaGetLastError());
@@ -2258,173 +2326,174 @@ static void probe_copy_out(idx_engine* e, GptState* g, const ProbeBufs& pb) {
 }
 
 // ------------------------------------------------------------------ beam-sample host driver --
+// What the last beam-search call chose, per request: (parent, token) and running score of every beam after each step.
 struct BeamTrace {
-  int nutt = 0, m = 0, steps = 0, max_new = 0;
-  std::vector<int> pt;        // [steps][8][2] (parent, token)
-  std::vector<float> sc;      // [steps][8]
-  double final_score[8] = {0};
+  struct Utt {
+    int steps = 0;
+    std::vector<int> pt;        // [steps][m][2] (parent, token)
+    std::vector<float> sc;      // [steps][m]
+    double final_score = 0;
+  };
+  int m = 0;
+  std::vector<Utt> utt;
 };
 
 static void beam_trace_free(GptState* g) { delete g->beam_trace; g->beam_trace = nullptr; }
 
-static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* reqs, int nreq, const idx_sampling* sp,
-                          bool probe_on, bool pprobe_on) {
-  const idx_gpt_config& c = g->cfg;
-  const int D = c.model_dim, V = c.number_mel_codes, max_new = sp->max_new_tokens, m = sp->num_beams;
-  IDX_CHECK(m >= 2 && m <= BEAM_MAX, IDX_ERR_ARG, "num_beams must be 1..4");
-  IDX_CHECK(nreq * m <= 8 && nreq * m <= c.max_batch, IDX_ERR_ARG,
-            "beam search needs num_beams rows per request: nreq * num_beams must be <= max_batch (<= 8)");
-  IDX_CHECK(V <= 40 * 256, IDX_ERR_ARG, "vocabulary too large for the device sampler");
-  cudaStream_t st = e->stream;
-  const int rows = nreq * m, wv = (V + 31) / 32, hs = max_new + 2;
-  bool want_logits = false;
-  for (int i = 0; i < nreq; ++i) want_logits |= reqs[i].logits_out != nullptr;
+static void beam_trace_reset(GptState* g, int m) {
+  if (!g->beam_trace) g->beam_trace = new BeamTrace();
+  g->beam_trace->m = m;
+  g->beam_trace->utt.clear();
+}
 
-  int total_rows = 0;
-  std::vector<int> plen(8, 0), row0(8, 0), plen_rows(8, 0);
-  for (int i = 0; i < nreq; ++i) {
-    IDX_CHECK(reqs[i].prompt_emb && reqs[i].prompt_len >= 1 && reqs[i].prompt_len <= c.max_prompt, IDX_ERR_ARG, "bad prompt");
-    IDX_CHECK(reqs[i].prompt_len + max_new + 1 <= g->maxpos, IDX_ERR_ARG, "KV cache too small");
-    IDX_CHECK(!reqs[i].forced_codes, IDX_ERR_ARG, "forced_codes is not defined for beam search");
-    plen[i] = reqs[i].prompt_len;
-    row0[i] = total_rows;
-    total_rows += plen[i];
-    for (int j = 0; j < m; ++j) plen_rows[i * m + j] = plen[i];
-  }
-  std::vector<PrefillTile> tiles;
-  for (int i = 0; i < nreq; ++i)
-    for (int p0 = 0; p0 < plen[i]; p0 += 8)
-      tiles.push_back({i * m, p0, std::min(8, plen[i] - p0), row0[i] + p0});     // prompt KV lives in the first beam's slot
+// Device state of one beam search over nreq requests of m beam rows each (rows u * m + j of 8-row buffers, the layout
+// beam_step_kernel reads), carved from the engine arena.
+struct BeamBufs {
+  int nreq = 0, m = 0, hs = 0, wv = 0, max_new = 0;
+  unsigned* seen[2] = {nullptr, nullptr};
+  int* hist[2] = {nullptr, nullptr};
+  unsigned char* phys[2] = {nullptr, nullptr};
+  float *bscore = nullptr, *trsc = nullptr, *ldump = nullptr;
+  double *hscore = nullptr, *worst = nullptr;
+  int *hlen = nullptr, *horder = nullptr, *nhyp = nullptr, *done = nullptr, *htok = nullptr, *trpt = nullptr;
+};
 
-  size_t need = (size_t)(total_rows + 8) * D * 4 + tiles.size() * sizeof(PrefillTile) + 2 * 8 * (size_t)wv * 4 +
-                2 * 8 * (size_t)hs * 4 + 2 * 8 * (size_t)hs + (size_t)nreq * (m + 1) * hs * 4 + 8 * (size_t)max_new * 12 + (1 << 16);
+static size_t beam_bufs_bytes(int nreq, int m, int max_new, int V, bool want_logits) {
+  const size_t wv = (V + 31) / 32, hs = max_new + 2;
+  size_t need = 2 * 8 * wv * 4 + 2 * 8 * hs * 4 + 2 * 8 * hs + (size_t)nreq * (m + 1) * hs * 4 + 8 * (size_t)max_new * 12 + (1 << 16);
   if (want_logits) need += (size_t)max_new * 8 * V * 4;
-  e->ensure_arena(need + (1 << 20));
-  e->arena.reset();
-  float* d_prompt = e->arena.get<float>((size_t)(total_rows + 8) * D);
-  PrefillTile* d_tiles = e->arena.get<PrefillTile>(tiles.size());
-  unsigned* d_seen[2] = {e->arena.get<unsigned>(8 * (size_t)wv), e->arena.get<unsigned>(8 * (size_t)wv)};
-  int* d_hist[2] = {e->arena.get<int>(8 * (size_t)hs), e->arena.get<int>(8 * (size_t)hs)};
-  unsigned char* d_phys[2] = {e->arena.get<unsigned char>(8 * (size_t)hs + 16), e->arena.get<unsigned char>(8 * (size_t)hs + 16)};
-  float* d_bscore = e->arena.get<float>(8);
-  double* d_hscore = e->arena.get<double>((size_t)nreq * (m + 1) + 2);
-  double* d_worst = e->arena.get<double>(nreq + 2);
-  int* d_hlen = e->arena.get<int>((size_t)nreq * (m + 1));
-  int* d_horder = e->arena.get<int>((size_t)nreq * (m + 1));
-  int* d_nhyp = e->arena.get<int>(nreq);
-  int* d_done = e->arena.get<int>(nreq);
-  int* d_htok = e->arena.get<int>((size_t)nreq * (m + 1) * hs);
-  int* d_trpt = e->arena.get<int>((size_t)max_new * 16);
-  float* d_trsc = e->arena.get<float>((size_t)max_new * 8);
-  float* d_ldump = want_logits ? e->arena.get<float>((size_t)max_new * 8 * V) : nullptr;
+  return need;
+}
 
-  IDX_CUDA(cudaEventRecord(g->ev0, st));
-  for (int i = 0; i < nreq; ++i)
-    idx_to_device(e, d_prompt + (size_t)row0[i] * D, reqs[i].prompt_emb, (size_t)plen[i] * D * 4);
-  IDX_CUDA(cudaMemcpyAsync(d_tiles, tiles.data(), tiles.size() * sizeof(PrefillTile), cudaMemcpyHostToDevice, st));
-  {
-    std::vector<int> h_tok(8, c.start_mel_token), zeros(16, 0);
-    std::vector<unsigned> h_seen(8 * (size_t)wv, 0u);
-    std::vector<float> h_bs(8, -1e9f);
-    std::vector<unsigned char> h_phys(8 * (size_t)hs + 16, 0);
-    std::vector<double> h_worst(nreq + 2, 1e9);
-    for (int r = 0; r < rows; ++r) {
-      h_seen[(size_t)r * wv + (1 >> 5)] |= 1u << 1;                                      // trap P2
-      h_seen[(size_t)r * wv + (c.start_mel_token >> 5)] |= 1u << (c.start_mel_token & 31);
-      if (r % m == 0) h_bs[r] = 0.f;          // only the first beam carries probability mass at step 0 (:3408-3410)
-      h_phys[(size_t)r * hs] = (unsigned char)r;
-    }
-    IDX_CUDA(cudaMemcpyAsync(g->tok, h_tok.data(), 32, cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemcpyAsync(g->finished, zeros.data(), 32, cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemcpyAsync(g->done, zeros.data(), 4, cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemcpyAsync(g->prompt_len, plen_rows.data(), 32, cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemcpyAsync(d_seen[0], h_seen.data(), h_seen.size() * 4, cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemcpyAsync(d_bscore, h_bs.data(), 32, cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemcpyAsync(d_phys[0], h_phys.data(), h_phys.size(), cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemcpyAsync(d_worst, h_worst.data(), h_worst.size() * 8, cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemsetAsync(d_nhyp, 0, nreq * 4, st));
-    IDX_CUDA(cudaMemsetAsync(d_done, 0, nreq * 4, st));
-    IDX_CUDA(cudaMemsetAsync(d_hlen, 0, (size_t)nreq * (m + 1) * 4, st));
-    IDX_CUDA(cudaStreamSynchronize(st));
+static BeamBufs beam_bufs_get(idx_engine* e, int nreq, int m, int max_new, int V, bool want_logits) {
+  BeamBufs b;
+  b.nreq = nreq; b.m = m; b.max_new = max_new; b.hs = max_new + 2; b.wv = (V + 31) / 32;
+  const size_t wv = b.wv, hs = b.hs;
+  b.seen[0] = e->arena.get<unsigned>(8 * wv); b.seen[1] = e->arena.get<unsigned>(8 * wv);
+  b.hist[0] = e->arena.get<int>(8 * hs); b.hist[1] = e->arena.get<int>(8 * hs);
+  b.phys[0] = e->arena.get<unsigned char>(8 * hs + 16); b.phys[1] = e->arena.get<unsigned char>(8 * hs + 16);
+  b.bscore = e->arena.get<float>(8);
+  b.hscore = e->arena.get<double>((size_t)nreq * (m + 1) + 2);
+  b.worst = e->arena.get<double>(nreq + 2);
+  b.hlen = e->arena.get<int>((size_t)nreq * (m + 1));
+  b.horder = e->arena.get<int>((size_t)nreq * (m + 1));
+  b.nhyp = e->arena.get<int>(nreq);
+  b.done = e->arena.get<int>(nreq);
+  b.htok = e->arena.get<int>((size_t)nreq * (m + 1) * hs);
+  b.trpt = e->arena.get<int>((size_t)max_new * 16);
+  b.trsc = e->arena.get<float>((size_t)max_new * 8);
+  b.ldump = want_logits ? e->arena.get<float>((size_t)max_new * 8 * V) : nullptr;
+  return b;
+}
+
+// step-0 state: start token, the fake prompt ids in the repetition bitmaps, only the first beam of a request carrying
+// probability mass, every row's map naming its own slot, empty hypothesis lists
+static void beam_bufs_init(idx_engine* e, GptState* g, const BeamBufs& b) {
+  const idx_gpt_config& c = g->cfg;
+  cudaStream_t st = e->stream;
+  const int rows = b.nreq * b.m, wv = b.wv, hs = b.hs;
+  std::vector<int> h_tok(8, c.start_mel_token);
+  std::vector<unsigned> h_seen(8 * (size_t)wv, 0u);
+  std::vector<float> h_bs(8, -1e9f);
+  std::vector<unsigned char> h_phys(8 * (size_t)hs + 16, 0);
+  std::vector<double> h_worst(b.nreq + 2, 1e9);
+  for (int r = 0; r < rows; ++r) {
+    h_seen[(size_t)r * wv + (1 >> 5)] |= 1u << 1;                                      // trap P2
+    h_seen[(size_t)r * wv + (c.start_mel_token >> 5)] |= 1u << (c.start_mel_token & 31);
+    if (r % b.m == 0) h_bs[r] = 0.f;          // only the first beam carries probability mass at step 0 (:3408-3410)
+    h_phys[(size_t)r * hs] = (unsigned char)r;
   }
+  IDX_CUDA(cudaMemcpyAsync(g->tok, h_tok.data(), 32, cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaMemcpyAsync(b.seen[0], h_seen.data(), h_seen.size() * 4, cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaMemcpyAsync(b.bscore, h_bs.data(), 32, cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaMemcpyAsync(b.phys[0], h_phys.data(), h_phys.size(), cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaMemcpyAsync(b.worst, h_worst.data(), h_worst.size() * 8, cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaMemsetAsync(b.nhyp, 0, b.nreq * 4, st));
+  IDX_CUDA(cudaMemsetAsync(b.done, 0, b.nreq * 4, st));
+  IDX_CUDA(cudaMemsetAsync(b.hlen, 0, (size_t)b.nreq * (b.m + 1) * 4, st));
+  IDX_CUDA(cudaStreamSynchronize(st));   // host vectors go out of scope
+}
 
-  GptParams p;
-  ProbeBufs pb;
-  fill_common(e, g, p);
-  p.B = 8; p.mode = 0; p.nsteps = (int)tiles.size(); p.prompt = d_prompt; p.tiles = d_tiles;
-  p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
-  p.beams = m;                                   // the prefill probe's request index is the tile's slot / m
-  if (pprobe_on) probe_arm_prefill(e, g, p, pb);
-  launch_fused(e, g, p);
-  IDX_CUDA(cudaEventRecord(g->ev1, st));
-
-  fill_common(e, g, p);
-  p.B = rows; p.mode = 1; p.max_new = max_new; p.ext_sample = 1; p.beams = m; p.phys_stride = hs;
-  p.pos_plain = sp->mel_pos_mode == 1;
-  if (probe_on) probe_arm_decode(e, g, p, pb, max_new);
+static BeamParams beam_params(idx_engine* e, GptState* g, const BeamBufs& b, const idx_sampling* sp, const float* logits,
+                              int utt_base) {
+  const idx_gpt_config& c = g->cfg;
   BeamParams bp;
   memset(&bp, 0, sizeof(bp));
-  bp.logits = g->logits; bp.V = V; bp.m = m; bp.max_new = max_new; bp.stop_tok = c.stop_mel_token;
-  bp.forbid_stop_before = sp->forbid_stop_before; bp.hist_stride = hs;
+  bp.logits = logits; bp.V = c.number_mel_codes; bp.m = b.m; bp.max_new = b.max_new; bp.stop_tok = c.stop_mel_token;
+  bp.forbid_stop_before = sp->forbid_stop_before; bp.hist_stride = b.hs;
   bp.rep_penalty = sp->repetition_penalty;
   bp.do_sample = sp->do_sample;
   bp.top_k = sp->do_sample ? sp->top_k : 0;
   bp.top_p = sp->do_sample ? sp->top_p : 1.0f;
   bp.inv_temp = (sp->do_sample && sp->temperature > 0.f) ? 1.0f / sp->temperature : 1.0f;
-  bp.length_penalty = sp->length_penalty; bp.seed = sp->seed; bp.utt_base = g->seq_base;
-  bp.beam_scores = d_bscore; bp.tok = g->tok;
-  bp.hyp_score = d_hscore; bp.hyp_len = d_hlen; bp.hyp_tok = d_htok; bp.hyp_order = d_horder; bp.nhyp = d_nhyp;
-  bp.worst = d_worst; bp.done_u = d_done; bp.ldump = d_ldump; bp.trace_pt = d_trpt; bp.trace_sc = d_trsc;
+  bp.length_penalty = sp->length_penalty; bp.seed = sp->seed; bp.utt_base = utt_base;
+  bp.beam_scores = b.bscore; bp.tok = g->tok;
+  bp.hyp_score = b.hscore; bp.hyp_len = b.hlen; bp.hyp_tok = b.htok; bp.hyp_order = b.horder; bp.nhyp = b.nhyp;
+  bp.worst = b.worst; bp.done_u = b.done; bp.ldump = b.ldump; bp.trace_pt = b.trpt; bp.trace_sc = b.trsc;
   bp.flag = e->dev_flag;
-  int* h_done = (int*)e->pinned_buf(64);
-  int steps = 0;
-  for (int k = 0; k < max_new; ++k) {
-    const int cur = k & 1, nxt = cur ^ 1;
-    p.step0 = k; p.nsteps = 1; p.phys = d_phys[cur];
-    launch_fused(e, g, p);
-    bp.k = k;
-    bp.seen_cur = d_seen[cur]; bp.seen_nxt = d_seen[nxt];
-    bp.hist_cur = d_hist[cur]; bp.hist_nxt = d_hist[nxt];
-    bp.phys_cur = d_phys[cur]; bp.phys_nxt = d_phys[nxt];
-    beam_step_kernel<<<nreq, 256, 0, st>>>(bp);
-    IDX_CUDA(cudaGetLastError());
-    e->launches++;
-    g->last_launches++;
-    steps = k + 1;
-    if ((k & 7) == 7 || k + 1 == max_new) {
-      IDX_CUDA(cudaMemcpyAsync(h_done, d_done, nreq * 4, cudaMemcpyDeviceToHost, st));
-      IDX_CUDA(cudaStreamSynchronize(st));
-      bool all = true;
-      for (int i = 0; i < nreq; ++i) all &= h_done[i] != 0;
-      if (all) break;
-    }
-  }
-  IDX_CUDA(cudaEventRecord(g->ev2, st));
-  e->check_flag(kTieOverflow);
+  return bp;
+}
 
-  // ---- BeamSearchScorer.finalize (transformers_beam_search.py:322-420) on the host ----
+// The beam step of step k (its logits written by the forward pass); true when every request is done.  The host polls the
+// done flags every 8 steps, so up to 7 pad steps may run after the scorer finished.
+static bool beam_step(idx_engine* e, GptState* g, BeamParams& bp, const BeamBufs& b, int k) {
+  cudaStream_t st = e->stream;
+  const int cur = k & 1, nxt = cur ^ 1;
+  bp.k = k;
+  bp.seen_cur = b.seen[cur]; bp.seen_nxt = b.seen[nxt];
+  bp.hist_cur = b.hist[cur]; bp.hist_nxt = b.hist[nxt];
+  bp.phys_cur = b.phys[cur]; bp.phys_nxt = b.phys[nxt];
+  beam_step_kernel<<<b.nreq, 256, 0, st>>>(bp);
+  IDX_CUDA(cudaGetLastError());
+  e->launches++;
+  g->last_launches++;
+  if ((k & 7) != 7 && k + 1 != b.max_new) return false;
+  int* h_done = (int*)e->pinned_buf(64);
+  IDX_CUDA(cudaMemcpyAsync(h_done, b.done, b.nreq * 4, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaStreamSynchronize(st));
+  bool all = true;
+  for (int i = 0; i < b.nreq; ++i) all &= h_done[i] != 0;
+  return all;
+}
+
+// BeamSearchScorer.finalize (transformers_beam_search.py:322-420) on the host after `steps` beam steps: each request's best
+// hypothesis to codes_out / n_codes_out, its beams' logits to logits_out [steps][m][V], and its trace appended to
+// g->beam_trace.
+static void beam_finish(idx_engine* e, GptState* g, const idx_gpt_request* reqs, const idx_sampling* sp, const BeamBufs& b,
+                       int steps) {
+  const idx_gpt_config& c = g->cfg;
+  cudaStream_t st = e->stream;
+  const int nreq = b.nreq, m = b.m, hs = b.hs, max_new = b.max_new, V = c.number_mel_codes;
   const int fin = steps & 1;      // buffers written by the last beam step
   std::vector<int> h_hist(8 * (size_t)hs), h_hlen((size_t)nreq * (m + 1)), h_horder((size_t)nreq * (m + 1)), h_nhyp(nreq), h_dn(nreq);
   std::vector<int> h_htok((size_t)nreq * (m + 1) * hs);
   std::vector<double> h_hscore((size_t)nreq * (m + 1) + 2);
   std::vector<float> h_bs(8);
-  BeamTrace* tr = g->beam_trace ? g->beam_trace : (g->beam_trace = new BeamTrace());
-  tr->nutt = nreq; tr->m = m; tr->steps = steps; tr->max_new = max_new;
-  tr->pt.assign((size_t)steps * 16, 0); tr->sc.assign((size_t)steps * 8, 0.f);
-  IDX_CUDA(cudaMemcpyAsync(h_hist.data(), d_hist[fin], h_hist.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_hlen.data(), d_hlen, h_hlen.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_horder.data(), d_horder, h_horder.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_nhyp.data(), d_nhyp, nreq * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_dn.data(), d_done, nreq * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_htok.data(), d_htok, h_htok.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_hscore.data(), d_hscore, (size_t)nreq * (m + 1) * 8, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_bs.data(), d_bscore, 32, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(tr->pt.data(), d_trpt, tr->pt.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(tr->sc.data(), d_trsc, tr->sc.size() * 4, cudaMemcpyDeviceToHost, st));
-  probe_copy_out(e, g, pb);
+  std::vector<int> h_pt((size_t)steps * 16);
+  std::vector<float> h_sc((size_t)steps * 8);
+  IDX_CUDA(cudaMemcpyAsync(h_hist.data(), b.hist[fin], h_hist.size() * 4, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_hlen.data(), b.hlen, h_hlen.size() * 4, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_horder.data(), b.horder, h_horder.size() * 4, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_nhyp.data(), b.nhyp, nreq * 4, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_dn.data(), b.done, nreq * 4, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_htok.data(), b.htok, h_htok.size() * 4, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_hscore.data(), b.hscore, (size_t)nreq * (m + 1) * 8, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_bs.data(), b.bscore, 32, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_pt.data(), b.trpt, h_pt.size() * 4, cudaMemcpyDeviceToHost, st));
+  IDX_CUDA(cudaMemcpyAsync(h_sc.data(), b.trsc, h_sc.size() * 4, cudaMemcpyDeviceToHost, st));
   IDX_CUDA(cudaStreamSynchronize(st));
-  int maxn = 0;
   for (int u = 0; u < nreq; ++u) {
+    BeamTrace::Utt tu;
+    tu.steps = steps;
+    tu.pt.resize((size_t)steps * m * 2);
+    tu.sc.resize((size_t)steps * m);
+    for (int k = 0; k < steps; ++k)
+      for (int j = 0; j < m; ++j) {
+        const size_t r = (size_t)k * 8 + u * m + j;
+        tu.pt[((size_t)k * m + j) * 2] = h_pt[r * 2];
+        tu.pt[((size_t)k * m + j) * 2 + 1] = h_pt[r * 2 + 1];
+        tu.sc[(size_t)k * m + j] = h_sc[r];
+      }
     struct Hyp { double score; const int* tok; int len; };
     std::vector<Hyp> list;
     for (int q = 0; q < h_nhyp[u]; ++q) {
@@ -2455,28 +2524,164 @@ static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* req
     for (size_t q = 1; q < list.size(); ++q) if (list[q].score >= list[best].score) best = q;
     std::vector<int> codes(list[best].tok, list[best].tok + list[best].len);
     if ((int)codes.size() < max_new) codes.push_back(c.stop_mel_token);
-    tr->final_score[u] = list[best].score;
-    maxn = std::max(maxn, (int)codes.size());
+    tu.final_score = list[best].score;
+    g->beam_trace->utt.push_back(std::move(tu));
     if (reqs[u].n_codes_out) *reqs[u].n_codes_out = (int)codes.size();
     if (reqs[u].codes_out) {
-      IDX_CUDA(cudaMemcpyAsync(d_trpt, codes.data(), codes.size() * 4, cudaMemcpyHostToDevice, st));
+      IDX_CUDA(cudaMemcpyAsync(b.trpt, codes.data(), codes.size() * 4, cudaMemcpyHostToDevice, st));
       IDX_CUDA(cudaStreamSynchronize(st));
-      idx_from_device(e, reqs[u].codes_out, d_trpt, codes.size() * 4);
+      idx_from_device(e, reqs[u].codes_out, b.trpt, codes.size() * 4);
       IDX_CUDA(cudaStreamSynchronize(st));
     }
     if (reqs[u].logits_out) {
-      // [steps][m][V]: the raw logits every beam of this utterance saw at each step
+      // [steps][m][V]: the raw logits every beam of this request saw at each step
       for (int k = 0; k < steps; ++k)
-        idx_from_device(e, reqs[u].logits_out + ((size_t)k * m) * V, d_ldump + ((size_t)k * 8 + u * m) * V, (size_t)m * V * 4);
+        idx_from_device(e, reqs[u].logits_out + ((size_t)k * m) * V, b.ldump + ((size_t)k * 8 + u * m) * V, (size_t)m * V * 4);
     }
   }
   IDX_CUDA(cudaStreamSynchronize(st));
+}
+
+static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* reqs, int nreq, const idx_sampling* sp,
+                          bool probe_on, bool pprobe_on) {
+  const idx_gpt_config& c = g->cfg;
+  const int D = c.model_dim, V = c.number_mel_codes, max_new = sp->max_new_tokens, m = sp->num_beams;
+  IDX_CHECK(m >= 2 && m <= BEAM_MAX, IDX_ERR_ARG, "num_beams must be 1..4");
+  IDX_CHECK(nreq * m <= 8 && nreq * m <= c.max_batch, IDX_ERR_ARG,
+            "beam search needs num_beams rows per request: nreq * num_beams must be <= max_batch (<= 8)");
+  IDX_CHECK(V <= 40 * 256, IDX_ERR_ARG, "vocabulary too large for the device sampler");
+  cudaStream_t st = e->stream;
+  const int rows = nreq * m, hs = max_new + 2;
+  bool want_logits = false;
+  for (int i = 0; i < nreq; ++i) want_logits |= reqs[i].logits_out != nullptr;
+
+  int total_rows = 0;
+  std::vector<int> plen(8, 0), row0(8, 0), plen_rows(8, 0);
+  for (int i = 0; i < nreq; ++i) {
+    IDX_CHECK(reqs[i].prompt_emb && reqs[i].prompt_len >= 1 && reqs[i].prompt_len <= c.max_prompt, IDX_ERR_ARG, "bad prompt");
+    IDX_CHECK(reqs[i].prompt_len + max_new + 1 <= g->maxpos, IDX_ERR_ARG, "KV cache too small");
+    IDX_CHECK(!reqs[i].forced_codes, IDX_ERR_ARG, "forced_codes is not defined for beam search");
+    plen[i] = reqs[i].prompt_len;
+    row0[i] = total_rows;
+    total_rows += plen[i];
+    for (int j = 0; j < m; ++j) plen_rows[i * m + j] = plen[i];
+  }
+  std::vector<PrefillTile> tiles;
+  for (int i = 0; i < nreq; ++i)
+    for (int p0 = 0; p0 < plen[i]; p0 += 8)
+      tiles.push_back({i * m, p0, std::min(8, plen[i] - p0), row0[i] + p0});     // prompt KV lives in the first beam's slot
+
+  const size_t need = (size_t)(total_rows + 8) * D * 4 + tiles.size() * sizeof(PrefillTile) +
+                      beam_bufs_bytes(nreq, m, max_new, V, want_logits);
+  e->ensure_arena(need + (1 << 20));
+  e->arena.reset();
+  float* d_prompt = e->arena.get<float>((size_t)(total_rows + 8) * D);
+  PrefillTile* d_tiles = e->arena.get<PrefillTile>(tiles.size());
+  const BeamBufs b = beam_bufs_get(e, nreq, m, max_new, V, want_logits);
+
+  IDX_CUDA(cudaEventRecord(g->ev0, st));
+  for (int i = 0; i < nreq; ++i)
+    idx_to_device(e, d_prompt + (size_t)row0[i] * D, reqs[i].prompt_emb, (size_t)plen[i] * D * 4);
+  IDX_CUDA(cudaMemcpyAsync(d_tiles, tiles.data(), tiles.size() * sizeof(PrefillTile), cudaMemcpyHostToDevice, st));
+  {
+    std::vector<int> zeros(16, 0);
+    IDX_CUDA(cudaMemcpyAsync(g->finished, zeros.data(), 32, cudaMemcpyHostToDevice, st));
+    IDX_CUDA(cudaMemcpyAsync(g->done, zeros.data(), 4, cudaMemcpyHostToDevice, st));
+    IDX_CUDA(cudaMemcpyAsync(g->prompt_len, plen_rows.data(), 32, cudaMemcpyHostToDevice, st));
+    beam_bufs_init(e, g, b);
+  }
+
+  GptParams p;
+  ProbeBufs pb;
+  fill_common(e, g, p);
+  p.B = 8; p.mode = 0; p.nsteps = (int)tiles.size(); p.prompt = d_prompt; p.tiles = d_tiles;
+  p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
+  p.beams = m;                                   // the prefill probe's request index is the tile's slot / m
+  if (pprobe_on) probe_arm_prefill(e, g, p, pb);
+  launch_fused(e, g, p);
+  IDX_CUDA(cudaEventRecord(g->ev1, st));
+
+  fill_common(e, g, p);
+  p.B = rows; p.mode = 1; p.max_new = max_new; p.ext_sample = 1; p.beams = m; p.phys_stride = hs;
+  p.pos_plain = sp->mel_pos_mode == 1;
+  if (probe_on) probe_arm_decode(e, g, p, pb, max_new);
+  BeamParams bp = beam_params(e, g, b, sp, g->logits, g->seq_base);
+  int steps = 0;
+  for (int k = 0; k < max_new; ++k) {
+    p.step0 = k; p.nsteps = 1; p.phys = b.phys[k & 1];
+    launch_fused(e, g, p);
+    steps = k + 1;
+    if (beam_step(e, g, bp, b, k)) break;
+  }
+  IDX_CUDA(cudaEventRecord(g->ev2, st));
+  e->check_flag(kTieOverflow);
+  probe_copy_out(e, g, pb);
+  beam_trace_reset(g, m);
+  beam_finish(e, g, reqs, sp, b, steps);
   float ms01 = 0, ms12 = 0;
   IDX_CUDA(cudaEventElapsedTime(&ms01, g->ev0, g->ev1));
   IDX_CUDA(cudaEventElapsedTime(&ms12, g->ev1, g->ev2));
   g->t_prefill_ms = ms01;
   g->t_decode_ms = ms12;
   g->last_steps = steps;
+}
+
+// Beam search on the strict fp32 path: one request at a time, its num_beams rows through the R-row strict kernels.  The
+// prompt is prefilled once into slot 0; beam row r appends to slot r and reads its lineage through the phys map that
+// beam_step_kernel maintains.  The Philox stream of request i is that of global request seq_base + i.
+static void strict_beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* reqs, int nreq, const idx_sampling* sp) {
+  GptStrict* s = g->strict;
+  const idx_gpt_config& c = g->cfg;
+  const int D = c.model_dim, V = c.number_mel_codes, max_new = sp->max_new_tokens, m = sp->num_beams;
+  cudaStream_t st = e->stream;
+  for (int i = 0; i < nreq; ++i) {
+    IDX_CHECK(reqs[i].prompt_emb && reqs[i].prompt_len >= 1 && reqs[i].prompt_len <= c.max_prompt, IDX_ERR_ARG, "bad prompt");
+    IDX_CHECK(reqs[i].prompt_len + max_new + 1 <= g->maxpos, IDX_ERR_ARG, "KV cache too small");
+  }
+  const float* mel_emb = e->Wf("gpt.mel_embedding.weight");
+  const float* mel_pos = e->Wf("gpt.mel_pos_embedding.emb.weight");
+  beam_trace_reset(g, m);
+  double tp = 0, td = 0;
+  int max_steps = 0;
+  for (int i = 0; i < nreq; ++i) {
+    const int plen = reqs[i].prompt_len;
+    e->ensure_arena((size_t)plen * D * 4 + beam_bufs_bytes(1, m, max_new, V, reqs[i].logits_out != nullptr) + (1 << 20));
+    e->arena.reset();
+    float* d_prompt = e->arena.get<float>((size_t)plen * D);
+    const BeamBufs b = beam_bufs_get(e, 1, m, max_new, V, reqs[i].logits_out != nullptr);
+    IDX_CUDA(cudaEventRecord(g->ev0, st));
+    idx_to_device(e, d_prompt, reqs[i].prompt_emb, (size_t)plen * D * 4);
+    beam_bufs_init(e, g, b);
+    for (int pos = 0; pos < plen; ++pos) {                                   // prompt positions, one at a time, slot 0
+      strict_embed_kernel<<<(D + 255) / 256, 256, 0, st>>>(s->x, d_prompt + (size_t)pos * D, nullptr, nullptr, nullptr, 0, D);
+      strict_layers(e, g, pos);
+    }
+    IDX_CUDA(cudaEventRecord(g->ev1, st));
+    BeamParams bp = beam_params(e, g, b, sp, s->logits, g->seq_base + i);
+    int steps = 0;
+    for (int k = 0; k < max_new; ++k) {
+      strict_embed_kernel<<<dim3((D + 255) / 256, m), 256, 0, st>>>(s->x, nullptr, mel_emb, mel_pos, g->tok,
+                                                                    (k == 0 || sp->mel_pos_mode == 1) ? k : k + 1, D);
+      strict_layers(e, g, plen + k, m, b.phys[k & 1], b.hs, plen);
+      strict_head(e, g, m);
+      e->launches += 4;
+      g->last_launches += 4;
+      steps = k + 1;
+      if (beam_step(e, g, bp, b, k)) break;
+    }
+    IDX_CUDA(cudaEventRecord(g->ev2, st));
+    e->check_flag(kTieOverflow);
+    beam_finish(e, g, reqs + i, sp, b, steps);
+    max_steps = std::max(max_steps, steps);
+    float ms01 = 0, ms12 = 0;
+    IDX_CUDA(cudaEventElapsedTime(&ms01, g->ev0, g->ev1));
+    IDX_CUDA(cudaEventElapsedTime(&ms12, g->ev1, g->ev2));
+    tp += ms01;
+    td += ms12;
+  }
+  g->t_prefill_ms = tp;
+  g->t_decode_ms = td;
+  g->last_steps = max_steps;      // beam steps run, as on the fused path: the rows of each request's logits dump
 }
 
 extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int nreq,
@@ -2542,10 +2747,16 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
             "max_new_tokens must satisfy k+1 <= mel_pos rows - 1 (SURVEY A.3)");
   IDX_CUDA(cudaSetDevice(e->device));
   const int D = c.model_dim, V = c.number_mel_codes, max_new = sp->max_new_tokens;
+  if (g->strict && sp->num_beams > 1) {
+    // one sequence slot per beam row (strict_init allocates min(max_batch, 4))
+    IDX_CHECK(sp->num_beams <= BEAM_MAX && sp->num_beams <= c.max_batch, IDX_ERR_ARG,
+              "strict fp32 beam search needs num_beams <= max_batch (<= 4): one sequence slot per beam");
+    for (int i = 0; i < nreq; ++i) IDX_CHECK(!reqs[i].forced_codes, IDX_ERR_ARG, "forced_codes is not defined for beam search");
+  }
   g->last_launches = 0;
   if (g->strict) {
-    IDX_CHECK(sp->num_beams == 1, IDX_ERR_ARG, "the strict fp32 path decodes one sequence at a time (num_beams = 1)");
-    strict_generate(e, g, reqs, nreq, sp);
+    if (sp->num_beams > 1) strict_beam_generate(e, g, reqs, nreq, sp);
+    else strict_generate(e, g, reqs, nreq, sp);
     return IDX_OK;
   }
   if (sp->num_beams > 1) {
@@ -2790,19 +3001,13 @@ extern "C" int idx_gpt_beam_trace(const idx_engine* e, int utterance, int32_t* p
                                   int max_steps, int32_t* steps_out, double* final_score) {
   if (!e || !e->gpt || !e->gpt->beam_trace) return IDX_ERR_STATE;
   const BeamTrace* t = e->gpt->beam_trace;
-  if (utterance < 0 || utterance >= t->nutt) return IDX_ERR_ARG;
-  const int n = std::min(max_steps, t->steps), m = t->m;
-  for (int k = 0; k < n; ++k)
-    for (int j = 0; j < m; ++j) {
-      const int r = utterance * m + j;
-      if (parents_tokens) {
-        parents_tokens[((size_t)k * m + j) * 2] = t->pt[((size_t)k * 8 + r) * 2];
-        parents_tokens[((size_t)k * m + j) * 2 + 1] = t->pt[((size_t)k * 8 + r) * 2 + 1];
-      }
-      if (scores) scores[(size_t)k * m + j] = t->sc[(size_t)k * 8 + r];
-    }
-  if (steps_out) *steps_out = t->steps;
-  if (final_score) *final_score = t->final_score[utterance];
+  if (utterance < 0 || utterance >= (int)t->utt.size()) return IDX_ERR_ARG;
+  const BeamTrace::Utt& tu = t->utt[utterance];
+  const int n = std::min(max_steps, tu.steps), m = t->m;
+  if (parents_tokens) std::copy(tu.pt.begin(), tu.pt.begin() + (size_t)n * m * 2, parents_tokens);
+  if (scores) std::copy(tu.sc.begin(), tu.sc.begin() + (size_t)n * m, scores);
+  if (steps_out) *steps_out = tu.steps;
+  if (final_score) *final_score = tu.final_score;
   return IDX_OK;
 }
 

@@ -261,7 +261,7 @@ def attach_v1(tts, engine: Engine = None, device: int = 0):
     engine.gpt_init(len(gpt.gpt.h), D, gpt.heads, gpt.number_mel_codes, gpt.start_mel_token, gpt.stop_mel_token,
                     sd["mel_pos_embedding.emb.weight"].shape[0],
                     max_prompt=sd["text_pos_embedding.emb.weight"].shape[0] + sd["perceiver_encoder.latents"].shape[0] + 8,
-                    max_batch=1, weights_bf16=False)
+                    max_batch=4, weights_bf16=False)      # room for the default 3 beams
     E, Q = "conditioning_encoder.", "perceiver_encoder."
     od = sd[E + "embed.out.0.weight"].shape[0]
     fsub = sd[E + "embed.out.0.weight"].shape[1] // od
