@@ -164,6 +164,39 @@ typedef struct {
 int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int nreq,
                      const idx_sampling* sp);
 
+/* Resumable decode of ONE request: the codes come back a few at a time while the decode carries on, so a caller can
+ * vocode the first ones (idx_stream_vocode) before the last ones exist.  Over a whole stream codes_out ends up bitwise
+ * equal to the codes_out of idx_gpt_generate with the same request, idx_sampling (seed included) and sequence index: the
+ * stream runs the same steps, only split into launches at other boundaries.
+ *   begin  checks the request and sampling as idx_gpt_generate does and runs the prefill.  Refused (IDX_ERR_ARG): the
+ *          strict fp32 path (weights_bf16 = 0) and forced_codes.  prompt_emb is read during the call only; codes_out,
+ *          n_codes_out and logits_out of req are not used.
+ *   next   decodes until at least `until` codes are COMMITTED (codes that can no longer change), the sequence has
+ *          finished or max_new_tokens codes exist, and writes the newly committed codes to
+ *          codes_out[old *n_committed, new *n_committed) (host or device, [max_new_tokens]).  *finished = 1 once every
+ *          code is committed; the last one is the stop token when it was produced.  until < 1 -> IDX_ERR_ARG.
+ *          num_beams = 1: every decoded code is committed; the launches end exactly at `until` steps.
+ *          num_beams = 2..4: every 8 steps the committed prefix grows to the longest common prefix of the live beams'
+ *          histories and the stored finished hypotheses (the only candidates the result can still come from); at the end
+ *          it is the hypothesis BeamSearchScorer.finalize picks, stop token included.  It trails the decode by the steps
+ *          over which the beams still disagree.
+ *   end    closes the stream (idx_destroy closes it as well).
+ * The stream's state lives in device memory it allocates at begin and frees at end, not in the engine's work arena:
+ * codec, length regulator, CFM, BigVGAN and idx_codes_to_wav* / idx_stream_vocode calls may run between two next
+ * calls.  While a stream is open, idx_gpt_init, idx_gpt_generate, idx_gpt_latents_v1 and the GPT probes
+ * (idx_gpt_probe_attention / _prefill, idx_gpt_debug_kv) return IDX_ERR_STATE; next / end without an open stream and a
+ * second begin return IDX_ERR_STATE.                                                                              */
+int idx_gpt_stream_begin(idx_engine* e, const idx_gpt_request* req, const idx_sampling* sp);
+int idx_gpt_stream_next(idx_engine* e, int32_t until, int32_t* codes_out, int32_t* n_committed, int32_t* finished);
+int idx_gpt_stream_end(idx_engine* e);
+/* Diagnostic (tests): the beam buffers of an open beam stream as its last poll left them (host or device memory):
+ * hist [num_beams][max_new_tokens + 2] the live beams' histories (the first *steps entries of a row are valid),
+ * hyp_tok [num_beams + 1][max_new_tokens + 2] and hyp_len [num_beams + 1] the stored finished hypotheses (physical
+ * slots), hyp_order [num_beams + 1] the slots in list order, nhyp_done [2] = (hypotheses stored, request done) and
+ * *steps the beam steps run.  Any of them may be NULL.  IDX_ERR_STATE without an open beam stream.                */
+int idx_gpt_stream_beam_state(idx_engine* e, int32_t* hist, int32_t* hyp_tok, int32_t* hyp_len, int32_t* hyp_order,
+                              int32_t* nhyp_done, int32_t* steps);
+
 /* Build the [cond(3)][start_text, text.., stop_text] prompt embeddings of
  * prepare_gpt_inputs (gpt/model_v2.py:648-714,754-768) on the device.
  *   style      [192] f32   campplus embedding (infer_v2_5.py:644-649)
@@ -541,6 +574,27 @@ int idx_codes_to_wav(idx_engine* e, const idx_vocode_request* r, int n_steps, fl
  * idx_s2mel_last_ms reports the solves as the CFM time and the codec and length regulator times summed over the
  * requests; idx_bigvgan_last_ms the summed BigVGAN time.                                                             */
 int idx_codes_to_wav_batch(idx_engine* e, const idx_vocode_request* reqs, int n, int n_steps, float cfg_rate);
+
+/* One window of a chunked stream (the join of the reference's TensorRT StreamingDecoder.generate, on the device).  The
+ * window r runs through the tail of idx_codes_to_wav (its fp32 waveform, and any output r asks for, bitwise equal to
+ * that call's); then one kernel joins it onto the last overlap_samples (ovlp) of the previous window, which the engine
+ * keeps in memory of its own between the calls, and writes int16 as pcm16_out does (clamp(32767 x), truncated):
+ *   - no kept tail (the first window, IDX_STREAM_FIRST drops any kept tail): emit wav[0, len - ovlp), keep the last ovlp;
+ *   - a kept tail of n0 samples: the first n = min(n0, len(head)) samples are tail[i] * fade_out[i] + head[i] * fade_in[i]
+ *     with head = wav[0, min(ovlp, len)) and fade_in | fade_out = the two halves of np.hanning(2n); then
+ *     wav[ovlp, len - ovlp) follows and the last ovlp samples are kept;
+ *   - IDX_STREAM_LAST: nothing is kept and everything after the blend (wav[ovlp, len), or all of wav without a kept tail)
+ *     is emitted, the last 512 samples scaled by np.linspace(1, 0, 512) when more than 512 are emitted.  A last window
+ *     shorter than ovlp emits only its blend of n samples (the reference drops the rest of the tail too);
+ *   - r == NULL with IDX_STREAM_LAST (flush): emit the kept tail, faded out as above, and keep nothing.
+ * len = F * 256.  *n_pcm: on input the capacity of pcm_out in samples, which must be at least F * 256 plus the kept tail
+ * (the kept tail is at most the previous window's overlap_samples; the flush counts F = 0); on return the samples
+ * written.  pcm_out: host or device memory.  Errors (IDX_ERR_ARG, nothing is emitted and the kept tail stays as it was):
+ * overlap_samples < 0, a window that is not the last with len < 2 * ovlp, a smaller capacity, r == NULL without
+ * IDX_STREAM_LAST, and whatever idx_codes_to_wav refuses.                                                        */
+enum { IDX_STREAM_FIRST = 1, IDX_STREAM_LAST = 2 };
+int idx_stream_vocode(idx_engine* e, const idx_vocode_request* r, int n_steps, float cfg_rate, int32_t overlap_samples,
+                      int32_t flags, int16_t* pcm_out, int32_t* n_pcm);
 
 /* Device ms of the last codec decode / length regulator / CFM solve (CUDA events).       */
 int idx_s2mel_last_ms(const idx_engine* e, double* ms3);

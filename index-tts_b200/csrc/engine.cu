@@ -133,6 +133,7 @@ void idx_destroy(idx_engine* e) {
   if (e->v1cond) emo_destroy(e->v1cond);
   if (e->semantic) semantic_destroy(e->semantic);
   if (e->v1voc) v1voc_destroy(e->v1voc);
+  if (e->sjoin) stream_join_destroy(e->sjoin);
   for (auto& kv : e->weights) cudaFree(kv.second.d);
   for (auto ev : e->events) if (ev) cudaEventDestroy(ev);
   if (e->order_ev) cudaEventDestroy(e->order_ev);

@@ -56,6 +56,7 @@ struct V1VocoderState; // bigvgan.cu (latent-conditioned BigVGAN + ECAPA-TDNN, r
 struct BigvganState;  // bigvgan.cu
 struct S2melState;    // s2mel.cu
 struct SemanticState; // semantic.cu
+struct StreamJoin;    // pipeline.cu (idx_stream_vocode)
 
 // Bump allocator for per-call activations: reset at the start of each forward call.
 struct Arena {
@@ -101,6 +102,7 @@ struct idx_engine {
   EmoState* v1cond = nullptr;   // v1 prompt encoder (32-latent conformer-perceiver)
   V1VocoderState* v1voc = nullptr;
   SemanticState* semantic = nullptr;   // w2v-BERT 2.0 prompt encoder (get_emb)
+  StreamJoin* sjoin = nullptr;         // idx_stream_vocode: the window tail kept on the device between two windows
 
   const DevTensor& W(const std::string& name) const {
     auto it = weights.find(name);
@@ -134,6 +136,7 @@ void s2mel_destroy(S2melState*);
 void emo_destroy(EmoState*);
 void v1voc_destroy(V1VocoderState*);
 void semantic_destroy(SemanticState*);
+void stream_join_destroy(StreamJoin*);
 
 #define IDX_API_BEGIN try {
 #define IDX_API_END(e)                                     \

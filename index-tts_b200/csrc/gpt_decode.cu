@@ -41,6 +41,7 @@
 #include <algorithm>
 #include <cstring>
 #include <cmath>
+#include <memory>
 #include <type_traits>
 
 namespace {
@@ -1682,6 +1683,7 @@ struct GptState {
   idx_gpt_config cfg;
   GptStrict* strict = nullptr;   // fp32 per-op path (weights_bf16 = 0)
   struct BeamTrace* beam_trace = nullptr;
+  struct GptStream* gstream = nullptr;   // the open resumable decode (idx_gpt_stream_begin .. idx_gpt_stream_end)
   int seq_base = 0;             // first request of the decode group being run (idx_gpt_generate splits large calls)
   int G = 0, FF = 0, nst = 0, bias_cap = 0, ocap = 0, bar_flavor = 0;
   size_t smem = 0;                // gpt_fused_kernel: dynamic shared memory with an nst-stage ring
@@ -1726,8 +1728,10 @@ struct GptState {
 };
 
 static void beam_trace_free(GptState* g);
+static void gpt_stream_free(GptState* g);
 void gpt_destroy(GptState* g) {
   if (!g) return;
+  gpt_stream_free(g);
   delete g->strict;
   beam_trace_free(g);
   for (void* p : g->owned) cudaFree(p);
@@ -1748,6 +1752,8 @@ static T* galloc(GptState* g, size_t n) {
 
 // the samplers' error flag: a top-k boundary tie wider than the CMAX candidate slots
 static const char* const kTieOverflow = "more than 128 tokens tie at the top-k boundary";
+// the GPT calls that would share the decode state with an open stream refuse to run
+static const char* const kStreamOpen = "a GPT stream is open (idx_gpt_stream_end closes it)";
 
 // ------------------------------------------------------------------ strict fp32 host path --
 struct StrictLayer {
@@ -2008,6 +2014,7 @@ extern "C" int idx_gpt_init(idx_engine* e, const idx_gpt_config* cfg) {
   IDX_API_BEGIN
   IDX_CHECK(e && cfg, IDX_ERR_ARG, "null argument");
   IDX_CUDA(cudaSetDevice(e->device));
+  IDX_CHECK(!e->gpt || !e->gpt->gstream, IDX_ERR_STATE, kStreamOpen);
   if (e->gpt) { gpt_destroy(e->gpt); e->gpt = nullptr; }
   // built into a local state and published only on success: a failed init must not leave a half-built e->gpt that passes the
   // "idx_gpt_init has not been called" guards (ADVICE r1)
@@ -2347,7 +2354,7 @@ static void beam_trace_reset(GptState* g, int m) {
 }
 
 // Device state of one beam search over nreq requests of m beam rows each (rows u * m + j of 8-row buffers, the layout
-// beam_step_kernel reads), carved from the engine arena.
+// beam_step_kernel reads), carved from an arena: the engine's for a generate call, the stream's own block for a stream.
 struct BeamBufs {
   int nreq = 0, m = 0, hs = 0, wv = 0, max_new = 0;
   unsigned* seen[2] = {nullptr, nullptr};
@@ -2365,24 +2372,24 @@ static size_t beam_bufs_bytes(int nreq, int m, int max_new, int V, bool want_log
   return need;
 }
 
-static BeamBufs beam_bufs_get(idx_engine* e, int nreq, int m, int max_new, int V, bool want_logits) {
+static BeamBufs beam_bufs_get(Arena& a, int nreq, int m, int max_new, int V, bool want_logits) {
   BeamBufs b;
   b.nreq = nreq; b.m = m; b.max_new = max_new; b.hs = max_new + 2; b.wv = (V + 31) / 32;
   const size_t wv = b.wv, hs = b.hs;
-  b.seen[0] = e->arena.get<unsigned>(8 * wv); b.seen[1] = e->arena.get<unsigned>(8 * wv);
-  b.hist[0] = e->arena.get<int>(8 * hs); b.hist[1] = e->arena.get<int>(8 * hs);
-  b.phys[0] = e->arena.get<unsigned char>(8 * hs + 16); b.phys[1] = e->arena.get<unsigned char>(8 * hs + 16);
-  b.bscore = e->arena.get<float>(8);
-  b.hscore = e->arena.get<double>((size_t)nreq * (m + 1) + 2);
-  b.worst = e->arena.get<double>(nreq + 2);
-  b.hlen = e->arena.get<int>((size_t)nreq * (m + 1));
-  b.horder = e->arena.get<int>((size_t)nreq * (m + 1));
-  b.nhyp = e->arena.get<int>(nreq);
-  b.done = e->arena.get<int>(nreq);
-  b.htok = e->arena.get<int>((size_t)nreq * (m + 1) * hs);
-  b.trpt = e->arena.get<int>((size_t)max_new * 16);
-  b.trsc = e->arena.get<float>((size_t)max_new * 8);
-  b.ldump = want_logits ? e->arena.get<float>((size_t)max_new * 8 * V) : nullptr;
+  b.seen[0] = a.get<unsigned>(8 * wv); b.seen[1] = a.get<unsigned>(8 * wv);
+  b.hist[0] = a.get<int>(8 * hs); b.hist[1] = a.get<int>(8 * hs);
+  b.phys[0] = a.get<unsigned char>(8 * hs + 16); b.phys[1] = a.get<unsigned char>(8 * hs + 16);
+  b.bscore = a.get<float>(8);
+  b.hscore = a.get<double>((size_t)nreq * (m + 1) + 2);
+  b.worst = a.get<double>(nreq + 2);
+  b.hlen = a.get<int>((size_t)nreq * (m + 1));
+  b.horder = a.get<int>((size_t)nreq * (m + 1));
+  b.nhyp = a.get<int>(nreq);
+  b.done = a.get<int>(nreq);
+  b.htok = a.get<int>((size_t)nreq * (m + 1) * hs);
+  b.trpt = a.get<int>((size_t)max_new * 16);
+  b.trsc = a.get<float>((size_t)max_new * 8);
+  b.ldump = want_logits ? a.get<float>((size_t)max_new * 8 * V) : nullptr;
   return b;
 }
 
@@ -2577,7 +2584,7 @@ static void beam_generate(idx_engine* e, GptState* g, const idx_gpt_request* req
   e->arena.reset();
   float* d_prompt = e->arena.get<float>((size_t)(total_rows + 8) * D);
   PrefillTile* d_tiles = e->arena.get<PrefillTile>(tiles.size());
-  const BeamBufs b = beam_bufs_get(e, nreq, m, max_new, V, want_logits);
+  const BeamBufs b = beam_bufs_get(e->arena, nreq, m, max_new, V, want_logits);
 
   IDX_CUDA(cudaEventRecord(g->ev0, st));
   for (int i = 0; i < nreq; ++i)
@@ -2648,7 +2655,7 @@ static void strict_beam_generate(idx_engine* e, GptState* g, const idx_gpt_reque
     e->ensure_arena((size_t)plen * D * 4 + beam_bufs_bytes(1, m, max_new, V, reqs[i].logits_out != nullptr) + (1 << 20));
     e->arena.reset();
     float* d_prompt = e->arena.get<float>((size_t)plen * D);
-    const BeamBufs b = beam_bufs_get(e, 1, m, max_new, V, reqs[i].logits_out != nullptr);
+    const BeamBufs b = beam_bufs_get(e->arena, 1, m, max_new, V, reqs[i].logits_out != nullptr);
     IDX_CUDA(cudaEventRecord(g->ev0, st));
     idx_to_device(e, d_prompt, reqs[i].prompt_emb, (size_t)plen * D * 4);
     beam_bufs_init(e, g, b);
@@ -2684,13 +2691,29 @@ static void strict_beam_generate(idx_engine* e, GptState* g, const idx_gpt_reque
   g->last_steps = max_steps;      // beam steps run, as on the fused path: the rows of each request's logits dump
 }
 
-extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int nreq,
-                                const idx_sampling* sp) {
-  IDX_API_BEGIN
-  IDX_CHECK(e && e->gpt, IDX_ERR_STATE, "idx_gpt_init has not been called");
-  IDX_CHECK(reqs && sp && nreq >= 1, IDX_ERR_ARG, "bad request");
-  GptState* g = e->gpt;
+// Step-0 state of nreq decode rows with num_beams = 1 (plen: [8] prompt lengths): start token, no codes yet, the fake
+// prompt ids in the repetition bitmaps.
+static void reset_rows(idx_engine* e, GptState* g, int nreq, const std::vector<int>& plen) {
   const idx_gpt_config& c = g->cfg;
+  const size_t wv = (size_t)((c.number_mel_codes + 31) / 32);
+  std::vector<int> h_tok(8, c.start_mel_token), zeros(8, 0);
+  std::vector<unsigned> h_seen(8 * wv, 0u);
+  for (int i = 0; i < nreq; ++i) {
+    // P2: the fake prompt ids [1,...,1, start_mel] are part of input_ids
+    h_seen[i * wv + (1 >> 5)] |= 1u << 1;
+    h_seen[i * wv + (c.start_mel_token >> 5)] |= 1u << (c.start_mel_token & 31);
+  }
+  IDX_CUDA(cudaMemcpyAsync(g->tok, h_tok.data(), 32, cudaMemcpyHostToDevice, e->stream));
+  IDX_CUDA(cudaMemcpyAsync(g->nout, zeros.data(), 32, cudaMemcpyHostToDevice, e->stream));
+  IDX_CUDA(cudaMemcpyAsync(g->finished, zeros.data(), 32, cudaMemcpyHostToDevice, e->stream));
+  IDX_CUDA(cudaMemcpyAsync(g->done, zeros.data(), 4, cudaMemcpyHostToDevice, e->stream));
+  IDX_CUDA(cudaMemcpyAsync(g->prompt_len, plen.data(), 32, cudaMemcpyHostToDevice, e->stream));
+  IDX_CUDA(cudaMemcpyAsync(g->seen, h_seen.data(), h_seen.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  IDX_CUDA(cudaStreamSynchronize(e->stream));  // host vectors go out of scope
+}
+
+// The sampler inputs every decode path refuses (idx_gpt_generate, idx_gpt_stream_begin).
+static void check_sampling(const idx_sampling* sp) {
   IDX_CHECK(sp->num_beams >= 1, IDX_ERR_ARG, "num_beams must be >= 1");
   // HF semantics are kept exactly or refused: top_k = 0 (warper disabled) or top_k > CMAX would need more candidate slots
   // than the device samplers hold, and capping them silently would change the support of the top-p / multinomial step
@@ -2705,6 +2728,17 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   // the paths read the mode as `mel_pos_mode == 1`: any other value would silently decode with the KV-cache rule
   IDX_CHECK(sp->mel_pos_mode == 0 || sp->mel_pos_mode == 1, IDX_ERR_ARG,
             "mel_pos_mode must be 0 (mel position k + 1 at step k >= 1, KV cache) or 1 (position k, no cache)");
+}
+
+extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int nreq,
+                                const idx_sampling* sp) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && e->gpt, IDX_ERR_STATE, "idx_gpt_init has not been called");
+  IDX_CHECK(!e->gpt->gstream, IDX_ERR_STATE, kStreamOpen);
+  IDX_CHECK(reqs && sp && nreq >= 1, IDX_ERR_ARG, "bad request");
+  GptState* g = e->gpt;
+  const idx_gpt_config& c = g->cfg;
+  check_sampling(sp);
   // an armed attention probe is consumed by this call, whatever its outcome
   const int probe_on = g->probe_armed, pprobe_on = g->pprobe_armed;
   g->probe_armed = g->pprobe_armed = 0;
@@ -2778,7 +2812,6 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   for (int i = 0; i < nreq; ++i)
     for (int p0 = 0; p0 < plen[i]; p0 += 8)
       tiles.push_back({i, p0, std::min(8, plen[i] - p0), row0[i] + p0});
-  const size_t wv = (size_t)((V + 31) / 32);
   size_t need = (size_t)(total_rows + 8) * D * 4 + tiles.size() * sizeof(PrefillTile) + 8 * (size_t)max_new * 8 + 4096;
   bool want_logits = false, want_forced = false;
   for (int i = 0; i < nreq; ++i) { want_logits |= reqs[i].logits_out != nullptr; want_forced |= reqs[i].forced_codes != nullptr; }
@@ -2802,23 +2835,7 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
       idx_to_device(e, d_forced + (size_t)i * max_new, reqs[i].forced_codes, (size_t)max_new * 4);
     }
   }
-  // per-sequence state
-  {
-    std::vector<int> h_tok(8, c.start_mel_token), zeros(8, 0);
-    std::vector<unsigned> h_seen(8 * wv, 0u);
-    for (int i = 0; i < nreq; ++i) {
-      // P2: the fake prompt ids [1,...,1, start_mel] are part of input_ids
-      h_seen[i * wv + (1 >> 5)] |= 1u << 1;
-      h_seen[i * wv + (c.start_mel_token >> 5)] |= 1u << (c.start_mel_token & 31);
-    }
-    IDX_CUDA(cudaMemcpyAsync(g->tok, h_tok.data(), 32, cudaMemcpyHostToDevice, e->stream));
-    IDX_CUDA(cudaMemcpyAsync(g->nout, zeros.data(), 32, cudaMemcpyHostToDevice, e->stream));
-    IDX_CUDA(cudaMemcpyAsync(g->finished, zeros.data(), 32, cudaMemcpyHostToDevice, e->stream));
-    IDX_CUDA(cudaMemcpyAsync(g->done, zeros.data(), 4, cudaMemcpyHostToDevice, e->stream));
-    IDX_CUDA(cudaMemcpyAsync(g->prompt_len, plen.data(), 32, cudaMemcpyHostToDevice, e->stream));
-    IDX_CUDA(cudaMemcpyAsync(g->seen, h_seen.data(), h_seen.size() * 4, cudaMemcpyHostToDevice, e->stream));
-    IDX_CUDA(cudaStreamSynchronize(e->stream));  // host vectors go out of scope
-  }
+  reset_rows(e, g, nreq, plen);
 
   // ---- prefill: tiles of 8 prompt positions through the same fused kernel ----
   GptParams p;
@@ -2878,6 +2895,266 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   g->t_prefill_ms = ms01;
   g->t_decode_ms = ms12;
   g->last_steps = maxn;
+  IDX_API_END(e)
+}
+
+// ------------------------------------------------------------------ resumable decode (streaming) --
+// One request decoded a few codes at a time (include/idxtts.h idx_gpt_stream_*).  The decode runs exactly the launches
+// idx_gpt_generate runs for that request, only split at other step boundaries: every step's Philox counter is (step,
+// sequence) and the tagged hand-over epochs carry across launches, so the split changes no code.  Everything the decode
+// needs between two calls lives in one device block the stream owns, never in the engine arena: the tail calls that run
+// between two idx_gpt_stream_next calls reset the arena.
+namespace {
+// The committed prefix of a beam stream (one request): the longest common prefix of every candidate that can still become
+// the result, i.e. the live beams' histories (until the request is done) and the stored finished hypotheses.  Any later
+// hypothesis descends from a live beam, so the prefix never shrinks.  codes[0, lcp) = the prefix, *ncommit = lcp.
+__global__ void __launch_bounds__(256) beam_commit_kernel(const int* hist, int hs, int m, int steps, const int* htok,
+                                                          const int* hlen, const int* horder, const int* nhyp,
+                                                          const int* done, int* codes, int* ncommit) {
+  __shared__ const int* cand[2 * BEAM_MAX + 2];
+  __shared__ int nc, len0, lcp;
+  if (threadIdx.x == 0) {
+    int n = 0, len = 0x7fffffff;
+    if (!*done)
+      for (int j = 0; j < m; ++j) { cand[n++] = hist + (size_t)j * hs; len = min(len, steps); }
+    for (int q = 0; q < *nhyp; ++q) {
+      const int slot = horder[q];
+      cand[n++] = htok + (size_t)slot * hs;
+      len = min(len, hlen[slot]);
+    }
+    nc = n;
+    len0 = n ? len : 0;
+    lcp = len0;
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < len0; t += blockDim.x) {
+    const int v = cand[0][t];
+    for (int i = 1; i < nc; ++i)
+      if (cand[i][t] != v) { atomicMin(&lcp, t); break; }
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < lcp; t += blockDim.x) codes[t] = cand[0][t];
+  if (threadIdx.x == 0) *ncommit = lcp;
+}
+}  // namespace
+
+struct GptStream {
+  idx_sampling sp;
+  int m = 1, max_new = 0;
+  bool dec1 = false;                   // num_beams = 1: gpt_decode1_kernel (else gpt_fused_kernel), as idx_gpt_generate picks
+  int steps = 0, committed = 0, finished = 0;
+  void* mem = nullptr;                 // the stream's device block, carved by `a`
+  Arena a;
+  int* codes = nullptr;                // [max_new + 2]: the decode's codes (num_beams 1) / the committed prefix (beams)
+  int* ncommit = nullptr;              // beams: length of the committed prefix at the last poll
+  BeamBufs b;
+  BeamParams bp;
+  GptParams p;                         // the decode launches' parameters
+  std::vector<int> held;               // beams: the codes committed so far
+  ~GptStream() { if (mem) cudaFree(mem); }
+};
+
+static void gpt_stream_free(GptState* g) { delete g->gstream; g->gstream = nullptr; }
+
+static GptStream* open_stream(idx_engine* e) {
+  IDX_CHECK(e && e->gpt && e->gpt->gstream, IDX_ERR_STATE, "no GPT stream is open (idx_gpt_stream_begin opens one)");
+  return e->gpt->gstream;
+}
+
+extern "C" int idx_gpt_stream_begin(idx_engine* e, const idx_gpt_request* req, const idx_sampling* sp) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && e->gpt, IDX_ERR_STATE, "idx_gpt_init has not been called");
+  GptState* g = e->gpt;
+  IDX_CHECK(!g->gstream, IDX_ERR_STATE, kStreamOpen);
+  IDX_CHECK(req && sp, IDX_ERR_ARG, "null argument");
+  IDX_CHECK(!g->strict, IDX_ERR_ARG, "idx_gpt_stream_begin: the strict fp32 path (weights_bf16 = 0) has no resumable decode");
+  IDX_CHECK(!req->forced_codes, IDX_ERR_ARG, "idx_gpt_stream_begin: forced_codes is not defined for a stream");
+  check_sampling(sp);
+  const idx_gpt_config& c = g->cfg;
+  const int m = sp->num_beams, max_new = sp->max_new_tokens, D = c.model_dim, V = c.number_mel_codes;
+  IDX_CHECK(m <= BEAM_MAX && m <= c.max_batch, IDX_ERR_ARG, "num_beams must be 1..4 and <= max_batch (one row per beam)");
+  IDX_CHECK(V <= 40 * 256, IDX_ERR_ARG, "vocabulary too large for the device sampler");
+  IDX_CHECK(max_new >= 1 && max_new + 2 <= c.max_mel_positions, IDX_ERR_ARG,
+            "max_new_tokens must satisfy k+1 <= mel_pos rows - 1 (SURVEY A.3)");
+  const int plen = req->prompt_len;
+  IDX_CHECK(req->prompt_emb && plen >= 1 && plen <= c.max_prompt, IDX_ERR_ARG, "bad prompt");
+  IDX_CHECK(plen + max_new + 1 <= g->maxpos, IDX_ERR_ARG, "KV cache too small");
+  IDX_CUDA(cudaSetDevice(e->device));
+  cudaStream_t st = e->stream;
+
+  std::unique_ptr<GptStream> s(new GptStream());
+  s->sp = *sp; s->m = m; s->max_new = max_new;
+  std::vector<PrefillTile> tiles;
+  for (int p0 = 0; p0 < plen; p0 += 8) tiles.push_back({0, p0, std::min(8, plen - p0), p0});
+  const size_t bytes = (size_t)(plen + 8) * D * 4 + tiles.size() * sizeof(PrefillTile) + (size_t)(max_new + 2) * 4 + 64 +
+                       (m > 1 ? beam_bufs_bytes(1, m, max_new, V, false) : 0) + 8 * 256;
+  IDX_CUDA(cudaMalloc(&s->mem, bytes));
+  s->a.base = (char*)s->mem;
+  s->a.cap = bytes;
+  float* d_prompt = s->a.get<float>((size_t)(plen + 8) * D);
+  PrefillTile* d_tiles = s->a.get<PrefillTile>(tiles.size());
+  s->codes = s->a.get<int>((size_t)max_new + 2);
+  s->ncommit = s->a.get<int>(16);
+  idx_to_device(e, d_prompt, req->prompt_emb, (size_t)plen * D * 4);
+  IDX_CUDA(cudaMemcpyAsync(d_tiles, tiles.data(), tiles.size() * sizeof(PrefillTile), cudaMemcpyHostToDevice, st));
+  std::vector<int> plen8(8, 0);
+  if (m > 1) {
+    s->b = beam_bufs_get(s->a, 1, m, max_new, V, false);
+    for (int j = 0; j < m; ++j) plen8[j] = plen;
+    std::vector<int> zeros(16, 0);
+    IDX_CUDA(cudaMemcpyAsync(g->finished, zeros.data(), 32, cudaMemcpyHostToDevice, st));
+    IDX_CUDA(cudaMemcpyAsync(g->done, zeros.data(), 4, cudaMemcpyHostToDevice, st));
+    IDX_CUDA(cudaMemcpyAsync(g->prompt_len, plen8.data(), 32, cudaMemcpyHostToDevice, st));
+    beam_bufs_init(e, g, s->b);
+  } else {
+    plen8[0] = plen;
+    reset_rows(e, g, 1, plen8);
+  }
+
+  // prefill: the prompt as tiles of 8 positions (beams: into the first beam's slot), as idx_gpt_generate runs it
+  GptParams& p = s->p;
+  fill_common(e, g, p);
+  p.B = 8; p.mode = 0; p.nsteps = (int)tiles.size(); p.prompt = d_prompt; p.tiles = d_tiles;
+  p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
+  if (m > 1) p.beams = m;
+  launch_fused(e, g, p);
+
+  fill_common(e, g, p);
+  if (m > 1) {
+    p.B = m; p.mode = 1; p.max_new = max_new; p.ext_sample = 1; p.beams = m; p.phys_stride = s->b.hs;
+    p.pos_plain = sp->mel_pos_mode == 1;
+    s->bp = beam_params(e, g, s->b, sp, g->logits, g->seq_base);
+  } else {
+    p.B = 1; p.mode = 1; p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
+    p.forbid_stop_before = sp->forbid_stop_before;
+    p.do_sample = sp->do_sample; p.top_k = sp->top_k; p.top_p = sp->top_p; p.temperature = sp->temperature;
+    p.seed = sp->seed;
+    p.seq_base = g->seq_base;
+    p.pos_plain = sp->mel_pos_mode == 1;
+    p.codes = s->codes;
+    s->dec1 = g->v2 != 0;
+  }
+  IDX_CUDA(cudaStreamSynchronize(st));   // the prompt block is not read again
+  g->gstream = s.release();
+  IDX_API_END(e)
+}
+
+// num_beams = 1: every decoded code is committed; launches end exactly at `until` (at most 64 steps for the batch-1 kernel,
+// 32 for gpt_fused_kernel, as in idx_gpt_generate).
+static void stream_next1(idx_engine* e, GptState* g, GptStream* s, int until) {
+  GptParams& p = s->p;
+  const int SPL = s->dec1 ? 64 : 32;
+  int* h = (int*)e->pinned_buf(64);
+  while (!s->finished && s->steps < until && s->steps < s->max_new) {
+    p.step0 = s->steps;
+    p.nsteps = std::min(SPL, std::min(until, s->max_new) - s->steps);
+    if (s->dec1) launch_decode1(e, g, p);
+    else launch_fused(e, g, p);
+    IDX_CUDA(cudaMemcpyAsync(h, g->done, 4, cudaMemcpyDeviceToHost, e->stream));
+    IDX_CUDA(cudaMemcpyAsync(h + 1, g->nout, 4, cudaMemcpyDeviceToHost, e->stream));
+    IDX_CUDA(cudaStreamSynchronize(e->stream));
+    s->steps += p.nsteps;
+    s->committed = h[1];
+    s->finished = h[0] != 0;
+  }
+  e->check_flag(kTieOverflow);
+}
+
+// num_beams > 1: one beam step per launch; at each poll of beam_step (every 8 steps) the committed prefix grows to the
+// longest common prefix of the candidates; at the end it becomes beam_finish's result.
+static void stream_next_beams(idx_engine* e, GptState* g, GptStream* s, int until) {
+  GptParams& p = s->p;
+  const BeamBufs& b = s->b;
+  cudaStream_t st = e->stream;
+  while (!s->finished && s->committed < until) {
+    const int k = s->steps;
+    p.step0 = k; p.nsteps = 1; p.phys = b.phys[k & 1];
+    launch_fused(e, g, p);
+    s->steps = k + 1;
+    const bool all = beam_step(e, g, s->bp, b, k);
+    if ((k & 7) != 7 && k + 1 != s->max_new) continue;   // no poll at this step
+    e->check_flag(kTieOverflow);
+    if (all || k + 1 == s->max_new) {
+      int n = 0;
+      idx_gpt_request rq;
+      memset(&rq, 0, sizeof(rq));
+      rq.codes_out = s->codes;
+      rq.n_codes_out = &n;
+      beam_trace_reset(g, s->m);
+      beam_finish(e, g, &rq, &s->sp, b, s->steps);
+      std::vector<int> fin(n);
+      IDX_CUDA(cudaMemcpyAsync(fin.data(), s->codes, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+      IDX_CUDA(cudaStreamSynchronize(st));
+      IDX_CHECK(n >= s->committed && std::equal(s->held.begin(), s->held.end(), fin.begin()), IDX_ERR_STATE,
+                "internal: the beam result does not extend the committed prefix");
+      s->held = fin;
+      s->committed = n;
+      s->finished = 1;
+      break;
+    }
+    beam_commit_kernel<<<1, 256, 0, st>>>(b.hist[s->steps & 1], b.hs, b.m, s->steps, b.htok, b.hlen, b.horder, b.nhyp,
+                                          b.done, s->codes, s->ncommit);
+    IDX_CUDA(cudaGetLastError());
+    e->launches++;
+    int* h = (int*)e->pinned_buf(64);
+    IDX_CUDA(cudaMemcpyAsync(h, s->ncommit, 4, cudaMemcpyDeviceToHost, st));
+    IDX_CUDA(cudaStreamSynchronize(st));
+    const int n = h[0];
+    IDX_CHECK(n >= s->committed, IDX_ERR_STATE, "internal: the committed prefix of a beam stream shrank");
+    if (n > s->committed) {
+      s->held.resize(n);
+      IDX_CUDA(cudaMemcpyAsync(s->held.data() + s->committed, s->codes + s->committed, (size_t)(n - s->committed) * 4,
+                               cudaMemcpyDeviceToHost, st));
+      IDX_CUDA(cudaStreamSynchronize(st));
+      s->committed = n;
+    }
+  }
+}
+
+extern "C" int idx_gpt_stream_next(idx_engine* e, int32_t until, int32_t* codes_out, int32_t* n_committed,
+                                   int32_t* finished) {
+  IDX_API_BEGIN
+  GptStream* s = open_stream(e);
+  IDX_CHECK(until >= 1, IDX_ERR_ARG, "idx_gpt_stream_next: until must be >= 1");
+  IDX_CHECK(codes_out, IDX_ERR_ARG, "idx_gpt_stream_next: null codes_out");
+  IDX_CUDA(cudaSetDevice(e->device));
+  const int old = s->committed;
+  if (s->m == 1) stream_next1(e, e->gpt, s, until);
+  else stream_next_beams(e, e->gpt, s, until);
+  if (s->committed > old) idx_from_device(e, codes_out + old, s->codes + old, (size_t)(s->committed - old) * 4);
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  if (n_committed) *n_committed = s->committed;
+  if (finished) *finished = s->finished;
+  IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_stream_end(idx_engine* e) {
+  IDX_API_BEGIN
+  open_stream(e);
+  IDX_CUDA(cudaSetDevice(e->device));
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  gpt_stream_free(e->gpt);
+  IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_stream_beam_state(idx_engine* e, int32_t* hist, int32_t* hyp_tok, int32_t* hyp_len,
+                                         int32_t* hyp_order, int32_t* nhyp_done, int32_t* steps) {
+  IDX_API_BEGIN
+  GptStream* s = open_stream(e);
+  IDX_CHECK(s->m > 1, IDX_ERR_STATE, "idx_gpt_stream_beam_state: the open stream is not a beam search");
+  IDX_CUDA(cudaSetDevice(e->device));
+  const BeamBufs& b = s->b;
+  const size_t hs = b.hs, m = b.m;
+  if (hist) idx_from_device(e, hist, b.hist[s->steps & 1], m * hs * 4);
+  if (hyp_tok) idx_from_device(e, hyp_tok, b.htok, (m + 1) * hs * 4);
+  if (hyp_len) idx_from_device(e, hyp_len, b.hlen, (m + 1) * 4);
+  if (hyp_order) idx_from_device(e, hyp_order, b.horder, (m + 1) * 4);
+  if (nhyp_done) {
+    idx_from_device(e, nhyp_done, b.nhyp, 4);
+    idx_from_device(e, nhyp_done + 1, b.done, 4);
+  }
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  if (steps) *steps = s->steps;
   IDX_API_END(e)
 }
 
@@ -2948,6 +3225,7 @@ extern "C" int idx_gpt_profile_fine(idx_engine* e, int64_t* stamps_out, int n) {
 extern "C" int idx_gpt_probe_attention(idx_engine* e, int layer, int max_steps, int max_seqs, float* qo_out, int32_t* nsplit_out) {
   IDX_API_BEGIN
   IDX_CHECK(e && e->gpt && !e->gpt->strict, IDX_ERR_STATE, "idx_gpt_init (bf16 path) has not been called");
+  IDX_CHECK(!e->gpt->gstream, IDX_ERR_STATE, kStreamOpen);
   GptState* g = e->gpt;
   IDX_CHECK(layer >= -1 && layer < g->cfg.layers, IDX_ERR_ARG, "layer must be -1 (all) or a layer index");
   IDX_CHECK(max_steps >= 1 && max_seqs >= 1 && max_seqs <= 8 && qo_out && nsplit_out, IDX_ERR_ARG, "bad probe buffers");
@@ -2963,6 +3241,7 @@ extern "C" int idx_gpt_probe_attention(idx_engine* e, int layer, int max_steps, 
 extern "C" int idx_gpt_probe_prefill(idx_engine* e, int layer, int max_rows, int max_seqs, float* qo_out) {
   IDX_API_BEGIN
   IDX_CHECK(e && e->gpt && !e->gpt->strict, IDX_ERR_STATE, "idx_gpt_init (bf16 path) has not been called");
+  IDX_CHECK(!e->gpt->gstream, IDX_ERR_STATE, kStreamOpen);
   GptState* g = e->gpt;
   IDX_CHECK(layer >= -1 && layer < g->cfg.layers, IDX_ERR_ARG, "layer must be -1 (all) or a layer index");
   IDX_CHECK(max_rows >= 1 && max_seqs >= 1 && max_seqs <= 8 && qo_out, IDX_ERR_ARG, "bad probe buffers");
@@ -2977,6 +3256,7 @@ extern "C" int idx_gpt_probe_prefill(idx_engine* e, int layer, int max_rows, int
 extern "C" int idx_gpt_debug_kv(idx_engine* e, int layer, int seq, int pos0, int n, float* k_out, float* v_out) {
   IDX_API_BEGIN
   IDX_CHECK(e && e->gpt && !e->gpt->strict, IDX_ERR_STATE, "idx_gpt_init (bf16 path) has not been called");
+  IDX_CHECK(!e->gpt->gstream, IDX_ERR_STATE, kStreamOpen);
   GptState* g = e->gpt;
   const idx_gpt_config& c = g->cfg;
   IDX_CHECK(layer >= 0 && layer < c.layers && seq >= 0 && seq < c.max_batch && pos0 >= 0 && n >= 1 && pos0 + n <= g->maxpos &&
@@ -3085,6 +3365,7 @@ extern "C" int idx_gpt_latents_v1(idx_engine* e, const float* conds, int n_laten
   IDX_CHECK(e && e->gpt, IDX_ERR_STATE, "idx_gpt_init has not been called");
   IDX_CHECK(conds && codes && latents_out && n_latents >= 1 && n_text >= 0 && n_codes >= 1, IDX_ERR_ARG, "bad arguments");
   IDX_CUDA(cudaSetDevice(e->device));
+  IDX_CHECK(!e->gpt->gstream, IDX_ERR_STATE, kStreamOpen);
   GptState* g = e->gpt;
   GptStrict* s = g->strict;
   const int D = g->cfg.model_dim, R = n_latents + n_text + 2 + n_codes + 2;

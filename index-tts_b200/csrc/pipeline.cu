@@ -19,6 +19,26 @@ __global__ void pcm16_kernel(const float* wav, int16_t* pcm, long long n) {
   float v = fminf(fmaxf(32767.f * wav[i], -32767.f), 32767.f);
   pcm[i] = (int16_t)v;
 }
+// One window of a chunked stream joined onto the tail the previous window kept (include/idxtts.h idx_stream_vocode), with
+// the rules of the reference's StreamingDecoder.generate: out[i] = tail[i] * fade_out[i] + wav[i] * fade_in[i] for i < nb
+// (the two halves of np.hanning(2 nb)), wav[src0 + i - nb] after that; the last 512 samples scaled by np.linspace(1, 0,
+// 512) when `fade`; int16 with the truncation of pcm16_kernel.  In double, as numpy computes the blend.
+__global__ void stream_join_kernel(const float* wav, const float* tail, int nb, long long src0, long long n_out, int fade,
+                                   int16_t* pcm) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_out) return;
+  double v;
+  if (i < nb) {
+    const double w = 6.283185307179586 / (2.0 * nb - 1.0);
+    const double fade_in = 0.5 - 0.5 * cos(w * (double)i), fade_out = 0.5 - 0.5 * cos(w * (double)(nb + i));
+    v = (double)tail[i] * fade_out + (double)wav[i] * fade_in;
+  } else {
+    v = (double)wav[src0 + i - nb];
+  }
+  if (fade && i >= n_out - 512) v *= 1.0 - (double)(i - (n_out - 512)) / 511.0;
+  v = fmin(fmax(32767.0 * v, -32767.0), 32767.0);
+  pcm[i] = (int16_t)v;
+}
 // why the tail refuses a request, or nullptr
 const char* request_error(const idx_vocode_request* r) {
   if (!(r->codes && r->n_codes >= 1 && r->F >= 1 && r->P >= 0 && r->style && r->z)) return "bad request";
@@ -169,6 +189,102 @@ void codes_to_wav(idx_engine* e, const idx_vocode_request* reqs, int n, int n_st
   bigvgan_set_ms(bv, ms_bv);
 }
 }  // namespace
+
+// idx_stream_vocode's device state: the last overlap_samples of the previous window (kept until the next window blends
+// them in) and the window's waveform and int16 buffers, all engine-owned: the tail runs of the windows reset the arena.
+struct StreamJoin {
+  float* tail = nullptr;
+  long long tail_len = 0, tail_cap = 0;
+  bool has_tail = false;      // false: the next window is joined as the first one
+  float* wav = nullptr;
+  int16_t* pcm = nullptr;
+  long long wav_cap = 0, pcm_cap = 0;
+};
+
+void stream_join_destroy(StreamJoin* j) {
+  if (!j) return;
+  cudaFree(j->tail);
+  cudaFree(j->wav);
+  cudaFree(j->pcm);
+  delete j;
+}
+
+namespace {
+// grow a device buffer to n elements, keeping its first `keep` elements
+template <typename T>
+void grow(idx_engine* e, T*& buf, long long& cap, long long n, long long keep) {
+  if (cap >= n) return;
+  T* nb = nullptr;
+  IDX_CUDA(cudaMalloc((void**)&nb, (size_t)n * sizeof(T)));
+  if (keep > 0) IDX_CUDA(cudaMemcpyAsync(nb, buf, (size_t)keep * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  cudaFree(buf);
+  buf = nb;
+  cap = n;
+}
+}  // namespace
+
+extern "C" int idx_stream_vocode(idx_engine* e, const idx_vocode_request* r, int n_steps, float cfg_rate,
+                                 int32_t overlap_samples, int32_t flags, int16_t* pcm_out, int32_t* n_pcm) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && pcm_out && n_pcm, IDX_ERR_ARG, "idx_stream_vocode: null argument");
+  IDX_CHECK((flags & ~(IDX_STREAM_FIRST | IDX_STREAM_LAST)) == 0, IDX_ERR_ARG, "idx_stream_vocode: unknown flags");
+  const bool first = flags & IDX_STREAM_FIRST, last = flags & IDX_STREAM_LAST;
+  IDX_CHECK(r || last, IDX_ERR_ARG, "idx_stream_vocode: a NULL window is the flush and needs IDX_STREAM_LAST");
+  IDX_CHECK(overlap_samples >= 0, IDX_ERR_ARG, "idx_stream_vocode: overlap_samples must be >= 0");
+  IDX_CUDA(cudaSetDevice(e->device));
+  if (!e->sjoin) e->sjoin = new StreamJoin();
+  StreamJoin* j = e->sjoin;
+  const bool joined = !first && j->has_tail;          // a window without a kept tail is joined as the first one
+  const long long kept = joined ? j->tail_len : 0, ovlp = overlap_samples;
+  long long len = 0;
+  if (r) {
+    IDX_CHECK(e->bigvgan, IDX_ERR_STATE, "s2mel / codec / bigvgan not initialised");
+    IDX_CHECK(r->F >= 1, IDX_ERR_ARG, "bad request");
+    len = (long long)r->F * bigvgan_total_up(e->bigvgan);
+    IDX_CHECK(last || len >= 2 * ovlp, IDX_ERR_ARG,
+              "idx_stream_vocode: a window that is not the last needs F * 256 >= 2 * overlap_samples");
+  }
+  IDX_CHECK((long long)*n_pcm >= len + kept, IDX_ERR_ARG,
+            "idx_stream_vocode: *n_pcm (the capacity of pcm_out) must be >= F * 256 plus the kept tail (at most the previous "
+            "window's overlap_samples)");
+  // what is emitted: nb blended samples, then wav[src0, src0 + n_out - nb)
+  long long nb = 0, src0 = 0, n_out = 0;
+  if (!r) {
+    n_out = kept;
+  } else if (!joined) {
+    n_out = last ? len : len - ovlp;
+  } else {
+    const long long head = std::min(ovlp, len), rest = std::max(0LL, len - ovlp);
+    nb = std::min(kept, head);
+    src0 = std::min(ovlp, len);
+    n_out = last ? nb + rest : nb + rest - ovlp;
+  }
+  grow(e, j->pcm, j->pcm_cap, std::max(n_out, 1LL), 0);
+  if (r) {
+    grow(e, j->wav, j->wav_cap, len, 0);
+    idx_vocode_request w = *r;                        // the window's tail: the driver of idx_codes_to_wav
+    w.wav_out = j->wav;
+    codes_to_wav(e, &w, 1, n_steps, cfg_rate, false);
+    if (r->wav_out) idx_from_device(e, r->wav_out, j->wav, (size_t)len * 4);
+  }
+  if (n_out > 0) {      // the window's waveform, or the kept tail for the flush (read after the buffers have grown)
+    stream_join_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, e->stream>>>(r ? j->wav : j->tail, j->tail, (int)nb, src0, n_out,
+                                                                             last && n_out > 512, j->pcm);
+    IDX_CUDA(cudaGetLastError()); e->launches++;
+    idx_from_device(e, pcm_out, j->pcm, (size_t)n_out * 2);
+  }
+  if (r && !last) {                                   // keep the window's last overlap_samples for the next one
+    grow(e, j->tail, j->tail_cap, std::max(ovlp, 1LL), 0);
+    if (ovlp > 0)
+      IDX_CUDA(cudaMemcpyAsync(j->tail, j->wav + (len - ovlp), (size_t)ovlp * 4, cudaMemcpyDeviceToDevice, e->stream));
+  }
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  j->has_tail = r && !last;
+  j->tail_len = j->has_tail ? ovlp : 0;
+  *n_pcm = (int32_t)n_out;
+  IDX_API_END(e)
+}
 
 extern "C" int idx_codes_to_wav(idx_engine* e, const idx_vocode_request* r, int n_steps, float cfg_rate) {
   IDX_API_BEGIN

@@ -251,6 +251,12 @@ def load_library(path: str = None):
         C.c_longlong, C.c_void_p, C.c_void_p]
     lib.idx_codes_to_wav.argtypes = [C.c_void_p, C.POINTER(VocodeRequest), C.c_int, C.c_float]
     lib.idx_codes_to_wav_batch.argtypes = [C.c_void_p, C.POINTER(VocodeRequest), C.c_int, C.c_int, C.c_float]
+    lib.idx_gpt_stream_begin.argtypes = [C.c_void_p, C.POINTER(GptRequest), C.POINTER(Sampling)]
+    lib.idx_gpt_stream_next.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    lib.idx_gpt_stream_end.argtypes = [C.c_void_p]
+    lib.idx_gpt_stream_beam_state.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.POINTER(C.c_int32)]
+    lib.idx_stream_vocode.argtypes = [C.c_void_p, C.POINTER(VocodeRequest), C.c_int, C.c_float, C.c_int32, C.c_int32,
+                                      C.c_void_p, C.POINTER(C.c_int32)]
     _lib = lib
     return lib
 
@@ -304,6 +310,53 @@ class _OrderedLib:
                 raw.idx_wait_stream(eng.h, C.c_void_p(torch.cuda.current_stream(eng.device).cuda_stream))
             return fn(*a)
         return call
+
+
+class GptStream:
+    """An open resumable decode (Engine.gpt_stream).  `codes` holds every code committed so far."""
+
+    def __init__(self, eng, max_new_tokens, num_beams):
+        self._eng, self.num_beams = eng, num_beams
+        self._buf = np.zeros(max_new_tokens, dtype=np.int32)
+        self.n_committed, self.finished, self._open = 0, False, True
+
+    @property
+    def codes(self):
+        return self._buf[:self.n_committed]
+
+    def next(self, until):
+        """Decode until at least `until` codes are committed (or the sequence has finished); returns (the newly committed
+        codes as int32, finished)."""
+        eng, old = self._eng, self.n_committed
+        n, fin = C.c_int32(0), C.c_int32(0)
+        eng._check(eng.lib.idx_gpt_stream_next(eng.h, int(until), _ptr(self._buf), C.byref(n), C.byref(fin)),
+                   "idx_gpt_stream_next")
+        self.n_committed, self.finished = int(n.value), bool(fin.value)
+        return self._buf[old:self.n_committed].copy(), self.finished
+
+    def beam_state(self):
+        """Diagnostic: the beam buffers as the last poll left them (include/idxtts.h idx_gpt_stream_beam_state)."""
+        eng, m, hs = self._eng, self.num_beams, len(self._buf) + 2
+        hist = np.zeros((m, hs), np.int32)
+        htok = np.zeros((m + 1, hs), np.int32)
+        hlen, horder, nd = np.zeros(m + 1, np.int32), np.zeros(m + 1, np.int32), np.zeros(2, np.int32)
+        steps = C.c_int32(0)
+        eng._check(eng.lib.idx_gpt_stream_beam_state(eng.h, _ptr(hist), _ptr(htok), _ptr(hlen), _ptr(horder), _ptr(nd),
+                                                     C.byref(steps)), "idx_gpt_stream_beam_state")
+        return dict(hist=hist, hyp_tok=htok, hyp_len=hlen, hyp_order=horder, nhyp=int(nd[0]), done=bool(nd[1]),
+                    steps=int(steps.value))
+
+    def close(self):
+        if self._open:
+            self._open = False
+            self._eng._check(self._eng.lib.idx_gpt_stream_end(self._eng.h), "idx_gpt_stream_end")
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+        return False
 
 
 class Engine:
@@ -434,6 +487,28 @@ class Engine:
                 return out, [logits[i][:steps] for i in range(n)]
             return out, [logits[i][: int(ncodes[i][0])] for i in range(n)]
         return out
+
+    def gpt_stream(self, prompt, max_new_tokens, repetition_penalty=10.0, do_sample=False, num_beams=1, top_k=0,
+                   top_p=1.0, temperature=1.0, length_penalty=0.0, seed=0, forbid_stop_before=0, forced_codes=None,
+                   return_logits=False, mel_pos_mode=0):
+        """Resumable decode of one prompt (include/idxtts.h idx_gpt_stream_*): the arguments of gpt_generate for one
+        request; the prefill runs here.  Returns a GptStream: `.next(until)` decodes until at least `until` codes are
+        committed and returns (the newly committed codes, finished).  Over the whole stream the codes are those
+        gpt_generate returns.  Close it with `.close()` or a `with` block: GPT calls are refused while it is open."""
+        if return_logits:
+            raise ValueError("gpt_stream does not return logits")
+        pr = _as_f32(prompt)
+        req = GptRequest()
+        req.prompt_emb = _ptr(pr)
+        req.prompt_len = int(pr.shape[0])
+        if forced_codes is not None:        # passed through: the library refuses teacher forcing on a stream
+            fc = np.zeros(max_new_tokens, dtype=np.int32)
+            req.forced_codes = _ptr(fc)
+        sp = Sampling(int(do_sample), int(num_beams), int(top_k), float(top_p), float(temperature),
+                      float(repetition_penalty), float(length_penalty), int(max_new_tokens),
+                      int(seed), int(forbid_stop_before), int(mel_pos_mode))
+        self._check(self.lib.idx_gpt_stream_begin(self.h, C.byref(req), C.byref(sp)), "idx_gpt_stream_begin")
+        return GptStream(self, int(max_new_tokens), int(num_beams))
 
     # ------------------------------------------------------- v1 / v1.5 GPT side (row a13) --
     def v1_cond_init(self, c: dict, n_latents=32):
@@ -675,6 +750,32 @@ class Engine:
         Returns dict(wav=[F*256] f32, pcm16=..., mel=[80,F])."""
         r, res, _ = self._vocode_request(codes, prompt_condition, ref_mel, style, z, F, want_wav, want_pcm16, want_mel)
         self._check(self.lib.idx_codes_to_wav(self.h, C.byref(r), int(n_steps), float(cfg_rate)), "idx_codes_to_wav")
+        return res
+
+    def stream_vocode(self, codes=None, prompt_condition=None, ref_mel=None, style=None, z=None, F=0, overlap_samples=0,
+                      first=False, last=False, n_steps=25, cfg_rate=0.7, want_wav=False):
+        """One window of a chunked stream (include/idxtts.h idx_stream_vocode): the window runs through the tail of
+        codes_to_wav, then its waveform is cross-faded onto the last overlap_samples the previous window kept on the
+        device.  first: drop any kept tail; last: emit everything, faded out over its last 512 samples.  codes=None with
+        last=True flushes the kept tail.  Buffers pass through as in codes_to_wav (the int16 output lives where z lives).
+        Returns dict(pcm=int16 [emitted samples], wav=[F*256] f32 of the window when want_wav)."""
+        if first:
+            self._join_kept = 0
+        kept = getattr(self, "_join_kept", 0)
+        if codes is None:
+            r, res, keep, n = None, {}, None, kept
+        else:
+            r, res, keep = self._vocode_request(codes, prompt_condition, ref_mel, style, z, F, want_wav, False, False)
+            n = int(F) * self._bigvgan_up + kept
+        on_dev = codes is not None and _is_cuda(z)
+        pcm = torch.empty(max(n, 1), dtype=torch.int16, device=z.device) if on_dev else np.empty(max(n, 1), dtype=np.int16)
+        n_pcm = C.c_int32(n)
+        flags = (1 if first else 0) | (2 if last else 0)
+        self._check(self.lib.idx_stream_vocode(self.h, None if r is None else C.byref(r), int(n_steps), float(cfg_rate),
+                                               int(overlap_samples), flags, _ptr(pcm), C.byref(n_pcm)),
+                    "idx_stream_vocode")
+        self._join_kept = 0 if (last or codes is None) else int(overlap_samples)
+        res["pcm"] = pcm[:n_pcm.value]
         return res
 
     def codes_to_wav_batch(self, requests, n_steps=25, cfg_rate=0.7, want_wav=True, want_pcm16=False, want_mel=False):
