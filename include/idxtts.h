@@ -196,6 +196,28 @@ int idx_gpt_stream_end(idx_engine* e);
  * *steps the beam steps run.  Any of them may be NULL.  IDX_ERR_STATE without an open beam stream.                */
 int idx_gpt_stream_beam_state(idx_engine* e, int32_t* hist, int32_t* hyp_tok, int32_t* hyp_len, int32_t* hyp_order,
                               int32_t* nhyp_done, int32_t* steps);
+/* Resumable decode of a GROUP of nreq requests (idx_gpt_stream_begin / _next / _beam_state are its nreq = 1 case).  Over a
+ * whole stream request i's codes are bitwise those idx_gpt_generate(e, reqs, nreq, sp) returns for request i: the same
+ * kernel (gpt_decode1_kernel for nreq = 1, gpt_decode8_kernel for nreq > 1, gpt_fused_kernel under IDX_GPT_V8=0 and with
+ * beams), the same Philox sequence index i, only other launch boundaries.
+ *   begin  as idx_gpt_stream_begin; also refused (IDX_ERR_ARG) when the group does not fit in one decode group:
+ *          nreq * num_beams > max_batch.  The stream never splits into consecutive groups.
+ *   next   until [nreq] (each >= 1), codes_out [nreq] pointers (host or device, [max_new_tokens] each), n_committed and
+ *          finished [nreq] (may be NULL).  Decodes, and returns as soon as some unfinished request has at least until[i]
+ *          committed codes, some request finished during the call, or every request is finished; request i's newly
+ *          committed codes go to codes_out[i][old, new).
+ *          num_beams = 1: the rows advance in lockstep; every launch ends at the smallest until[i] of the unfinished
+ *          requests (at most 64 steps per launch with gpt_decode1_kernel, 32 otherwise).
+ *          num_beams = 2..4: at every poll (every 8 steps) one kernel computes each request's committed prefix (the LCP of
+ *          its live beams and stored hypotheses).  A request whose scorer is done is finished at that poll with the
+ *          hypothesis BeamSearchScorer.finalize picks from its stored hypotheses; the rest finish when the group ends.
+ *   beam_state  idx_gpt_stream_beam_state for request `req` of a beam stream.
+ * end: idx_gpt_stream_end.  The state rules of idx_gpt_stream_begin hold: one open stream per engine (of any nreq).  */
+int idx_gpt_stream_begin_batch(idx_engine* e, const idx_gpt_request* reqs, int nreq, const idx_sampling* sp);
+int idx_gpt_stream_next_batch(idx_engine* e, const int32_t* until, int32_t* const* codes_out, int32_t* n_committed,
+                              int32_t* finished);
+int idx_gpt_stream_beam_state_batch(idx_engine* e, int32_t req, int32_t* hist, int32_t* hyp_tok, int32_t* hyp_len,
+                                    int32_t* hyp_order, int32_t* nhyp_done, int32_t* steps);
 
 /* Build the [cond(3)][start_text, text.., stop_text] prompt embeddings of
  * prepare_gpt_inputs (gpt/model_v2.py:648-714,754-768) on the device.
@@ -595,6 +617,21 @@ int idx_codes_to_wav_batch(idx_engine* e, const idx_vocode_request* reqs, int n,
 enum { IDX_STREAM_FIRST = 1, IDX_STREAM_LAST = 2 };
 int idx_stream_vocode(idx_engine* e, const idx_vocode_request* r, int n_steps, float cfg_rate, int32_t overlap_samples,
                       int32_t flags, int16_t* pcm_out, int32_t* n_pcm);
+/* Several streams' windows in one call (idx_stream_vocode is its one-window, slot-0 case).  Each of IDX_STREAM_SLOTS
+ * slots keeps its own tail between calls.  The non-NULL windows run through ONE idx_codes_to_wav_batch driver call (one
+ * packed CFM solve in the default tail mode), so each window's waveform is bitwise that of its solo idx_codes_to_wav; one
+ * kernel then joins every window onto its slot's kept tail by the rules of idx_stream_vocode.  Every window is checked
+ * before any work (slot range, a slot used twice, flags, overlap, capacity, the request); a refusal (IDX_ERR_ARG) names
+ * the window's index, emits nothing and leaves every slot's kept tail as it was.                                    */
+enum { IDX_STREAM_SLOTS = 8 };
+typedef struct {
+  int32_t slot;                       /* 0..IDX_STREAM_SLOTS-1: the stream whose kept tail this window joins         */
+  const idx_vocode_request* window;   /* NULL: flush the slot's kept tail (needs IDX_STREAM_LAST)                     */
+  int32_t overlap_samples, flags;     /* as idx_stream_vocode                                                         */
+  int16_t* pcm_out;                   /* as idx_stream_vocode                                                         */
+  int32_t* n_pcm;                     /* as idx_stream_vocode: capacity in, samples emitted out                       */
+} idx_stream_window;
+int idx_stream_vocode_batch(idx_engine* e, const idx_stream_window* w, int n, int n_steps, float cfg_rate);
 
 /* Device ms of the last codec decode / length regulator / CFM solve (CUDA events).       */
 int idx_s2mel_last_ms(const idx_engine* e, double* ms3);

@@ -2463,57 +2463,48 @@ static bool beam_step(idx_engine* e, GptState* g, BeamParams& bp, const BeamBufs
   return all;
 }
 
-// BeamSearchScorer.finalize (transformers_beam_search.py:322-420) on the host after `steps` beam steps: each request's best
-// hypothesis to codes_out / n_codes_out, its beams' logits to logits_out [steps][m][V], and its trace appended to
-// g->beam_trace.
-static void beam_finish(idx_engine* e, GptState* g, const idx_gpt_request* reqs, const idx_sampling* sp, const BeamBufs& b,
-                       int steps) {
-  const idx_gpt_config& c = g->cfg;
-  cudaStream_t st = e->stream;
-  const int nreq = b.nreq, m = b.m, hs = b.hs, max_new = b.max_new, V = c.number_mel_codes;
-  const int fin = steps & 1;      // buffers written by the last beam step
-  std::vector<int> h_hist(8 * (size_t)hs), h_hlen((size_t)nreq * (m + 1)), h_horder((size_t)nreq * (m + 1)), h_nhyp(nreq), h_dn(nreq);
-  std::vector<int> h_htok((size_t)nreq * (m + 1) * hs);
-  std::vector<double> h_hscore((size_t)nreq * (m + 1) + 2);
-  std::vector<float> h_bs(8);
-  std::vector<int> h_pt((size_t)steps * 16);
-  std::vector<float> h_sc((size_t)steps * 8);
-  IDX_CUDA(cudaMemcpyAsync(h_hist.data(), b.hist[fin], h_hist.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_hlen.data(), b.hlen, h_hlen.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_horder.data(), b.horder, h_horder.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_nhyp.data(), b.nhyp, nreq * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_dn.data(), b.done, nreq * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_htok.data(), b.htok, h_htok.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_hscore.data(), b.hscore, (size_t)nreq * (m + 1) * 8, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_bs.data(), b.bscore, 32, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_pt.data(), b.trpt, h_pt.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaMemcpyAsync(h_sc.data(), b.trsc, h_sc.size() * 4, cudaMemcpyDeviceToHost, st));
-  IDX_CUDA(cudaStreamSynchronize(st));
-  for (int u = 0; u < nreq; ++u) {
-    BeamTrace::Utt tu;
-    tu.steps = steps;
-    tu.pt.resize((size_t)steps * m * 2);
-    tu.sc.resize((size_t)steps * m);
-    for (int k = 0; k < steps; ++k)
-      for (int j = 0; j < m; ++j) {
-        const size_t r = (size_t)k * 8 + u * m + j;
-        tu.pt[((size_t)k * m + j) * 2] = h_pt[r * 2];
-        tu.pt[((size_t)k * m + j) * 2 + 1] = h_pt[r * 2 + 1];
-        tu.sc[(size_t)k * m + j] = h_sc[r];
-      }
+// Host copies of the beam buffers after `steps` beam steps (trace: also the per-step parent / token / score trace).
+struct BeamHost {
+  std::vector<int> hist, hlen, horder, nhyp, dn, htok, pt;
+  std::vector<double> hscore;
+  std::vector<float> bs, sc;
+  BeamHost(idx_engine* e, const BeamBufs& b, int steps, bool trace) {
+    cudaStream_t st = e->stream;
+    const size_t nreq = b.nreq, m1 = b.m + 1, hs = b.hs;
+    hist.resize(8 * hs); hlen.resize(nreq * m1); horder.resize(nreq * m1); nhyp.resize(nreq); dn.resize(nreq);
+    htok.resize(nreq * m1 * hs); hscore.resize(nreq * m1 + 2); bs.resize(8);
+    IDX_CUDA(cudaMemcpyAsync(hist.data(), b.hist[steps & 1], hist.size() * 4, cudaMemcpyDeviceToHost, st));  // last step's
+    IDX_CUDA(cudaMemcpyAsync(hlen.data(), b.hlen, hlen.size() * 4, cudaMemcpyDeviceToHost, st));
+    IDX_CUDA(cudaMemcpyAsync(horder.data(), b.horder, horder.size() * 4, cudaMemcpyDeviceToHost, st));
+    IDX_CUDA(cudaMemcpyAsync(nhyp.data(), b.nhyp, nreq * 4, cudaMemcpyDeviceToHost, st));
+    IDX_CUDA(cudaMemcpyAsync(dn.data(), b.done, nreq * 4, cudaMemcpyDeviceToHost, st));
+    IDX_CUDA(cudaMemcpyAsync(htok.data(), b.htok, htok.size() * 4, cudaMemcpyDeviceToHost, st));
+    IDX_CUDA(cudaMemcpyAsync(hscore.data(), b.hscore, nreq * m1 * 8, cudaMemcpyDeviceToHost, st));
+    IDX_CUDA(cudaMemcpyAsync(bs.data(), b.bscore, 32, cudaMemcpyDeviceToHost, st));
+    if (trace) {
+      pt.resize((size_t)steps * 16);
+      sc.resize((size_t)steps * 8);
+      IDX_CUDA(cudaMemcpyAsync(pt.data(), b.trpt, pt.size() * 4, cudaMemcpyDeviceToHost, st));
+      IDX_CUDA(cudaMemcpyAsync(sc.data(), b.trsc, sc.size() * 4, cudaMemcpyDeviceToHost, st));
+    }
+    IDX_CUDA(cudaStreamSynchronize(st));
+  }
+  // BeamSearchScorer.finalize's pick for request u: its codes (the stop token appended below max_new) and score.  Once the
+  // request is done only its stored hypotheses take part, so from then on the pick cannot change.
+  std::vector<int> pick(int u, int m, int hs, int steps, int max_new, int stop_tok, float length_penalty, double* score) const {
     struct Hyp { double score; const int* tok; int len; };
     std::vector<Hyp> list;
-    for (int q = 0; q < h_nhyp[u]; ++q) {
-      const int slot = h_horder[(size_t)u * (m + 1) + q];
-      list.push_back({h_hscore[(size_t)u * (m + 1) + slot], &h_htok[((size_t)u * (m + 1) + slot) * hs], h_hlen[(size_t)u * (m + 1) + slot]});
+    for (int q = 0; q < nhyp[u]; ++q) {
+      const int slot = horder[(size_t)u * (m + 1) + q];
+      list.push_back({hscore[(size_t)u * (m + 1) + slot], &htok[((size_t)u * (m + 1) + slot) * hs], hlen[(size_t)u * (m + 1) + slot]});
     }
     double worst = 1e9;
     for (auto& h : list) worst = std::min(worst, h.score);
-    if (!h_dn[u]) {
+    if (!dn[u]) {
       for (int j = 0; j < m; ++j) {           // add the live beams (:345-356); generated_len = steps
-        const double score = (double)h_bs[u * m + j] / std::pow((double)steps, (double)sp->length_penalty);
+        const double score = (double)bs[u * m + j] / std::pow((double)steps, (double)length_penalty);
         if ((int)list.size() < m || score > worst) {
-          list.push_back({score, &h_hist[(size_t)(u * m + j) * hs], steps});
+          list.push_back({score, &hist[(size_t)(u * m + j) * hs], steps});
           if ((int)list.size() > m) {
             size_t lo = 0;
             for (size_t q = 1; q < list.size(); ++q) if (list[q].score < list[lo].score) lo = q;
@@ -2530,8 +2521,34 @@ static void beam_finish(idx_engine* e, GptState* g, const idx_gpt_request* reqs,
     size_t best = 0;
     for (size_t q = 1; q < list.size(); ++q) if (list[q].score >= list[best].score) best = q;
     std::vector<int> codes(list[best].tok, list[best].tok + list[best].len);
-    if ((int)codes.size() < max_new) codes.push_back(c.stop_mel_token);
-    tu.final_score = list[best].score;
+    if ((int)codes.size() < max_new) codes.push_back(stop_tok);
+    if (score) *score = list[best].score;
+    return codes;
+  }
+};
+
+// BeamSearchScorer.finalize (transformers_beam_search.py:322-420) on the host after `steps` beam steps: each request's best
+// hypothesis to codes_out / n_codes_out, its beams' logits to logits_out [steps][m][V], and its trace appended to
+// g->beam_trace.
+static void beam_finish(idx_engine* e, GptState* g, const idx_gpt_request* reqs, const idx_sampling* sp, const BeamBufs& b,
+                       int steps) {
+  const idx_gpt_config& c = g->cfg;
+  cudaStream_t st = e->stream;
+  const int nreq = b.nreq, m = b.m, hs = b.hs, max_new = b.max_new, V = c.number_mel_codes;
+  const BeamHost h(e, b, steps, true);
+  for (int u = 0; u < nreq; ++u) {
+    BeamTrace::Utt tu;
+    tu.steps = steps;
+    tu.pt.resize((size_t)steps * m * 2);
+    tu.sc.resize((size_t)steps * m);
+    for (int k = 0; k < steps; ++k)
+      for (int j = 0; j < m; ++j) {
+        const size_t r = (size_t)k * 8 + u * m + j;
+        tu.pt[((size_t)k * m + j) * 2] = h.pt[r * 2];
+        tu.pt[((size_t)k * m + j) * 2 + 1] = h.pt[r * 2 + 1];
+        tu.sc[(size_t)k * m + j] = h.sc[r];
+      }
+    const std::vector<int> codes = h.pick(u, m, hs, steps, max_new, c.stop_mel_token, sp->length_penalty, &tu.final_score);
     g->beam_trace->utt.push_back(std::move(tu));
     if (reqs[u].n_codes_out) *reqs[u].n_codes_out = (int)codes.size();
     if (reqs[u].codes_out) {
@@ -2899,26 +2916,28 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
 }
 
 // ------------------------------------------------------------------ resumable decode (streaming) --
-// One request decoded a few codes at a time (include/idxtts.h idx_gpt_stream_*).  The decode runs exactly the launches
-// idx_gpt_generate runs for that request, only split at other step boundaries: every step's Philox counter is (step,
-// sequence) and the tagged hand-over epochs carry across launches, so the split changes no code.  Everything the decode
-// needs between two calls lives in one device block the stream owns, never in the engine arena: the tail calls that run
-// between two idx_gpt_stream_next calls reset the arena.
+// A group of nreq requests decoded a few codes at a time (include/idxtts.h idx_gpt_stream_*).  The decode runs exactly the
+// launches idx_gpt_generate runs for that group, only split at other step boundaries: every step's Philox counter is
+// (step, sequence) and the tagged hand-over epochs carry across launches, so the split changes no code.  Everything the
+// decode needs between two calls lives in one device block the stream owns, never in the engine arena: the tail calls
+// that run between two idx_gpt_stream_next calls reset the arena.
 namespace {
-// The committed prefix of a beam stream (one request): the longest common prefix of every candidate that can still become
-// the result, i.e. the live beams' histories (until the request is done) and the stored finished hypotheses.  Any later
-// hypothesis descends from a live beam, so the prefix never shrinks.  codes[0, lcp) = the prefix, *ncommit = lcp.
+// The committed prefix of each request of a beam stream (block u: request u): the longest common prefix of every
+// candidate that can still become the result, i.e. the live beams' histories (until the request is done) and the stored
+// finished hypotheses.  Any later hypothesis descends from a live beam, so the prefix never shrinks.
+// codes[u * cs, u * cs + lcp) = the prefix, ncommit[u] = lcp.
 __global__ void __launch_bounds__(256) beam_commit_kernel(const int* hist, int hs, int m, int steps, const int* htok,
                                                           const int* hlen, const int* horder, const int* nhyp,
-                                                          const int* done, int* codes, int* ncommit) {
+                                                          const int* done, int* codes, int cs, int* ncommit) {
   __shared__ const int* cand[2 * BEAM_MAX + 2];
   __shared__ int nc, len0, lcp;
+  const int u = blockIdx.x;
   if (threadIdx.x == 0) {
     int n = 0, len = 0x7fffffff;
-    if (!*done)
-      for (int j = 0; j < m; ++j) { cand[n++] = hist + (size_t)j * hs; len = min(len, steps); }
-    for (int q = 0; q < *nhyp; ++q) {
-      const int slot = horder[q];
+    if (!done[u])
+      for (int j = 0; j < m; ++j) { cand[n++] = hist + (size_t)(u * m + j) * hs; len = min(len, steps); }
+    for (int q = 0; q < nhyp[u]; ++q) {
+      const int slot = u * (m + 1) + horder[u * (m + 1) + q];
       cand[n++] = htok + (size_t)slot * hs;
       len = min(len, hlen[slot]);
     }
@@ -2933,24 +2952,26 @@ __global__ void __launch_bounds__(256) beam_commit_kernel(const int* hist, int h
       if (cand[i][t] != v) { atomicMin(&lcp, t); break; }
   }
   __syncthreads();
-  for (int t = threadIdx.x; t < lcp; t += blockDim.x) codes[t] = cand[0][t];
-  if (threadIdx.x == 0) *ncommit = lcp;
+  for (int t = threadIdx.x; t < lcp; t += blockDim.x) codes[(size_t)u * cs + t] = cand[0][t];
+  if (threadIdx.x == 0) ncommit[u] = lcp;
 }
 }  // namespace
 
 struct GptStream {
   idx_sampling sp;
-  int m = 1, max_new = 0;
-  bool dec1 = false;                   // num_beams = 1: gpt_decode1_kernel (else gpt_fused_kernel), as idx_gpt_generate picks
-  int steps = 0, committed = 0, finished = 0;
+  int nreq = 1, m = 1, max_new = 0;
+  int cs = 0;                          // stride of a request's row of `codes`
+  int kind = 0;                        // num_beams = 1: 1 gpt_decode1_kernel, 8 gpt_decode8_kernel, 0 gpt_fused_kernel
+  int steps = 0;
+  int committed[8] = {}, finished[8] = {};
   void* mem = nullptr;                 // the stream's device block, carved by `a`
   Arena a;
-  int* codes = nullptr;                // [max_new + 2]: the decode's codes (num_beams 1) / the committed prefix (beams)
-  int* ncommit = nullptr;              // beams: length of the committed prefix at the last poll
+  int* codes = nullptr;                // [nreq][cs]: the decode's codes (num_beams 1) / the committed prefixes (beams)
+  int* ncommit = nullptr;              // beams: [nreq] length of each committed prefix at the last poll
   BeamBufs b;
   BeamParams bp;
   GptParams p;                         // the decode launches' parameters
-  std::vector<int> held;               // beams: the codes committed so far
+  std::vector<int> held[8];            // beams: the codes committed so far, per request
   ~GptStream() { if (mem) cudaFree(mem); }
 };
 
@@ -2961,57 +2982,68 @@ static GptStream* open_stream(idx_engine* e) {
   return e->gpt->gstream;
 }
 
-extern "C" int idx_gpt_stream_begin(idx_engine* e, const idx_gpt_request* req, const idx_sampling* sp) {
+extern "C" int idx_gpt_stream_begin_batch(idx_engine* e, const idx_gpt_request* reqs, int nreq, const idx_sampling* sp) {
   IDX_API_BEGIN
   IDX_CHECK(e && e->gpt, IDX_ERR_STATE, "idx_gpt_init has not been called");
   GptState* g = e->gpt;
   IDX_CHECK(!g->gstream, IDX_ERR_STATE, kStreamOpen);
-  IDX_CHECK(req && sp, IDX_ERR_ARG, "null argument");
+  IDX_CHECK(reqs && sp && nreq >= 1, IDX_ERR_ARG, "null argument or nreq < 1");
   IDX_CHECK(!g->strict, IDX_ERR_ARG, "idx_gpt_stream_begin: the strict fp32 path (weights_bf16 = 0) has no resumable decode");
-  IDX_CHECK(!req->forced_codes, IDX_ERR_ARG, "idx_gpt_stream_begin: forced_codes is not defined for a stream");
+  for (int i = 0; i < nreq; ++i)
+    IDX_CHECK(!reqs[i].forced_codes, IDX_ERR_ARG, "idx_gpt_stream_begin: forced_codes is not defined for a stream");
   check_sampling(sp);
   const idx_gpt_config& c = g->cfg;
   const int m = sp->num_beams, max_new = sp->max_new_tokens, D = c.model_dim, V = c.number_mel_codes;
   IDX_CHECK(m <= BEAM_MAX && m <= c.max_batch, IDX_ERR_ARG, "num_beams must be 1..4 and <= max_batch (one row per beam)");
+  IDX_CHECK(nreq * m <= c.max_batch && nreq * m <= 8, IDX_ERR_ARG,
+            "a stream is one decode group: nreq * num_beams must be <= max_batch (<= 8)");
   IDX_CHECK(V <= 40 * 256, IDX_ERR_ARG, "vocabulary too large for the device sampler");
   IDX_CHECK(max_new >= 1 && max_new + 2 <= c.max_mel_positions, IDX_ERR_ARG,
             "max_new_tokens must satisfy k+1 <= mel_pos rows - 1 (SURVEY A.3)");
-  const int plen = req->prompt_len;
-  IDX_CHECK(req->prompt_emb && plen >= 1 && plen <= c.max_prompt, IDX_ERR_ARG, "bad prompt");
-  IDX_CHECK(plen + max_new + 1 <= g->maxpos, IDX_ERR_ARG, "KV cache too small");
+  int total_rows = 0;
+  std::vector<int> plen(8, 0), row0(8, 0);
+  for (int i = 0; i < nreq; ++i) {
+    IDX_CHECK(reqs[i].prompt_emb && reqs[i].prompt_len >= 1 && reqs[i].prompt_len <= c.max_prompt, IDX_ERR_ARG, "bad prompt");
+    IDX_CHECK(reqs[i].prompt_len + max_new + 1 <= g->maxpos, IDX_ERR_ARG, "KV cache too small");
+    plen[i] = reqs[i].prompt_len;
+    row0[i] = total_rows;
+    total_rows += plen[i];
+  }
   IDX_CUDA(cudaSetDevice(e->device));
   cudaStream_t st = e->stream;
 
   std::unique_ptr<GptStream> s(new GptStream());
-  s->sp = *sp; s->m = m; s->max_new = max_new;
-  std::vector<PrefillTile> tiles;
-  for (int p0 = 0; p0 < plen; p0 += 8) tiles.push_back({0, p0, std::min(8, plen - p0), p0});
-  const size_t bytes = (size_t)(plen + 8) * D * 4 + tiles.size() * sizeof(PrefillTile) + (size_t)(max_new + 2) * 4 + 64 +
-                       (m > 1 ? beam_bufs_bytes(1, m, max_new, V, false) : 0) + 8 * 256;
+  s->sp = *sp; s->nreq = nreq; s->m = m; s->max_new = max_new;
+  s->cs = m > 1 ? max_new + 2 : max_new;           // num_beams 1: the kernels' layout, codes[b * max_new + k]
+  std::vector<PrefillTile> tiles;                  // beams: the prompt KV lives in the first beam's slot
+  for (int i = 0; i < nreq; ++i)
+    for (int p0 = 0; p0 < plen[i]; p0 += 8) tiles.push_back({i * m, p0, std::min(8, plen[i] - p0), row0[i] + p0});
+  const size_t bytes = (size_t)(total_rows + 8) * D * 4 + tiles.size() * sizeof(PrefillTile) + (size_t)8 * (max_new + 2) * 4 +
+                       64 + (m > 1 ? beam_bufs_bytes(nreq, m, max_new, V, false) : 0) + 8 * 256;
   IDX_CUDA(cudaMalloc(&s->mem, bytes));
   s->a.base = (char*)s->mem;
   s->a.cap = bytes;
-  float* d_prompt = s->a.get<float>((size_t)(plen + 8) * D);
+  float* d_prompt = s->a.get<float>((size_t)(total_rows + 8) * D);
   PrefillTile* d_tiles = s->a.get<PrefillTile>(tiles.size());
-  s->codes = s->a.get<int>((size_t)max_new + 2);
+  s->codes = s->a.get<int>((size_t)8 * (max_new + 2));
   s->ncommit = s->a.get<int>(16);
-  idx_to_device(e, d_prompt, req->prompt_emb, (size_t)plen * D * 4);
+  for (int i = 0; i < nreq; ++i)
+    idx_to_device(e, d_prompt + (size_t)row0[i] * D, reqs[i].prompt_emb, (size_t)plen[i] * D * 4);
   IDX_CUDA(cudaMemcpyAsync(d_tiles, tiles.data(), tiles.size() * sizeof(PrefillTile), cudaMemcpyHostToDevice, st));
-  std::vector<int> plen8(8, 0);
   if (m > 1) {
-    s->b = beam_bufs_get(s->a, 1, m, max_new, V, false);
-    for (int j = 0; j < m; ++j) plen8[j] = plen;
-    std::vector<int> zeros(16, 0);
+    s->b = beam_bufs_get(s->a, nreq, m, max_new, V, false);
+    std::vector<int> plen_rows(8, 0), zeros(16, 0);
+    for (int i = 0; i < nreq; ++i)
+      for (int j = 0; j < m; ++j) plen_rows[i * m + j] = plen[i];
     IDX_CUDA(cudaMemcpyAsync(g->finished, zeros.data(), 32, cudaMemcpyHostToDevice, st));
     IDX_CUDA(cudaMemcpyAsync(g->done, zeros.data(), 4, cudaMemcpyHostToDevice, st));
-    IDX_CUDA(cudaMemcpyAsync(g->prompt_len, plen8.data(), 32, cudaMemcpyHostToDevice, st));
+    IDX_CUDA(cudaMemcpyAsync(g->prompt_len, plen_rows.data(), 32, cudaMemcpyHostToDevice, st));
     beam_bufs_init(e, g, s->b);
   } else {
-    plen8[0] = plen;
-    reset_rows(e, g, 1, plen8);
+    reset_rows(e, g, nreq, plen);
   }
 
-  // prefill: the prompt as tiles of 8 positions (beams: into the first beam's slot), as idx_gpt_generate runs it
+  // prefill: the prompts as tiles of 8 positions, as idx_gpt_generate runs them
   GptParams& p = s->p;
   fill_common(e, g, p);
   p.B = 8; p.mode = 0; p.nsteps = (int)tiles.size(); p.prompt = d_prompt; p.tiles = d_tiles;
@@ -3021,52 +3053,76 @@ extern "C" int idx_gpt_stream_begin(idx_engine* e, const idx_gpt_request* req, c
 
   fill_common(e, g, p);
   if (m > 1) {
-    p.B = m; p.mode = 1; p.max_new = max_new; p.ext_sample = 1; p.beams = m; p.phys_stride = s->b.hs;
+    p.B = nreq * m; p.mode = 1; p.max_new = max_new; p.ext_sample = 1; p.beams = m; p.phys_stride = s->b.hs;
     p.pos_plain = sp->mel_pos_mode == 1;
     s->bp = beam_params(e, g, s->b, sp, g->logits, g->seq_base);
   } else {
-    p.B = 1; p.mode = 1; p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
+    p.B = nreq; p.mode = 1; p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
     p.forbid_stop_before = sp->forbid_stop_before;
     p.do_sample = sp->do_sample; p.top_k = sp->top_k; p.top_p = sp->top_p; p.temperature = sp->temperature;
     p.seed = sp->seed;
     p.seq_base = g->seq_base;
     p.pos_plain = sp->mel_pos_mode == 1;
     p.codes = s->codes;
-    s->dec1 = g->v2 != 0;
+    s->kind = (nreq == 1 && g->v2) ? 1 : (nreq > 1 && g->v8) ? 8 : 0;   // the kernel idx_gpt_generate picks
   }
   IDX_CUDA(cudaStreamSynchronize(st));   // the prompt block is not read again
   g->gstream = s.release();
   IDX_API_END(e)
 }
 
-// num_beams = 1: every decoded code is committed; launches end exactly at `until` (at most 64 steps for the batch-1 kernel,
-// 32 for gpt_fused_kernel, as in idx_gpt_generate).
-static void stream_next1(idx_engine* e, GptState* g, GptStream* s, int until) {
+extern "C" int idx_gpt_stream_begin(idx_engine* e, const idx_gpt_request* req, const idx_sampling* sp) {
+  return idx_gpt_stream_begin_batch(e, req, 1, sp);
+}
+
+// Whether a next call returns now: some unfinished request reached its `until`, some request finished during the call
+// (fin0: the finished flags at its start), or every request is finished.
+static bool stream_stop(const GptStream* s, const int32_t* until, const int* fin0) {
+  bool all = true;
+  for (int i = 0; i < s->nreq; ++i) {
+    if (s->finished[i] && !fin0[i]) return true;
+    if (!s->finished[i] && s->committed[i] >= until[i]) return true;
+    all &= s->finished[i] != 0;
+  }
+  return all;
+}
+
+// num_beams = 1: the rows advance in lockstep and every decoded code is committed; each launch ends at the smallest
+// `until` of the unfinished requests (at most 64 steps for the batch-1 kernel, 32 otherwise, as in idx_gpt_generate).
+static void stream_next1(idx_engine* e, GptState* g, GptStream* s, const int32_t* until, const int* fin0) {
   GptParams& p = s->p;
-  const int SPL = s->dec1 ? 64 : 32;
-  int* h = (int*)e->pinned_buf(64);
-  while (!s->finished && s->steps < until && s->steps < s->max_new) {
+  const int SPL = s->kind == 1 ? 64 : 32;
+  int* h = (int*)e->pinned_buf(128);
+  while (!stream_stop(s, until, fin0)) {
+    int end = s->max_new;
+    for (int i = 0; i < s->nreq; ++i)
+      if (!s->finished[i]) end = std::min(end, (int)until[i]);
     p.step0 = s->steps;
-    p.nsteps = std::min(SPL, std::min(until, s->max_new) - s->steps);
-    if (s->dec1) launch_decode1(e, g, p);
+    p.nsteps = std::min(SPL, end - s->steps);
+    if (s->kind == 1) launch_decode1(e, g, p);
+    else if (s->kind == 8) launch_decode8(e, g, p);
     else launch_fused(e, g, p);
-    IDX_CUDA(cudaMemcpyAsync(h, g->done, 4, cudaMemcpyDeviceToHost, e->stream));
-    IDX_CUDA(cudaMemcpyAsync(h + 1, g->nout, 4, cudaMemcpyDeviceToHost, e->stream));
+    IDX_CUDA(cudaMemcpyAsync(h, g->nout, 32, cudaMemcpyDeviceToHost, e->stream));
+    IDX_CUDA(cudaMemcpyAsync(h + 8, g->finished, 32, cudaMemcpyDeviceToHost, e->stream));
     IDX_CUDA(cudaStreamSynchronize(e->stream));
     s->steps += p.nsteps;
-    s->committed = h[1];
-    s->finished = h[0] != 0;
+    for (int i = 0; i < s->nreq; ++i) {
+      s->committed[i] = h[i];
+      s->finished[i] = h[8 + i] != 0;
+    }
   }
   e->check_flag(kTieOverflow);
 }
 
-// num_beams > 1: one beam step per launch; at each poll of beam_step (every 8 steps) the committed prefix grows to the
-// longest common prefix of the candidates; at the end it becomes beam_finish's result.
-static void stream_next_beams(idx_engine* e, GptState* g, GptStream* s, int until) {
+// num_beams > 1: one beam step per launch; at each poll of beam_step (every 8 steps) every request's committed prefix
+// grows to the longest common prefix of its candidates, and a request whose scorer is done takes its final hypothesis;
+// where the group ends, beam_finish's results must extend (and, for the requests already finished, equal) them.
+static void stream_next_beams(idx_engine* e, GptState* g, GptStream* s, const int32_t* until, const int* fin0) {
   GptParams& p = s->p;
   const BeamBufs& b = s->b;
+  const int nreq = s->nreq, cs = s->cs, stop = g->cfg.stop_mel_token;
   cudaStream_t st = e->stream;
-  while (!s->finished && s->committed < until) {
+  while (!stream_stop(s, until, fin0)) {
     const int k = s->steps;
     p.step0 = k; p.nsteps = 1; p.phys = b.phys[k & 1];
     launch_fused(e, g, p);
@@ -3075,57 +3131,95 @@ static void stream_next_beams(idx_engine* e, GptState* g, GptStream* s, int unti
     if ((k & 7) != 7 && k + 1 != s->max_new) continue;   // no poll at this step
     e->check_flag(kTieOverflow);
     if (all || k + 1 == s->max_new) {
-      int n = 0;
-      idx_gpt_request rq;
-      memset(&rq, 0, sizeof(rq));
-      rq.codes_out = s->codes;
-      rq.n_codes_out = &n;
+      std::vector<int> n(nreq, 0);
+      std::vector<idx_gpt_request> rq(nreq);
+      for (int u = 0; u < nreq; ++u) {
+        memset(&rq[u], 0, sizeof(idx_gpt_request));
+        rq[u].codes_out = s->codes + (size_t)u * cs;
+        rq[u].n_codes_out = &n[u];
+      }
       beam_trace_reset(g, s->m);
-      beam_finish(e, g, &rq, &s->sp, b, s->steps);
-      std::vector<int> fin(n);
-      IDX_CUDA(cudaMemcpyAsync(fin.data(), s->codes, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-      IDX_CUDA(cudaStreamSynchronize(st));
-      IDX_CHECK(n >= s->committed && std::equal(s->held.begin(), s->held.end(), fin.begin()), IDX_ERR_STATE,
-                "internal: the beam result does not extend the committed prefix");
-      s->held = fin;
-      s->committed = n;
-      s->finished = 1;
+      beam_finish(e, g, rq.data(), &s->sp, b, s->steps);
+      for (int u = 0; u < nreq; ++u) {
+        std::vector<int> fin(n[u]);
+        IDX_CUDA(cudaMemcpyAsync(fin.data(), s->codes + (size_t)u * cs, (size_t)n[u] * 4, cudaMemcpyDeviceToHost, st));
+        IDX_CUDA(cudaStreamSynchronize(st));
+        IDX_CHECK(n[u] >= s->committed[u] && std::equal(s->held[u].begin(), s->held[u].end(), fin.begin()), IDX_ERR_STATE,
+                  "internal: the beam result does not extend the committed prefix");
+        IDX_CHECK(!s->finished[u] || n[u] == s->committed[u], IDX_ERR_STATE,
+                  "internal: the beam result of a request differs from the result it was finished with");
+        s->held[u] = fin;
+        s->committed[u] = n[u];
+        s->finished[u] = 1;
+      }
       break;
     }
-    beam_commit_kernel<<<1, 256, 0, st>>>(b.hist[s->steps & 1], b.hs, b.m, s->steps, b.htok, b.hlen, b.horder, b.nhyp,
-                                          b.done, s->codes, s->ncommit);
+    beam_commit_kernel<<<nreq, 256, 0, st>>>(b.hist[s->steps & 1], b.hs, b.m, s->steps, b.htok, b.hlen, b.horder, b.nhyp,
+                                             b.done, s->codes, cs, s->ncommit);
     IDX_CUDA(cudaGetLastError());
     e->launches++;
-    int* h = (int*)e->pinned_buf(64);
-    IDX_CUDA(cudaMemcpyAsync(h, s->ncommit, 4, cudaMemcpyDeviceToHost, st));
+    int* h = (int*)e->pinned_buf(128);
+    IDX_CUDA(cudaMemcpyAsync(h, s->ncommit, nreq * 4, cudaMemcpyDeviceToHost, st));
+    IDX_CUDA(cudaMemcpyAsync(h + 8, b.done, nreq * 4, cudaMemcpyDeviceToHost, st));
     IDX_CUDA(cudaStreamSynchronize(st));
-    const int n = h[0];
-    IDX_CHECK(n >= s->committed, IDX_ERR_STATE, "internal: the committed prefix of a beam stream shrank");
-    if (n > s->committed) {
-      s->held.resize(n);
-      IDX_CUDA(cudaMemcpyAsync(s->held.data() + s->committed, s->codes + s->committed, (size_t)(n - s->committed) * 4,
-                               cudaMemcpyDeviceToHost, st));
-      IDX_CUDA(cudaStreamSynchronize(st));
-      s->committed = n;
+    std::vector<int> lcp(h, h + nreq), done(h + 8, h + 8 + nreq);
+    bool any_done = false;
+    for (int u = 0; u < nreq; ++u) any_done |= done[u] && !s->finished[u];
+    std::unique_ptr<BeamHost> bh(any_done ? new BeamHost(e, b, s->steps, false) : nullptr);
+    for (int u = 0; u < nreq; ++u) {
+      if (s->finished[u]) continue;
+      std::vector<int>& held = s->held[u];
+      if (done[u]) {      // its stored hypotheses can no longer change: the pick is final
+        const std::vector<int> fin = bh->pick(u, s->m, b.hs, s->steps, s->max_new, stop, s->sp.length_penalty, nullptr);
+        IDX_CHECK((int)fin.size() >= s->committed[u] && std::equal(held.begin(), held.end(), fin.begin()), IDX_ERR_STATE,
+                  "internal: the beam result does not extend the committed prefix");
+        IDX_CUDA(cudaMemcpyAsync(s->codes + (size_t)u * cs, fin.data(), fin.size() * 4, cudaMemcpyHostToDevice, st));
+        IDX_CUDA(cudaStreamSynchronize(st));
+        held = fin;
+        s->committed[u] = (int)fin.size();
+        s->finished[u] = 1;
+        continue;
+      }
+      IDX_CHECK(lcp[u] >= s->committed[u], IDX_ERR_STATE, "internal: the committed prefix of a beam stream shrank");
+      if (lcp[u] > s->committed[u]) {
+        held.resize(lcp[u]);
+        IDX_CUDA(cudaMemcpyAsync(held.data() + s->committed[u], s->codes + (size_t)u * cs + s->committed[u],
+                                 (size_t)(lcp[u] - s->committed[u]) * 4, cudaMemcpyDeviceToHost, st));
+        IDX_CUDA(cudaStreamSynchronize(st));
+        s->committed[u] = lcp[u];
+      }
     }
   }
 }
 
-extern "C" int idx_gpt_stream_next(idx_engine* e, int32_t until, int32_t* codes_out, int32_t* n_committed,
-                                   int32_t* finished) {
+extern "C" int idx_gpt_stream_next_batch(idx_engine* e, const int32_t* until, int32_t* const* codes_out,
+                                         int32_t* n_committed, int32_t* finished) {
   IDX_API_BEGIN
   GptStream* s = open_stream(e);
-  IDX_CHECK(until >= 1, IDX_ERR_ARG, "idx_gpt_stream_next: until must be >= 1");
-  IDX_CHECK(codes_out, IDX_ERR_ARG, "idx_gpt_stream_next: null codes_out");
+  IDX_CHECK(until && codes_out, IDX_ERR_ARG, "idx_gpt_stream_next: null until / codes_out");
+  for (int i = 0; i < s->nreq; ++i) {
+    IDX_CHECK(until[i] >= 1, IDX_ERR_ARG, "idx_gpt_stream_next: until must be >= 1");
+    IDX_CHECK(codes_out[i], IDX_ERR_ARG, "idx_gpt_stream_next: null codes_out");
+  }
   IDX_CUDA(cudaSetDevice(e->device));
-  const int old = s->committed;
-  if (s->m == 1) stream_next1(e, e->gpt, s, until);
-  else stream_next_beams(e, e->gpt, s, until);
-  if (s->committed > old) idx_from_device(e, codes_out + old, s->codes + old, (size_t)(s->committed - old) * 4);
+  int old[8], fin0[8];
+  for (int i = 0; i < s->nreq; ++i) { old[i] = s->committed[i]; fin0[i] = s->finished[i]; }
+  if (s->m == 1) stream_next1(e, e->gpt, s, until, fin0);
+  else stream_next_beams(e, e->gpt, s, until, fin0);
+  for (int i = 0; i < s->nreq; ++i)
+    if (s->committed[i] > old[i])
+      idx_from_device(e, codes_out[i] + old[i], s->codes + (size_t)i * s->cs + old[i], (size_t)(s->committed[i] - old[i]) * 4);
   IDX_CUDA(cudaStreamSynchronize(e->stream));
-  if (n_committed) *n_committed = s->committed;
-  if (finished) *finished = s->finished;
+  for (int i = 0; i < s->nreq; ++i) {
+    if (n_committed) n_committed[i] = s->committed[i];
+    if (finished) finished[i] = s->finished[i];
+  }
   IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_stream_next(idx_engine* e, int32_t until, int32_t* codes_out, int32_t* n_committed,
+                                   int32_t* finished) {
+  return idx_gpt_stream_next_batch(e, &until, &codes_out, n_committed, finished);
 }
 
 extern "C" int idx_gpt_stream_end(idx_engine* e) {
@@ -3137,25 +3231,31 @@ extern "C" int idx_gpt_stream_end(idx_engine* e) {
   IDX_API_END(e)
 }
 
-extern "C" int idx_gpt_stream_beam_state(idx_engine* e, int32_t* hist, int32_t* hyp_tok, int32_t* hyp_len,
-                                         int32_t* hyp_order, int32_t* nhyp_done, int32_t* steps) {
+extern "C" int idx_gpt_stream_beam_state_batch(idx_engine* e, int32_t req, int32_t* hist, int32_t* hyp_tok, int32_t* hyp_len,
+                                               int32_t* hyp_order, int32_t* nhyp_done, int32_t* steps) {
   IDX_API_BEGIN
   GptStream* s = open_stream(e);
   IDX_CHECK(s->m > 1, IDX_ERR_STATE, "idx_gpt_stream_beam_state: the open stream is not a beam search");
+  IDX_CHECK(req >= 0 && req < s->nreq, IDX_ERR_ARG, "idx_gpt_stream_beam_state: req out of range");
   IDX_CUDA(cudaSetDevice(e->device));
   const BeamBufs& b = s->b;
-  const size_t hs = b.hs, m = b.m;
-  if (hist) idx_from_device(e, hist, b.hist[s->steps & 1], m * hs * 4);
-  if (hyp_tok) idx_from_device(e, hyp_tok, b.htok, (m + 1) * hs * 4);
-  if (hyp_len) idx_from_device(e, hyp_len, b.hlen, (m + 1) * 4);
-  if (hyp_order) idx_from_device(e, hyp_order, b.horder, (m + 1) * 4);
+  const size_t hs = b.hs, m = b.m, u = req;
+  if (hist) idx_from_device(e, hist, b.hist[s->steps & 1] + u * m * hs, m * hs * 4);
+  if (hyp_tok) idx_from_device(e, hyp_tok, b.htok + u * (m + 1) * hs, (m + 1) * hs * 4);
+  if (hyp_len) idx_from_device(e, hyp_len, b.hlen + u * (m + 1), (m + 1) * 4);
+  if (hyp_order) idx_from_device(e, hyp_order, b.horder + u * (m + 1), (m + 1) * 4);
   if (nhyp_done) {
-    idx_from_device(e, nhyp_done, b.nhyp, 4);
-    idx_from_device(e, nhyp_done + 1, b.done, 4);
+    idx_from_device(e, nhyp_done, b.nhyp + u, 4);
+    idx_from_device(e, nhyp_done + 1, b.done + u, 4);
   }
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   if (steps) *steps = s->steps;
   IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_stream_beam_state(idx_engine* e, int32_t* hist, int32_t* hyp_tok, int32_t* hyp_len,
+                                         int32_t* hyp_order, int32_t* nhyp_done, int32_t* steps) {
+  return idx_gpt_stream_beam_state_batch(e, 0, hist, hyp_tok, hyp_len, hyp_order, nhyp_done, steps);
 }
 
 extern "C" int idx_gpt_last_timing(const idx_engine* e, double* out4) {

@@ -19,25 +19,35 @@ __global__ void pcm16_kernel(const float* wav, int16_t* pcm, long long n) {
   float v = fminf(fmaxf(32767.f * wav[i], -32767.f), 32767.f);
   pcm[i] = (int16_t)v;
 }
-// One window of a chunked stream joined onto the tail the previous window kept (include/idxtts.h idx_stream_vocode), with
-// the rules of the reference's StreamingDecoder.generate: out[i] = tail[i] * fade_out[i] + wav[i] * fade_in[i] for i < nb
-// (the two halves of np.hanning(2 nb)), wav[src0 + i - nb] after that; the last 512 samples scaled by np.linspace(1, 0,
-// 512) when `fade`; int16 with the truncation of pcm16_kernel.  In double, as numpy computes the blend.
-__global__ void stream_join_kernel(const float* wav, const float* tail, int nb, long long src0, long long n_out, int fade,
-                                   int16_t* pcm) {
+// The windows of one idx_stream_vocode_batch call (at most one per slot), each joined onto the tail its slot kept
+// (include/idxtts.h idx_stream_vocode), with the rules of the reference's StreamingDecoder.generate: out[i] = tail[i] *
+// fade_out[i] + wav[i] * fade_in[i] for i < nb (the two halves of np.hanning(2 nb)), wav[src0 + i - nb] after that; the
+// last 512 samples scaled by np.linspace(1, 0, 512) when `fade`; int16 with the truncation of pcm16_kernel.  In double,
+// as numpy computes the blend.  blockIdx.y: the window.
+struct JoinWin {
+  const float* wav;
+  const float* tail;
+  int16_t* pcm;
+  long long src0, n_out;
+  int nb, fade;
+};
+struct JoinTable { JoinWin w[8]; };
+__global__ void stream_join_kernel(JoinTable t) {
+  const JoinWin& w = t.w[blockIdx.y];
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_out) return;
+  if (i >= w.n_out) return;
+  const int nb = w.nb;
   double v;
   if (i < nb) {
-    const double w = 6.283185307179586 / (2.0 * nb - 1.0);
-    const double fade_in = 0.5 - 0.5 * cos(w * (double)i), fade_out = 0.5 - 0.5 * cos(w * (double)(nb + i));
-    v = (double)tail[i] * fade_out + (double)wav[i] * fade_in;
+    const double c = 6.283185307179586 / (2.0 * nb - 1.0);
+    const double fade_in = 0.5 - 0.5 * cos(c * (double)i), fade_out = 0.5 - 0.5 * cos(c * (double)(nb + i));
+    v = (double)w.tail[i] * fade_out + (double)w.wav[i] * fade_in;
   } else {
-    v = (double)wav[src0 + i - nb];
+    v = (double)w.wav[w.src0 + i - nb];
   }
-  if (fade && i >= n_out - 512) v *= 1.0 - (double)(i - (n_out - 512)) / 511.0;
+  if (w.fade && i >= w.n_out - 512) v *= 1.0 - (double)(i - (w.n_out - 512)) / 511.0;
   v = fmin(fmax(32767.0 * v, -32767.0), 32767.0);
-  pcm[i] = (int16_t)v;
+  w.pcm[i] = (int16_t)v;
 }
 // why the tail refuses a request, or nullptr
 const char* request_error(const idx_vocode_request* r) {
@@ -190,12 +200,15 @@ void codes_to_wav(idx_engine* e, const idx_vocode_request* reqs, int n, int n_st
 }
 }  // namespace
 
-// idx_stream_vocode's device state: the last overlap_samples of the previous window (kept until the next window blends
-// them in) and the window's waveform and int16 buffers, all engine-owned: the tail runs of the windows reset the arena.
+// idx_stream_vocode(_batch)'s device state: per slot the last overlap_samples of its previous window (kept until its next
+// window blends them in), and the windows' waveform and int16 buffers, all engine-owned: the tail runs of the windows
+// reset the arena.
 struct StreamJoin {
-  float* tail = nullptr;
-  long long tail_len = 0, tail_cap = 0;
-  bool has_tail = false;      // false: the next window is joined as the first one
+  struct Slot {
+    float* tail = nullptr;
+    long long tail_len = 0, tail_cap = 0;
+    bool has_tail = false;    // false: the slot's next window is joined as the first one
+  } slot[IDX_STREAM_SLOTS];
   float* wav = nullptr;
   int16_t* pcm = nullptr;
   long long wav_cap = 0, pcm_cap = 0;
@@ -203,7 +216,7 @@ struct StreamJoin {
 
 void stream_join_destroy(StreamJoin* j) {
   if (!j) return;
-  cudaFree(j->tail);
+  for (auto& s : j->slot) cudaFree(s.tail);
   cudaFree(j->wav);
   cudaFree(j->pcm);
   delete j;
@@ -222,67 +235,124 @@ void grow(idx_engine* e, T*& buf, long long& cap, long long n, long long keep) {
   buf = nb;
   cap = n;
 }
+
+// What one window of a call emits: nb blended samples, then wav[src0, src0 + n_out - nb); len = its waveform's samples.
+struct WinPlan {
+  long long len = 0, nb = 0, src0 = 0, n_out = 0, wav_off = 0, pcm_off = 0;
+  bool first = false, last = false;
+};
+
+void stream_vocode_batch(idx_engine* e, const idx_stream_window* w, int n, int n_steps, float cfg_rate) {
+  IDX_CHECK(e && w && n >= 1 && n <= IDX_STREAM_SLOTS, IDX_ERR_ARG, "idx_stream_vocode: null argument or n not in 1..8");
+  IDX_CUDA(cudaSetDevice(e->device));
+  if (!e->sjoin) e->sjoin = new StreamJoin();
+  StreamJoin* j = e->sjoin;
+  // every window is checked before any work: a refused call emits nothing and keeps every slot's tail
+  std::vector<WinPlan> plan(n);
+  std::vector<idx_vocode_request> reqs;
+  bool used[IDX_STREAM_SLOTS] = {};
+  long long wav_total = 0, pcm_total = 0;
+  for (int i = 0; i < n; ++i) {
+    const idx_stream_window& x = w[i];
+    const std::string at = n > 1 ? "idx_stream_vocode_batch: window " + std::to_string(i) + ": " : "idx_stream_vocode: ";
+    auto need = [&](bool ok, const char* why) { if (!ok) throw IdxError(IDX_ERR_ARG, at + why); };
+    need(x.pcm_out && x.n_pcm, "null argument");
+    need(x.slot >= 0 && x.slot < IDX_STREAM_SLOTS, "slot must be 0..7");
+    need(!used[x.slot], "the slot is used by another window of the call");
+    used[x.slot] = true;
+    need((x.flags & ~(IDX_STREAM_FIRST | IDX_STREAM_LAST)) == 0, "unknown flags");
+    WinPlan& q = plan[i];
+    q.first = x.flags & IDX_STREAM_FIRST;
+    q.last = x.flags & IDX_STREAM_LAST;
+    need(x.window || q.last, "a NULL window is the flush and needs IDX_STREAM_LAST");
+    need(x.overlap_samples >= 0, "overlap_samples must be >= 0");
+    const StreamJoin::Slot& sl = j->slot[x.slot];
+    const bool joined = !q.first && sl.has_tail;      // a window without a kept tail is joined as the first one
+    const long long kept = joined ? sl.tail_len : 0, ovlp = x.overlap_samples;
+    if (x.window) {
+      IDX_CHECK(e->bigvgan, IDX_ERR_STATE, "s2mel / codec / bigvgan not initialised");
+      if (const char* why = request_error(x.window)) need(false, why);
+      q.len = (long long)x.window->F * bigvgan_total_up(e->bigvgan);
+      need(q.last || q.len >= 2 * ovlp, "a window that is not the last needs F * 256 >= 2 * overlap_samples");
+    }
+    need((long long)*x.n_pcm >= q.len + kept,
+         "*n_pcm (the capacity of pcm_out) must be >= F * 256 plus the kept tail (at most the previous window's "
+         "overlap_samples)");
+    if (!x.window) {
+      q.n_out = kept;
+    } else if (!joined) {
+      q.n_out = q.last ? q.len : q.len - ovlp;
+    } else {
+      const long long head = std::min(ovlp, q.len), rest = std::max(0LL, q.len - ovlp);
+      q.nb = std::min(kept, head);
+      q.src0 = std::min(ovlp, q.len);
+      q.n_out = q.last ? q.nb + rest : q.nb + rest - ovlp;
+    }
+    q.wav_off = wav_total;
+    q.pcm_off = pcm_total;
+    wav_total += q.len;
+    pcm_total += q.n_out;
+  }
+  grow(e, j->pcm, j->pcm_cap, std::max(pcm_total, 1LL), 0);
+  grow(e, j->wav, j->wav_cap, std::max(wav_total, 1LL), 0);
+  for (int i = 0; i < n; ++i)
+    if (w[i].window) {
+      reqs.push_back(*w[i].window);                   // the windows' tail: the driver of idx_codes_to_wav(_batch)
+      reqs.back().wav_out = j->wav + plan[i].wav_off;
+    }
+  if (!reqs.empty()) codes_to_wav(e, reqs.data(), (int)reqs.size(), n_steps, cfg_rate, n > 1);
+  for (int i = 0; i < n; ++i)
+    if (w[i].window && w[i].window->wav_out)
+      idx_from_device(e, w[i].window->wav_out, j->wav + plan[i].wav_off, (size_t)plan[i].len * 4);
+  // one launch joins every window (the flush reads its slot's kept tail), before any slot keeps a new tail
+  JoinTable t;
+  memset(&t, 0, sizeof(t));
+  long long max_out = 0;
+  for (int i = 0; i < n; ++i) {
+    const WinPlan& q = plan[i];
+    const float* tail = j->slot[w[i].slot].tail;
+    t.w[i] = {w[i].window ? j->wav + q.wav_off : tail, tail, j->pcm + q.pcm_off, q.src0, q.n_out, (int)q.nb,
+              q.last && q.n_out > 512};
+    max_out = std::max(max_out, q.n_out);
+  }
+  if (max_out > 0) {
+    stream_join_kernel<<<dim3((unsigned)((max_out + 255) / 256), (unsigned)n), 256, 0, e->stream>>>(t);
+    IDX_CUDA(cudaGetLastError()); e->launches++;
+    for (int i = 0; i < n; ++i)
+      if (plan[i].n_out > 0) idx_from_device(e, w[i].pcm_out, j->pcm + plan[i].pcm_off, (size_t)plan[i].n_out * 2);
+  }
+  for (int i = 0; i < n; ++i) {                       // keep each window's last overlap_samples for its slot's next one
+    const WinPlan& q = plan[i];
+    StreamJoin::Slot& sl = j->slot[w[i].slot];
+    const long long ovlp = w[i].overlap_samples;
+    if (w[i].window && !q.last) {
+      grow(e, sl.tail, sl.tail_cap, std::max(ovlp, 1LL), 0);
+      if (ovlp > 0)
+        IDX_CUDA(cudaMemcpyAsync(sl.tail, j->wav + q.wav_off + (q.len - ovlp), (size_t)ovlp * 4, cudaMemcpyDeviceToDevice,
+                                 e->stream));
+    }
+  }
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  for (int i = 0; i < n; ++i) {
+    StreamJoin::Slot& sl = j->slot[w[i].slot];
+    sl.has_tail = w[i].window && !plan[i].last;
+    sl.tail_len = sl.has_tail ? w[i].overlap_samples : 0;
+    *w[i].n_pcm = (int32_t)plan[i].n_out;
+  }
+}
 }  // namespace
+
+extern "C" int idx_stream_vocode_batch(idx_engine* e, const idx_stream_window* w, int n, int n_steps, float cfg_rate) {
+  IDX_API_BEGIN
+  stream_vocode_batch(e, w, n, n_steps, cfg_rate);
+  IDX_API_END(e)
+}
 
 extern "C" int idx_stream_vocode(idx_engine* e, const idx_vocode_request* r, int n_steps, float cfg_rate,
                                  int32_t overlap_samples, int32_t flags, int16_t* pcm_out, int32_t* n_pcm) {
   IDX_API_BEGIN
-  IDX_CHECK(e && pcm_out && n_pcm, IDX_ERR_ARG, "idx_stream_vocode: null argument");
-  IDX_CHECK((flags & ~(IDX_STREAM_FIRST | IDX_STREAM_LAST)) == 0, IDX_ERR_ARG, "idx_stream_vocode: unknown flags");
-  const bool first = flags & IDX_STREAM_FIRST, last = flags & IDX_STREAM_LAST;
-  IDX_CHECK(r || last, IDX_ERR_ARG, "idx_stream_vocode: a NULL window is the flush and needs IDX_STREAM_LAST");
-  IDX_CHECK(overlap_samples >= 0, IDX_ERR_ARG, "idx_stream_vocode: overlap_samples must be >= 0");
-  IDX_CUDA(cudaSetDevice(e->device));
-  if (!e->sjoin) e->sjoin = new StreamJoin();
-  StreamJoin* j = e->sjoin;
-  const bool joined = !first && j->has_tail;          // a window without a kept tail is joined as the first one
-  const long long kept = joined ? j->tail_len : 0, ovlp = overlap_samples;
-  long long len = 0;
-  if (r) {
-    IDX_CHECK(e->bigvgan, IDX_ERR_STATE, "s2mel / codec / bigvgan not initialised");
-    IDX_CHECK(r->F >= 1, IDX_ERR_ARG, "bad request");
-    len = (long long)r->F * bigvgan_total_up(e->bigvgan);
-    IDX_CHECK(last || len >= 2 * ovlp, IDX_ERR_ARG,
-              "idx_stream_vocode: a window that is not the last needs F * 256 >= 2 * overlap_samples");
-  }
-  IDX_CHECK((long long)*n_pcm >= len + kept, IDX_ERR_ARG,
-            "idx_stream_vocode: *n_pcm (the capacity of pcm_out) must be >= F * 256 plus the kept tail (at most the previous "
-            "window's overlap_samples)");
-  // what is emitted: nb blended samples, then wav[src0, src0 + n_out - nb)
-  long long nb = 0, src0 = 0, n_out = 0;
-  if (!r) {
-    n_out = kept;
-  } else if (!joined) {
-    n_out = last ? len : len - ovlp;
-  } else {
-    const long long head = std::min(ovlp, len), rest = std::max(0LL, len - ovlp);
-    nb = std::min(kept, head);
-    src0 = std::min(ovlp, len);
-    n_out = last ? nb + rest : nb + rest - ovlp;
-  }
-  grow(e, j->pcm, j->pcm_cap, std::max(n_out, 1LL), 0);
-  if (r) {
-    grow(e, j->wav, j->wav_cap, len, 0);
-    idx_vocode_request w = *r;                        // the window's tail: the driver of idx_codes_to_wav
-    w.wav_out = j->wav;
-    codes_to_wav(e, &w, 1, n_steps, cfg_rate, false);
-    if (r->wav_out) idx_from_device(e, r->wav_out, j->wav, (size_t)len * 4);
-  }
-  if (n_out > 0) {      // the window's waveform, or the kept tail for the flush (read after the buffers have grown)
-    stream_join_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, e->stream>>>(r ? j->wav : j->tail, j->tail, (int)nb, src0, n_out,
-                                                                             last && n_out > 512, j->pcm);
-    IDX_CUDA(cudaGetLastError()); e->launches++;
-    idx_from_device(e, pcm_out, j->pcm, (size_t)n_out * 2);
-  }
-  if (r && !last) {                                   // keep the window's last overlap_samples for the next one
-    grow(e, j->tail, j->tail_cap, std::max(ovlp, 1LL), 0);
-    if (ovlp > 0)
-      IDX_CUDA(cudaMemcpyAsync(j->tail, j->wav + (len - ovlp), (size_t)ovlp * 4, cudaMemcpyDeviceToDevice, e->stream));
-  }
-  IDX_CUDA(cudaStreamSynchronize(e->stream));
-  j->has_tail = r && !last;
-  j->tail_len = j->has_tail ? ovlp : 0;
-  *n_pcm = (int32_t)n_out;
+  const idx_stream_window w = {0, r, overlap_samples, flags, pcm_out, n_pcm};
+  stream_vocode_batch(e, &w, 1, n_steps, cfg_rate);
   IDX_API_END(e)
 }
 

@@ -82,6 +82,11 @@ class VocodeRequest(C.Structure):
                 ("F", C.c_int32), ("wav_out", C.c_void_p), ("pcm16_out", C.c_void_p), ("mel_out", C.c_void_p)]
 
 
+class StreamWindow(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("window", C.POINTER(VocodeRequest)), ("overlap_samples", C.c_int32),
+                ("flags", C.c_int32), ("pcm_out", C.c_void_p), ("n_pcm", C.POINTER(C.c_int32))]
+
+
 class DebugGemm(C.Structure):
     """include/idxtts.h idx_debug_gemm."""
     _fields_ = [("A", C.c_void_p), ("B", C.c_int32), ("Tin", C.c_int32), ("K", C.c_int32), ("lda", C.c_int32),
@@ -257,6 +262,11 @@ def load_library(path: str = None):
     lib.idx_gpt_stream_beam_state.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.POINTER(C.c_int32)]
     lib.idx_stream_vocode.argtypes = [C.c_void_p, C.POINTER(VocodeRequest), C.c_int, C.c_float, C.c_int32, C.c_int32,
                                       C.c_void_p, C.POINTER(C.c_int32)]
+    lib.idx_gpt_stream_begin_batch.argtypes = [C.c_void_p, C.POINTER(GptRequest), C.c_int, C.POINTER(Sampling)]
+    lib.idx_gpt_stream_next_batch.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_void_p),
+                                              C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    lib.idx_gpt_stream_beam_state_batch.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.POINTER(C.c_int32)]
+    lib.idx_stream_vocode_batch.argtypes = [C.c_void_p, C.POINTER(StreamWindow), C.c_int, C.c_int, C.c_float]
     _lib = lib
     return lib
 
@@ -312,37 +322,39 @@ class _OrderedLib:
         return call
 
 
-class GptStream:
-    """An open resumable decode (Engine.gpt_stream).  `codes` holds every code committed so far."""
+class GptStreamBatch:
+    """An open resumable decode of a group of requests (Engine.gpt_stream_batch).  `codes[i]` holds every code of request
+    i committed so far; `n_committed[i]` and `finished[i]` are its counts and flags."""
 
-    def __init__(self, eng, max_new_tokens, num_beams):
-        self._eng, self.num_beams = eng, num_beams
-        self._buf = np.zeros(max_new_tokens, dtype=np.int32)
-        self.n_committed, self.finished, self._open = 0, False, True
+    def __init__(self, eng, nreq, max_new_tokens, num_beams):
+        self._eng, self.nreq, self.num_beams = eng, nreq, num_beams
+        self._bufs = [np.zeros(max_new_tokens, dtype=np.int32) for _ in range(nreq)]
+        self.n_committed, self.finished, self._open = [0] * nreq, [False] * nreq, True
 
     @property
     def codes(self):
-        return self._buf[:self.n_committed]
+        return [b[:n] for b, n in zip(self._bufs, self.n_committed)]
 
     def next(self, until):
-        """Decode until at least `until` codes are committed (or the sequence has finished); returns (the newly committed
-        codes as int32, finished)."""
-        eng, old = self._eng, self.n_committed
-        n, fin = C.c_int32(0), C.c_int32(0)
-        eng._check(eng.lib.idx_gpt_stream_next(eng.h, int(until), _ptr(self._buf), C.byref(n), C.byref(fin)),
-                   "idx_gpt_stream_next")
-        self.n_committed, self.finished = int(n.value), bool(fin.value)
-        return self._buf[old:self.n_committed].copy(), self.finished
+        """Decode until some unfinished request i has at least until[i] committed codes, some request finishes, or all
+        are finished; returns (the newly committed codes of each request as int32 arrays, the finished flags)."""
+        eng, old, k = self._eng, list(self.n_committed), self.nreq
+        u = (C.c_int32 * k)(*[int(x) for x in until])
+        outs = (C.c_void_p * k)(*[b.ctypes.data for b in self._bufs])
+        n, fin = (C.c_int32 * k)(), (C.c_int32 * k)()
+        eng._check(eng.lib.idx_gpt_stream_next_batch(eng.h, u, outs, n, fin), "idx_gpt_stream_next")
+        self.n_committed, self.finished = [int(x) for x in n], [bool(x) for x in fin]
+        return [b[o:c].copy() for b, o, c in zip(self._bufs, old, self.n_committed)], list(self.finished)
 
-    def beam_state(self):
-        """Diagnostic: the beam buffers as the last poll left them (include/idxtts.h idx_gpt_stream_beam_state)."""
-        eng, m, hs = self._eng, self.num_beams, len(self._buf) + 2
+    def beam_state(self, i=0):
+        """Diagnostic: request i's beam buffers as the last poll left them (include/idxtts.h idx_gpt_stream_beam_state)."""
+        eng, m, hs = self._eng, self.num_beams, len(self._bufs[0]) + 2
         hist = np.zeros((m, hs), np.int32)
         htok = np.zeros((m + 1, hs), np.int32)
         hlen, horder, nd = np.zeros(m + 1, np.int32), np.zeros(m + 1, np.int32), np.zeros(2, np.int32)
         steps = C.c_int32(0)
-        eng._check(eng.lib.idx_gpt_stream_beam_state(eng.h, _ptr(hist), _ptr(htok), _ptr(hlen), _ptr(horder), _ptr(nd),
-                                                     C.byref(steps)), "idx_gpt_stream_beam_state")
+        eng._check(eng.lib.idx_gpt_stream_beam_state_batch(eng.h, int(i), _ptr(hist), _ptr(htok), _ptr(hlen), _ptr(horder),
+                                                           _ptr(nd), C.byref(steps)), "idx_gpt_stream_beam_state")
         return dict(hist=hist, hyp_tok=htok, hyp_len=hlen, hyp_order=horder, nhyp=int(nd[0]), done=bool(nd[1]),
                     steps=int(steps.value))
 
@@ -350,6 +362,38 @@ class GptStream:
         if self._open:
             self._open = False
             self._eng._check(self._eng.lib.idx_gpt_stream_end(self._eng.h), "idx_gpt_stream_end")
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+        return False
+
+
+class GptStream:
+    """An open resumable decode of one request (Engine.gpt_stream): the one-request case of GptStreamBatch.  `codes`
+    holds every code committed so far."""
+
+    def __init__(self, batch):
+        self._b, self.num_beams = batch, batch.num_beams
+
+    codes = property(lambda self: self._b.codes[0])
+    n_committed = property(lambda self: self._b.n_committed[0])
+    finished = property(lambda self: self._b.finished[0])
+
+    def next(self, until):
+        """Decode until at least `until` codes are committed (or the sequence has finished); returns (the newly committed
+        codes as int32, finished)."""
+        new, fin = self._b.next([until])
+        return new[0], fin[0]
+
+    def beam_state(self):
+        """Diagnostic: the beam buffers as the last poll left them (include/idxtts.h idx_gpt_stream_beam_state)."""
+        return self._b.beam_state(0)
+
+    def close(self):
+        self._b.close()
 
     def __enter__(self):
         return self
@@ -488,27 +532,37 @@ class Engine:
             return out, [logits[i][: int(ncodes[i][0])] for i in range(n)]
         return out
 
-    def gpt_stream(self, prompt, max_new_tokens, repetition_penalty=10.0, do_sample=False, num_beams=1, top_k=0,
-                   top_p=1.0, temperature=1.0, length_penalty=0.0, seed=0, forbid_stop_before=0, forced_codes=None,
-                   return_logits=False, mel_pos_mode=0):
+    def gpt_stream(self, prompt, max_new_tokens, **kw):
         """Resumable decode of one prompt (include/idxtts.h idx_gpt_stream_*): the arguments of gpt_generate for one
         request; the prefill runs here.  Returns a GptStream: `.next(until)` decodes until at least `until` codes are
         committed and returns (the newly committed codes, finished).  Over the whole stream the codes are those
         gpt_generate returns.  Close it with `.close()` or a `with` block: GPT calls are refused while it is open."""
+        return GptStream(self.gpt_stream_batch([prompt], max_new_tokens, **kw))
+
+    def gpt_stream_batch(self, prompts, max_new_tokens, repetition_penalty=10.0, do_sample=False, num_beams=1, top_k=0,
+                         top_p=1.0, temperature=1.0, length_penalty=0.0, seed=0, forbid_stop_before=0, forced_codes=None,
+                         return_logits=False, mel_pos_mode=0):
+        """Resumable decode of a group of prompts as ONE decode group (include/idxtts.h idx_gpt_stream_*_batch): the
+        arguments of gpt_generate; refused when len(prompts) * num_beams exceeds max_batch.  Returns a GptStreamBatch:
+        `.next(until_list)` returns (the newly committed codes of each request, their finished flags).  Over the whole
+        stream request i's codes are those gpt_generate(prompts)[i] returns.  Close it with `.close()` or a `with`
+        block: GPT calls are refused while it is open."""
         if return_logits:
             raise ValueError("gpt_stream does not return logits")
-        pr = _as_f32(prompt)
-        req = GptRequest()
-        req.prompt_emb = _ptr(pr)
-        req.prompt_len = int(pr.shape[0])
-        if forced_codes is not None:        # passed through: the library refuses teacher forcing on a stream
-            fc = np.zeros(max_new_tokens, dtype=np.int32)
-            req.forced_codes = _ptr(fc)
+        n = len(prompts)
+        prs = [_as_f32(p) for p in prompts]
+        reqs = (GptRequest * max(1, n))()
+        fc = np.zeros(max_new_tokens, dtype=np.int32)
+        for i, pr in enumerate(prs):
+            reqs[i].prompt_emb = _ptr(pr)
+            reqs[i].prompt_len = int(pr.shape[0])
+            if forced_codes is not None:    # passed through: the library refuses teacher forcing on a stream
+                reqs[i].forced_codes = _ptr(fc)
         sp = Sampling(int(do_sample), int(num_beams), int(top_k), float(top_p), float(temperature),
                       float(repetition_penalty), float(length_penalty), int(max_new_tokens),
                       int(seed), int(forbid_stop_before), int(mel_pos_mode))
-        self._check(self.lib.idx_gpt_stream_begin(self.h, C.byref(req), C.byref(sp)), "idx_gpt_stream_begin")
-        return GptStream(self, int(max_new_tokens), int(num_beams))
+        self._check(self.lib.idx_gpt_stream_begin_batch(self.h, reqs, n, C.byref(sp)), "idx_gpt_stream_begin")
+        return GptStreamBatch(self, n, int(max_new_tokens), int(num_beams))
 
     # ------------------------------------------------------- v1 / v1.5 GPT side (row a13) --
     def v1_cond_init(self, c: dict, n_latents=32):
@@ -758,25 +812,46 @@ class Engine:
         codes_to_wav, then its waveform is cross-faded onto the last overlap_samples the previous window kept on the
         device.  first: drop any kept tail; last: emit everything, faded out over its last 512 samples.  codes=None with
         last=True flushes the kept tail.  Buffers pass through as in codes_to_wav (the int16 output lives where z lives).
-        Returns dict(pcm=int16 [emitted samples], wav=[F*256] f32 of the window when want_wav)."""
-        if first:
-            self._join_kept = 0
-        kept = getattr(self, "_join_kept", 0)
-        if codes is None:
-            r, res, keep, n = None, {}, None, kept
-        else:
-            r, res, keep = self._vocode_request(codes, prompt_condition, ref_mel, style, z, F, want_wav, False, False)
-            n = int(F) * self._bigvgan_up + kept
-        on_dev = codes is not None and _is_cuda(z)
-        pcm = torch.empty(max(n, 1), dtype=torch.int16, device=z.device) if on_dev else np.empty(max(n, 1), dtype=np.int16)
-        n_pcm = C.c_int32(n)
-        flags = (1 if first else 0) | (2 if last else 0)
-        self._check(self.lib.idx_stream_vocode(self.h, None if r is None else C.byref(r), int(n_steps), float(cfg_rate),
-                                               int(overlap_samples), flags, _ptr(pcm), C.byref(n_pcm)),
+        Returns dict(pcm=int16 [emitted samples], wav=[F*256] f32 of the window when want_wav).  The one-window case of
+        stream_vocode_batch, on join slot 0."""
+        w = dict(slot=0, codes=codes, prompt_condition=prompt_condition, ref_mel=ref_mel, style=style, z=z, F=F,
+                 overlap_samples=overlap_samples, first=first, last=last, want_wav=want_wav)
+        return self.stream_vocode_batch([w], n_steps, cfg_rate)[0]
+
+    def stream_vocode_batch(self, windows, n_steps=25, cfg_rate=0.7):
+        """Windows of several chunked streams in one call (include/idxtts.h idx_stream_vocode_batch): their tails run as
+        one codes_to_wav_batch (one packed CFM solve), then one kernel joins each onto the tail its join slot kept.
+        windows: list of dicts with `slot` (0..7, at most one window per slot), the stream_vocode arguments (codes,
+        prompt_condition, ref_mel, style, z, F, overlap_samples, first, last, want_wav; codes=None flushes the slot).
+        Returns one dict per window: pcm (int16, where its z lives), wav when want_wav."""
+        kept = self.__dict__.setdefault("_join_kept", [0] * 8)
+        ws = (StreamWindow * max(1, len(windows)))()
+        hold, results, n_pcm = [], [], []
+        for i, q in enumerate(windows):
+            slot, first, last = int(q.get("slot", 0)), bool(q.get("first")), bool(q.get("last"))
+            codes, z = q.get("codes"), q.get("z")
+            k = 0 if (first or not 0 <= slot < 8) else kept[slot]
+            if codes is None:
+                r, res, n = None, {}, k
+            else:
+                r, res, keep = self._vocode_request(codes, q["prompt_condition"], q["ref_mel"], q["style"], z, q["F"],
+                                                    q.get("want_wav", False), False, False)
+                hold.append((r, keep))
+                n = int(q["F"]) * self._bigvgan_up + k
+            on_dev = codes is not None and _is_cuda(z)
+            pcm = torch.empty(max(n, 1), dtype=torch.int16, device=z.device) if on_dev else np.empty(max(n, 1), np.int16)
+            cnt = C.c_int32(n)
+            n_pcm.append(cnt)
+            res["pcm"] = pcm
+            results.append(res)
+            ws[i] = StreamWindow(slot, None if r is None else C.pointer(r), int(q.get("overlap_samples", 0)),
+                                 (1 if first else 0) | (2 if last else 0), _ptr(pcm), C.pointer(cnt))
+        self._check(self.lib.idx_stream_vocode_batch(self.h, ws, len(windows), int(n_steps), float(cfg_rate)),
                     "idx_stream_vocode")
-        self._join_kept = 0 if (last or codes is None) else int(overlap_samples)
-        res["pcm"] = pcm[:n_pcm.value]
-        return res
+        for q, res, cnt in zip(windows, results, n_pcm):
+            kept[int(q.get("slot", 0))] = 0 if (q.get("last") or q.get("codes") is None) else int(q.get("overlap_samples", 0))
+            res["pcm"] = res["pcm"][:cnt.value]
+        return results
 
     def codes_to_wav_batch(self, requests, n_steps=25, cfg_rate=0.7, want_wav=True, want_pcm16=False, want_mel=False):
         """codes_to_wav for several segments in one call (include/idxtts.h idx_codes_to_wav_batch): their CFM solves run as

@@ -69,49 +69,106 @@ def schedule(n_codes, chunk_codes=100, overlap_codes=20):
     return out
 
 
-def stream_segment(engine, prompt_emb, prompt_condition, ref_mel, style, *, chunk_codes=100, overlap_codes=20,
-                   duration_factor=1.0, n_steps=25, cfg_rate=0.7, **generation_kwargs):
-    """Decode one segment and yield its audio as int16 arrays, window by window.
+def stream_segments(engine, prompts, prompt_condition, ref_mel, style, *, chunk_codes=100, overlap_codes=20,
+                    duration_factor=1.0, n_steps=25, cfg_rate=0.7, **generation_kwargs):
+    """Decode several segments as one decode group and yield their audio, round by round, as (audio_list, done_list):
+    the shape of the reference's batch StreamingDecoder.generate.  audio_list[i] is request i's int16 array of the round,
+    or None when it has nothing this round; done_list[i] is True on the round that emits its last samples (exactly once
+    per request; a request that ends without a single code is done with audio None).
 
-    prompt_emb: the [cond][text] rows of Engine.gpt_prepare_inputs.  prompt_condition [P, content_dim], ref_mel [80, P],
-    style [style_dim]: the tensors infer_generator caches (cache_s2mel_prompt, cache_mel, cache_s2mel_style).
-    generation_kwargs: those of Engine.gpt_generate (max_new_tokens defaults to the reference's 1500).  Each window's
-    codes are cut before the stop token (infer_v2_5.py:809-821); its noise z [80, P + F] is drawn with torch.randn, as
-    cfm.inference draws it, on the device of ref_mel.  The arrays live where ref_mel lives (numpy for host inputs)."""
-    ws = WindowSchedule(chunk_codes, overlap_codes)
+    prompts: the [cond][text] rows of Engine.gpt_prepare_inputs, one per request; len(prompts) * num_beams must fit in
+    one decode group (max_batch).  prompt_condition, ref_mel, style: one set shared by every request, or lists with one
+    per request (P may differ).  Request i has its own window schedule (that of generate_chunks for that sample alone: a
+    request's last window runs as soon as that request finishes) and join slot i.
+
+    A round is one Engine.stream_vocode_batch call: after each GptStreamBatch.next (which returns as soon as a request
+    reaches its next window end or finishes), every window that is due (full windows, the final partial window of a
+    request that finished, the flush of one that ended without one) runs in one call; a request with several due
+    windows has them run in consecutive rounds.  Window noise z [80, P_i + F] is drawn with torch.randn on the device of
+    ref_mel, one draw per window, in the order the rounds run and, within a round, in request order."""
+    n_req = len(prompts)
+    per_req = isinstance(ref_mel, (list, tuple))
+    pcs, mels, styles = ((list(x) if per_req else [x] * n_req) for x in (prompt_condition, ref_mel, style))
+    if len(mels) != n_req or len(pcs) != n_req or len(styles) != n_req:
+        raise ValueError("prompt_condition / ref_mel / style: one set, or one per prompt")
     ovlp = overlap_samples(overlap_codes, duration_factor)
     if window_frames(chunk_codes, duration_factor) * HOP < 2 * ovlp:
         raise ValueError("a full window must hold at least twice the overlap: chunk_codes too small for overlap_codes")
     generation_kwargs.setdefault("max_new_tokens", 1500)
     stop = engine.gpt_cfg.stop_mel_token
-    P = int(ref_mel.shape[-1])
-    dev = ref_mel.device if (torch is not None and isinstance(ref_mel, torch.Tensor)) else "cpu"
-    first = True
+    scheds = [WindowSchedule(chunk_codes, overlap_codes) for _ in range(n_req)]
+    started = [False] * n_req           # a window of the request has run: its slot may keep a tail
+    ended = [False] * n_req             # the request's last codes are known
+    pending = [[] for _ in range(n_req)]   # due windows: (start, end, last), or None for the flush
+    reported = [False] * n_req
 
-    def window(codes, last):
-        nonlocal first
-        F = window_frames(len(codes), duration_factor)
-        z = torch.randn(80, P + F, device=dev)
-        if dev == "cpu":
-            z = z.numpy()
-        out = engine.stream_vocode(np.ascontiguousarray(codes), prompt_condition, ref_mel, style, z, F,
-                                   overlap_samples=ovlp, first=first, last=last, n_steps=n_steps, cfg_rate=cfg_rate)
-        first = False
-        return out["pcm"]
+    def devof(m):
+        return m.device if (torch is not None and isinstance(m, torch.Tensor)) else "cpu"
 
-    with engine.gpt_stream(prompt_emb, **generation_kwargs) as st:
-        n = 0
-        finished = False
-        while not finished:
-            _, finished = st.next(ws.next_end)
-            codes = st.codes
-            hit = np.flatnonzero(codes == stop)
-            n = int(hit[0]) if hit.size else len(codes)
-            finished = finished or bool(hit.size)
-            for a, b in ws.ready(n):
-                yield window(codes[a:b], False)
-    fin = ws.final(n)
-    if fin is not None:
-        yield window(st.codes[fin[0]:fin[1]], True)
-    elif not first:
-        yield engine.stream_vocode(None, last=True)["pcm"]
+    def rounds(st):
+        while any(pending):
+            calls, who = [], []
+            for i in range(n_req):
+                if not pending[i]:
+                    continue
+                w = pending[i].pop(0)
+                if w is None:
+                    calls.append(dict(slot=i, codes=None, last=True))
+                else:
+                    a, b, last = w
+                    F = window_frames(b - a, duration_factor)
+                    P = int(mels[i].shape[-1])
+                    z = torch.randn(80, P + F, device=devof(mels[i]))
+                    if devof(mels[i]) == "cpu":
+                        z = z.numpy()
+                    calls.append(dict(slot=i, codes=np.ascontiguousarray(st.codes[i][a:b]), prompt_condition=pcs[i],
+                                      ref_mel=mels[i], style=styles[i], z=z, F=F, overlap_samples=ovlp,
+                                      first=not started[i], last=last))
+                    started[i] = True
+                who.append(i)
+            outs = engine.stream_vocode_batch(calls, n_steps, cfg_rate)
+            audio, done = [None] * n_req, [False] * n_req
+            for i, o in zip(who, outs):
+                audio[i] = o["pcm"]
+                if ended[i] and not pending[i]:
+                    done[i] = reported[i] = True
+            yield audio, done
+
+    with engine.gpt_stream_batch(prompts, **generation_kwargs) as st:
+        while not all(ended):
+            st.next([1 if ended[i] else scheds[i].next_end for i in range(n_req)])
+            silent = [False] * n_req
+            for i in range(n_req):
+                if ended[i]:
+                    continue
+                codes = st.codes[i]
+                hit = np.flatnonzero(codes == stop)
+                n = int(hit[0]) if hit.size else len(codes)
+                pending[i] += [(a, b, False) for a, b in scheds[i].ready(n)]
+                if st.finished[i] or hit.size:
+                    ended[i] = True
+                    fin = scheds[i].final(n)
+                    if fin is not None:
+                        pending[i].append((fin[0], fin[1], True))
+                    elif started[i] or pending[i]:
+                        pending[i].append(None)
+                    else:
+                        silent[i] = reported[i] = True
+            yield from rounds(st)
+            if any(silent):
+                yield [None] * n_req, silent
+
+
+def stream_segment(engine, prompt_emb, prompt_condition, ref_mel, style, **kwargs):
+    """Decode one segment and yield its audio as int16 arrays, window by window: the one-request case of
+    stream_segments.
+
+    prompt_emb: the [cond][text] rows of Engine.gpt_prepare_inputs.  prompt_condition [P, content_dim], ref_mel [80, P],
+    style [style_dim]: the tensors infer_generator caches (cache_s2mel_prompt, cache_mel, cache_s2mel_style).
+    kwargs: chunk_codes, overlap_codes, duration_factor, n_steps, cfg_rate and those of Engine.gpt_generate
+    (max_new_tokens defaults to the reference's 1500).  Each window's codes are cut before the stop token
+    (infer_v2_5.py:809-821); its noise z [80, P + F] is drawn with torch.randn, as cfm.inference draws it, on the device
+    of ref_mel.  The arrays live where ref_mel lives (numpy for host inputs)."""
+    for audio, _ in stream_segments(engine, [prompt_emb], prompt_condition, ref_mel, style, **kwargs):
+        if audio[0] is not None:
+            yield audio[0]
