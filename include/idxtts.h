@@ -218,6 +218,36 @@ int idx_gpt_stream_next_batch(idx_engine* e, const int32_t* until, int32_t* cons
                               int32_t* finished);
 int idx_gpt_stream_beam_state_batch(idx_engine* e, int32_t req, int32_t* hist, int32_t* hyp_tok, int32_t* hyp_len,
                                     int32_t* hyp_order, int32_t* nhyp_done, int32_t* steps);
+/* A SERVING group: a resumable decode of `slots` rows that requests join and leave while it runs.  It is a GPT stream
+ * (idx_gpt_stream_end closes it; the state rules of idx_gpt_stream_begin hold, and idx_gpt_stream_next refuses it with
+ * IDX_ERR_STATE).  It always decodes on gpt_decode8_kernel with B = slots; empty, finished and released rows stay in
+ * every launch as masked columns.  A lone live request decodes on gpt_decode8_kernel too, not gpt_decode1_kernel.
+ * Contract: a request admitted at any group step, into any slot, decodes codes bitwise equal to those idx_gpt_generate
+ * returns for it as request seq_index of a call with the same idx_sampling (seed included), provided that call runs it
+ * in a decode group of at least 2 requests (where gpt_decode8_kernel is picked).  This holds whatever the other slots
+ * hold, and admissions, releases and tail calls between next calls do not change it: each row has its own step and its
+ * own Philox sequence, the MMA columns are independent, attention runs per (sequence, head pair), and the pick is keyed
+ * by (the row's step, seq_index).
+ *   begin    sampling and seed belong to the group.  slots 2..8 and <= max_batch.  Refused (IDX_ERR_ARG): num_beams != 1,
+ *            the strict fp32 path, an engine without gpt_decode8_kernel (IDX_GPT_V8=0 / IDX_GPT_V2=0) and whatever
+ *            idx_gpt_generate refuses in sp.  Every slot starts empty.
+ *   admit    runs req's prefill into the KV rows of `slot` (as idx_gpt_generate runs a prompt) and starts the request at
+ *            the group's current step with Philox sequence index seq_index (>= 0).  Nothing else is touched.  Refused
+ *            (IDX_ERR_ARG) before any work: slot out of range or occupied, forced_codes, a bad or too long prompt
+ *            (prompt_len > max_prompt, prompt_len + max_new_tokens + 1 > KV positions).  codes_out, n_codes_out and
+ *            logits_out of req are not used.
+ *   next     until, codes_out, n_committed, finished: [slots] each, as idx_gpt_stream_next_batch over the OCCUPIED slots
+ *            (empty slots' until and codes_out are not read; their n_committed and finished come back 0).  A slot's
+ *            counts are its request's own.  Returns as soon as a live slot has at least until[i] committed codes, a slot
+ *            finishes, or no slot is live (at once when nothing is admitted).  A launch covers at most 32 steps.
+ *   release  frees an occupied slot: after a finished request's codes have been read, or as a cancel of a live one (its
+ *            committed codes stay where next wrote them; the row is masked from the next launch on).  IDX_ERR_ARG for
+ *            an empty slot.                                                                                          */
+int idx_gpt_serve_begin(idx_engine* e, const idx_sampling* sp, int32_t slots);
+int idx_gpt_serve_admit(idx_engine* e, int32_t slot, const idx_gpt_request* req, int32_t seq_index);
+int idx_gpt_serve_next(idx_engine* e, const int32_t* until, int32_t* const* codes_out, int32_t* n_committed,
+                       int32_t* finished);
+int idx_gpt_serve_release(idx_engine* e, int32_t slot);
 
 /* Build the [cond(3)][start_text, text.., stop_text] prompt embeddings of
  * prepare_gpt_inputs (gpt/model_v2.py:648-714,754-768) on the device.

@@ -120,7 +120,11 @@ struct GptParams {
   uint2* kvt;           // [2][D] tagged k, v (bf16-valued) of the position being decoded
   unsigned epoch0;      // first epoch of this launch (2 per layer per step)
   int seq_base;         // global index of row 0 (requests beyond one decode group run as consecutive groups)
-  int pos_plain;        // 1: mel position k at step k (decoding without a cache, infer.py:101); 0: trap P1 (k + 1)
+  // gpt_decode8_kernel: row b's request took its step 0 at group step row_step0[b] and samples on Philox sequence
+  // row_seqidx[b] (ordinary groups: 0 and seq_base + b; a serving group admits requests at later steps)
+  int row_step0[8];
+  int row_seqidx[8];
+  int pos_plain;       // 1: mel position k at step k (decoding without a cache, infer.py:101); 0: trap P1 (k + 1)
   // beam search (beam_step_kernel runs between single-step launches)
   int ext_sample;       // 1: leave the logits in p.logits and skip the sampling phase
   int beams;            // rows per utterance (also set for the beam driver's prefill launch: the prefill probe's request index)
@@ -1701,6 +1705,7 @@ struct GptState {
   // second-generation batch-1 decode kernel
   int v2 = 0, ring_rows = 0;
   int v8 = 0, ring_rows8 = 0;       // gpt_decode8_kernel (2..8 sequences per group)
+  int bias_cap8 = 0;                // its per-CTA bias table (floats)
   size_t smem_v8 = 0;
   size_t smem_v2 = 0;
   __nv_bfloat16* wstream1 = nullptr;
@@ -1999,7 +2004,7 @@ static size_t smem_bytes_v8(int D, int R, int bias_cap, int ocap, int V) {
          sizeof(float) * 4 * (size_t)D + 64;
 }
 static void launch_decode8(idx_engine* e, GptState* g, GptParams& p) {
-  p.bias_cap = g->bias_cap;
+  p.bias_cap = g->bias_cap8;
   p.ocap = g->ocap;
   p.ring_rows = g->ring_rows8;
   IDX_CUDA(cudaMemsetAsync(g->barrier, 0, (32 + 256) * sizeof(unsigned), e->stream));
@@ -2173,12 +2178,23 @@ extern "C" int idx_gpt_init(idx_engine* e, const idx_gpt_config* cfg) {
       // the 8-row decode kernel shares the row stream; its ring is smaller (8 activation rows and 8-wide partial sums in shared memory)
       g->v8 = (H % 2 == 0) && 8 * (H / 2) <= G && !(getenv("IDX_GPT_V8") && atoi(getenv("IDX_GPT_V8")) == 0);
       if (g->v8) {
+        // sized by the exact per-CTA needs of this kernel: its bias table and its largest phase (every row of a phase sits
+        // in the ring at once).  The rounded-up bounds above left a 132-SM H100 one ring row short at model_dim 1280
+        // (62 rows for a 63-row mel head phase), and the 2..8-row decode fell back to gpt_fused_kernel there.
+        int need8 = 0;
+        g->bias_cap8 = 0;
+        auto cols = [&](int N, int i) { return (int)(((long long)N * (i + 1)) / G - ((long long)N * i) / G); };   // col_begin
+        for (int i = 0; i < G; ++i) {
+          const int nq = cols(3 * D, i), no = cols(D, i), nf = cols(FF, i), nh = cols(V, i);
+          g->bias_cap8 = std::max(g->bias_cap8, L * (nq + 2 * no + nf) + nh);
+          need8 = std::max(need8, std::max(std::max(nq, nf), std::max((FF / D) * no, nh)));
+        }
         int R8 = 0;
-        while (smem_bytes_v8(D, R8 + 1, g->bias_cap, g->ocap, V) <= (size_t)dev_smem - 1024) ++R8;
+        while (smem_bytes_v8(D, R8 + 1, g->bias_cap8, g->ocap, V) <= (size_t)dev_smem - 1024) ++R8;
         if (getenv("IDX_GPT_RING")) R8 = std::min(R8, atoi(getenv("IDX_GPT_RING")));
-        if (R8 >= std::max(std::max(mq, mf), std::max((FF / D) * mo, mh))) {
+        if (R8 >= need8) {
           g->ring_rows8 = R8;
-          g->smem_v8 = smem_bytes_v8(D, R8, g->bias_cap, g->ocap, V);
+          g->smem_v8 = smem_bytes_v8(D, R8, g->bias_cap8, g->ocap, V);
           if (D / 32 == 40) IDX_CUDA(cudaFuncSetAttribute(gpt_decode8_kernel<40>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->smem_v8));
           else IDX_CUDA(cudaFuncSetAttribute(gpt_decode8_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->smem_v8));
         } else {
@@ -2729,6 +2745,14 @@ static void reset_rows(idx_engine* e, GptState* g, int nreq, const std::vector<i
   IDX_CUDA(cudaStreamSynchronize(e->stream));  // host vectors go out of scope
 }
 
+// Rows of a group that starts together: row b takes its step 0 at group step 0 and samples as request seq_base + b.
+static void lockstep_rows(GptParams& p) {
+  for (int b = 0; b < 8; ++b) {
+    p.row_step0[b] = 0;
+    p.row_seqidx[b] = p.seq_base + b;
+  }
+}
+
 // The sampler inputs every decode path refuses (idx_gpt_generate, idx_gpt_stream_begin).
 static void check_sampling(const idx_sampling* sp) {
   IDX_CHECK(sp->num_beams >= 1, IDX_ERR_ARG, "num_beams must be >= 1");
@@ -2871,6 +2895,7 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   p.do_sample = sp->do_sample; p.top_k = sp->top_k; p.top_p = sp->top_p; p.temperature = sp->temperature;
   p.seed = sp->seed;
   p.seq_base = g->seq_base;
+  lockstep_rows(p);
   p.pos_plain = sp->mel_pos_mode == 1;
   p.codes = d_codes; p.forced = d_forced; p.logits_dump = d_ldump;
   if (probe_on) probe_arm_decode(e, g, p, pb, max_new);
@@ -2972,6 +2997,11 @@ struct GptStream {
   BeamParams bp;
   GptParams p;                         // the decode launches' parameters
   std::vector<int> held[8];            // beams: the codes committed so far, per request
+  // serving group (idx_gpt_serve_begin): nreq = slots; an empty slot is held finished so that the decode masks it
+  bool serve = false;
+  int occupied[8] = {};
+  float* prompt = nullptr;             // [max_prompt + 8][D] the admitted request's prompt
+  PrefillTile* tiles = nullptr;        // its prefill tiles
   ~GptStream() { if (mem) cudaFree(mem); }
 };
 
@@ -3062,6 +3092,7 @@ extern "C" int idx_gpt_stream_begin_batch(idx_engine* e, const idx_gpt_request* 
     p.do_sample = sp->do_sample; p.top_k = sp->top_k; p.top_p = sp->top_p; p.temperature = sp->temperature;
     p.seed = sp->seed;
     p.seq_base = g->seq_base;
+    lockstep_rows(p);
     p.pos_plain = sp->mel_pos_mode == 1;
     p.codes = s->codes;
     s->kind = (nreq == 1 && g->v2) ? 1 : (nreq > 1 && g->v8) ? 8 : 0;   // the kernel idx_gpt_generate picks
@@ -3087,18 +3118,19 @@ static bool stream_stop(const GptStream* s, const int32_t* until, const int* fin
   return all;
 }
 
-// num_beams = 1: the rows advance in lockstep and every decoded code is committed; each launch ends at the smallest
-// `until` of the unfinished requests (at most 64 steps for the batch-1 kernel, 32 otherwise, as in idx_gpt_generate).
+// num_beams = 1: every decoded code is committed and the unfinished rows advance together; each launch ends at the
+// smallest `until` of the unfinished requests (at most 64 steps for the batch-1 kernel, 32 otherwise, as in
+// idx_gpt_generate).  The rows of a serving group are at their own steps: the launch length is counted per row.
 static void stream_next1(idx_engine* e, GptState* g, GptStream* s, const int32_t* until, const int* fin0) {
   GptParams& p = s->p;
   const int SPL = s->kind == 1 ? 64 : 32;
   int* h = (int*)e->pinned_buf(128);
   while (!stream_stop(s, until, fin0)) {
-    int end = s->max_new;
+    int left = SPL;
     for (int i = 0; i < s->nreq; ++i)
-      if (!s->finished[i]) end = std::min(end, (int)until[i]);
+      if (!s->finished[i]) left = std::min(left, std::min((int)until[i], s->max_new) - s->committed[i]);
     p.step0 = s->steps;
-    p.nsteps = std::min(SPL, end - s->steps);
+    p.nsteps = left;
     if (s->kind == 1) launch_decode1(e, g, p);
     else if (s->kind == 8) launch_decode8(e, g, p);
     else launch_fused(e, g, p);
@@ -3196,6 +3228,7 @@ extern "C" int idx_gpt_stream_next_batch(idx_engine* e, const int32_t* until, in
                                          int32_t* n_committed, int32_t* finished) {
   IDX_API_BEGIN
   GptStream* s = open_stream(e);
+  IDX_CHECK(!s->serve, IDX_ERR_STATE, "idx_gpt_stream_next: the open stream is a serving group (idx_gpt_serve_next)");
   IDX_CHECK(until && codes_out, IDX_ERR_ARG, "idx_gpt_stream_next: null until / codes_out");
   for (int i = 0; i < s->nreq; ++i) {
     IDX_CHECK(until[i] >= 1, IDX_ERR_ARG, "idx_gpt_stream_next: until must be >= 1");
@@ -3228,6 +3261,159 @@ extern "C" int idx_gpt_stream_end(idx_engine* e) {
   IDX_CUDA(cudaSetDevice(e->device));
   IDX_CUDA(cudaStreamSynchronize(e->stream));
   gpt_stream_free(e->gpt);
+  IDX_API_END(e)
+}
+
+// ------------------------------------------------------------------ serving group --
+// A resumable decode whose rows are filled and freed while it runs (include/idxtts.h idx_gpt_serve_*): a GptStream of
+// `slots` rows that always decodes on gpt_decode8_kernel.  A request admitted at group step s runs its own step k - s
+// (GptParams::row_step0) and samples on its own Philox sequence (row_seqidx); MMA columns, attention (one CTA per
+// sequence and head pair) and the pick are per row, so its codes do not depend on where, when or beside whom it runs.
+// An empty or released slot is held finished on the device: a masked column of every launch.
+static GptStream* open_serve(idx_engine* e) {
+  GptStream* s = open_stream(e);
+  IDX_CHECK(s->serve, IDX_ERR_STATE, "the open stream is not a serving group (idx_gpt_serve_begin opens one)");
+  return s;
+}
+
+// the decode state of one row (host values, copied before the call returns)
+static void set_row(idx_engine* e, GptState* g, int row, int tok, int finished, int plen, const unsigned* seen) {
+  const int v[4] = {tok, 0, finished, plen};
+  cudaStream_t st = e->stream;
+  IDX_CUDA(cudaMemcpyAsync(g->tok + row, &v[0], 4, cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaMemcpyAsync(g->nout + row, &v[1], 4, cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaMemcpyAsync(g->finished + row, &v[2], 4, cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaMemcpyAsync(g->prompt_len + row, &v[3], 4, cudaMemcpyHostToDevice, st));
+  const size_t wv = (size_t)((g->cfg.number_mel_codes + 31) / 32);
+  if (seen) IDX_CUDA(cudaMemcpyAsync(g->seen + row * wv, seen, wv * 4, cudaMemcpyHostToDevice, st));
+  IDX_CUDA(cudaStreamSynchronize(st));
+}
+
+extern "C" int idx_gpt_serve_begin(idx_engine* e, const idx_sampling* sp, int32_t slots) {
+  IDX_API_BEGIN
+  IDX_CHECK(e && e->gpt, IDX_ERR_STATE, "idx_gpt_init has not been called");
+  GptState* g = e->gpt;
+  IDX_CHECK(!g->gstream, IDX_ERR_STATE, kStreamOpen);
+  IDX_CHECK(sp, IDX_ERR_ARG, "null sampling");
+  IDX_CHECK(!g->strict, IDX_ERR_ARG, "idx_gpt_serve_begin: the strict fp32 path (weights_bf16 = 0) has no serving group");
+  IDX_CHECK(g->v8, IDX_ERR_ARG,
+            "idx_gpt_serve_begin: a serving group decodes on gpt_decode8_kernel, which this engine does not run "
+            "(IDX_GPT_V8=0 / IDX_GPT_V2=0)");
+  check_sampling(sp);
+  IDX_CHECK(sp->num_beams == 1, IDX_ERR_ARG, "idx_gpt_serve_begin: num_beams must be 1");
+  const idx_gpt_config& c = g->cfg;
+  IDX_CHECK(slots >= 2 && slots <= 8 && slots <= c.max_batch, IDX_ERR_ARG, "idx_gpt_serve_begin: slots must be 2..8 and <= max_batch");
+  const int max_new = sp->max_new_tokens, D = c.model_dim;
+  IDX_CHECK(c.number_mel_codes <= 40 * 256, IDX_ERR_ARG, "vocabulary too large for the device sampler");
+  IDX_CHECK(max_new >= 1 && max_new + 2 <= c.max_mel_positions, IDX_ERR_ARG,
+            "max_new_tokens must satisfy k+1 <= mel_pos rows - 1 (SURVEY A.3)");
+  IDX_CUDA(cudaSetDevice(e->device));
+  std::unique_ptr<GptStream> s(new GptStream());
+  s->sp = *sp; s->nreq = slots; s->m = 1; s->max_new = max_new; s->cs = max_new; s->kind = 8; s->serve = true;
+  const int ntiles = (c.max_prompt + 7) / 8;
+  const size_t bytes = (size_t)(c.max_prompt + 8) * D * 4 + ntiles * sizeof(PrefillTile) + (size_t)8 * (max_new + 2) * 4 + 8 * 256;
+  IDX_CUDA(cudaMalloc(&s->mem, bytes));
+  s->a.base = (char*)s->mem;
+  s->a.cap = bytes;
+  s->prompt = s->a.get<float>((size_t)(c.max_prompt + 8) * D);
+  s->tiles = s->a.get<PrefillTile>(ntiles);
+  s->codes = s->a.get<int>((size_t)8 * (max_new + 2));
+  for (int i = 0; i < 8; ++i) {
+    set_row(e, g, i, c.start_mel_token, 1, 0, nullptr);
+    s->finished[i] = 1;
+  }
+  GptParams& p = s->p;
+  fill_common(e, g, p);
+  p.B = slots; p.mode = 1; p.max_new = max_new; p.rep_penalty = sp->repetition_penalty;
+  p.forbid_stop_before = sp->forbid_stop_before;
+  p.do_sample = sp->do_sample; p.top_k = sp->top_k; p.top_p = sp->top_p; p.temperature = sp->temperature;
+  p.seed = sp->seed;
+  p.pos_plain = sp->mel_pos_mode == 1;
+  p.codes = s->codes;
+  g->gstream = s.release();
+  IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_serve_admit(idx_engine* e, int32_t slot, const idx_gpt_request* req, int32_t seq_index) {
+  IDX_API_BEGIN
+  GptStream* s = open_serve(e);
+  GptState* g = e->gpt;
+  const idx_gpt_config& c = g->cfg;
+  IDX_CHECK(slot >= 0 && slot < s->nreq, IDX_ERR_ARG, "idx_gpt_serve_admit: slot out of range");
+  IDX_CHECK(!s->occupied[slot], IDX_ERR_ARG, "idx_gpt_serve_admit: the slot is occupied (idx_gpt_serve_release frees it)");
+  IDX_CHECK(req && seq_index >= 0, IDX_ERR_ARG, "idx_gpt_serve_admit: null request or seq_index < 0");
+  IDX_CHECK(!req->forced_codes, IDX_ERR_ARG, "idx_gpt_serve_admit: forced_codes is not defined for a stream");
+  const int plen = req->prompt_len, D = c.model_dim;
+  IDX_CHECK(req->prompt_emb && plen >= 1 && plen <= c.max_prompt, IDX_ERR_ARG, "bad prompt");
+  IDX_CHECK(plen + s->max_new + 1 <= g->maxpos, IDX_ERR_ARG, "KV cache too small");
+  IDX_CUDA(cudaSetDevice(e->device));
+  // prefill into the slot's cache rows, as idx_gpt_generate runs a prompt: tiles of 8 positions of gpt_fused_kernel.
+  // A prefill launch writes the KV of its tiles' sequence and the scratch rows every decode step rewrites before reading
+  // (xg, qg, fg, part); no other row's decode state or cache.
+  std::vector<PrefillTile> tiles;
+  for (int p0 = 0; p0 < plen; p0 += 8) tiles.push_back({slot, p0, std::min(8, plen - p0), p0});
+  idx_to_device(e, s->prompt, req->prompt_emb, (size_t)plen * D * 4);
+  IDX_CUDA(cudaMemcpyAsync(s->tiles, tiles.data(), tiles.size() * sizeof(PrefillTile), cudaMemcpyHostToDevice, e->stream));
+  GptParams pp;
+  fill_common(e, g, pp);
+  pp.B = 8; pp.mode = 0; pp.nsteps = (int)tiles.size(); pp.prompt = s->prompt; pp.tiles = s->tiles;
+  pp.max_new = s->max_new; pp.rep_penalty = s->sp.repetition_penalty;
+  launch_fused(e, g, pp);
+  // step-0 state of the row (reset_rows for one row): start token, no codes, the P2 fake prompt ids
+  std::vector<unsigned> seen((c.number_mel_codes + 31) / 32, 0u);
+  seen[1 >> 5] |= 1u << 1;
+  seen[c.start_mel_token >> 5] |= 1u << (c.start_mel_token & 31);
+  set_row(e, g, slot, c.start_mel_token, 0, plen, seen.data());
+  s->p.row_step0[slot] = s->steps;
+  s->p.row_seqidx[slot] = seq_index;
+  s->occupied[slot] = 1;
+  s->committed[slot] = 0;
+  s->finished[slot] = 0;
+  IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_serve_next(idx_engine* e, const int32_t* until, int32_t* const* codes_out, int32_t* n_committed,
+                                  int32_t* finished) {
+  IDX_API_BEGIN
+  GptStream* s = open_serve(e);
+  IDX_CHECK(until && codes_out, IDX_ERR_ARG, "idx_gpt_serve_next: null until / codes_out");
+  int u[8], old[8], fin0[8];
+  for (int i = 0; i < s->nreq; ++i) {
+    if (s->occupied[i]) {
+      IDX_CHECK(until[i] >= 1, IDX_ERR_ARG, "idx_gpt_serve_next: until must be >= 1");
+      IDX_CHECK(codes_out[i], IDX_ERR_ARG, "idx_gpt_serve_next: null codes_out");
+    }
+    u[i] = s->occupied[i] ? until[i] : 1;
+    old[i] = s->committed[i];
+    fin0[i] = s->finished[i];
+  }
+  IDX_CUDA(cudaSetDevice(e->device));
+  stream_next1(e, e->gpt, s, u, fin0);
+  for (int i = 0; i < s->nreq; ++i)
+    if (s->occupied[i] && s->committed[i] > old[i])
+      idx_from_device(e, codes_out[i] + old[i], s->codes + (size_t)i * s->cs + old[i], (size_t)(s->committed[i] - old[i]) * 4);
+  IDX_CUDA(cudaStreamSynchronize(e->stream));
+  for (int i = 0; i < s->nreq; ++i) {
+    if (n_committed) n_committed[i] = s->occupied[i] ? s->committed[i] : 0;
+    if (finished) finished[i] = s->occupied[i] ? s->finished[i] : 0;
+  }
+  IDX_API_END(e)
+}
+
+extern "C" int idx_gpt_serve_release(idx_engine* e, int32_t slot) {
+  IDX_API_BEGIN
+  GptStream* s = open_serve(e);
+  IDX_CHECK(slot >= 0 && slot < s->nreq, IDX_ERR_ARG, "idx_gpt_serve_release: slot out of range");
+  IDX_CHECK(s->occupied[slot], IDX_ERR_ARG, "idx_gpt_serve_release: the slot is empty");
+  IDX_CUDA(cudaSetDevice(e->device));
+  if (!s->finished[slot]) {      // a cancel: the row is masked from the next launch on
+    const int one = 1;
+    IDX_CUDA(cudaMemcpyAsync(e->gpt->finished + slot, &one, 4, cudaMemcpyHostToDevice, e->stream));
+    IDX_CUDA(cudaStreamSynchronize(e->stream));
+  }
+  s->occupied[slot] = 0;
+  s->finished[slot] = 1;
+  s->committed[slot] = 0;
   IDX_API_END(e)
 }
 

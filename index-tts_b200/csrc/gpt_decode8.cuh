@@ -152,7 +152,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
     sm.xres = (float*)q;          q += sizeof(float) * (size_t)B8 * p.ocap;
     sm.seen_s = (unsigned*)q;     q += sizeof(unsigned) * (size_t)wv;
   }
-  __shared__ int s_plen[B8], s_tok[B8], s_fin[B8];
+  __shared__ int s_plen[B8], s_tok[B8], s_fin[B8], s_step0[B8], s_seq[B8];
   if (tid == 0) {
     for (int s = 0; s < NBAR; ++s) ptx::mbar_init(&sm.full[s], 1);
     ptx::fence_mbar_init();
@@ -183,7 +183,14 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
     s_plen[tid] = (tid < B) ? p.prompt_len[tid] : 0;
     s_tok[tid] = (tid < B) ? p.tok[tid] : 0;
     s_fin[tid] = (tid < B) ? p.finished[tid] : 1;
+    s_step0[tid] = p.row_step0[tid];
+    s_seq[tid] = p.row_seqidx[tid];
   }
+  // Row b's own step at group step k.  Ordinary groups: k itself (k < max_new).  A finished or empty row of a serving
+  // group runs on as a masked column for as long as the group does: the cap keeps its KV write, attention context and
+  // mel position inside its own slot's rows.
+  auto row_k = [&](int b, int k) { return min(k - s_step0[b], p.max_new - 1); };
+  auto mel_row = [&](int kb) { return (kb == 0 || p.pos_plain) ? kb : kb + 1; };   // P1: mel position kb+1 with the KV cache
   auto make_phase = [&](int ncols, int nt, int nseg) {
     Phase1 ph;
     ph.nitems = nt * nseg;
@@ -309,12 +316,12 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
       v[j].w = (v[j].w - mean) * rstd * ww.w + b4.w;
     }
   };
-  auto ln_rows = [&](bool emb, int posidx, const float* w1, const float* b1, const float* w2, const float* b2) {
+  auto ln_rows = [&](bool emb, int k, const float* w1, const float* b1, const float* w2, const float* b2) {
     float4 v[NV];
     if (warp < B) {
       if (emb) {
         const float4* er = (const float4*)(p.mel_emb + (size_t)s_tok[warp] * D) + lane;
-        const float4* pr = (const float4*)(p.mel_pos + (size_t)posidx * D) + lane;
+        const float4* pr = (const float4*)(p.mel_pos + (size_t)mel_row(row_k(warp, k)) * D) + lane;
 #pragma unroll
         for (int j = 0; j < NV; ++j) {
           const float4 a4 = __ldg(er + 32 * j), c4 = __ldg(pr + 32 * j);
@@ -352,14 +359,15 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
   __nv_bfloat16* ob = (__nv_bfloat16*)p.part;      // [8][D] attention output, bf16 in fragment order (`part` is free in this kernel)
 
   for (; step < p.nsteps && !alldone; ++step) {
-    const int k = p.step0 + step;
-    const int posidx = (k == 0 || p.pos_plain) ? k : k + 1;   // P1: mel position k+1 with the KV cache
+    const int k = p.step0 + step;                // the group's step; row b is at its own step row_k(b, k)
     PROF_STAMP();
     // this CTA's slice of the residual stream of the 8 input rows
     for (int idx = tid; idx < B8 * no; idx += NCT) {
       const int b = idx / no, cl = idx % no;
       float v = 0.f;
-      if (b < B) v = rnd(__ldg(p.mel_emb + (size_t)s_tok[b] * D + o0 + cl) + __ldg(p.mel_pos + (size_t)posidx * D + o0 + cl), rr);
+      if (b < B)
+        v = rnd(__ldg(p.mel_emb + (size_t)s_tok[b] * D + o0 + cl) + __ldg(p.mel_pos + (size_t)mel_row(row_k(b, k)) * D + o0 + cl),
+                rr);
       sm.xres[b * p.ocap + cl] = v;
     }
     PROF_STAMP();
@@ -372,7 +380,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
       FINE8(0);
       cp_async_wait_all();
       ptx::named_bar_sync(1, NCT);                 // LN1 parameters (buffer A) visible
-      ln_rows(l == 0, posidx, lnA, lnA + D, nullptr, nullptr);
+      ln_rows(l == 0, k, lnA, lnA + D, nullptr, nullptr);
       ptx::named_bar_sync(1, NCT);
       issue_fitting();
       FINE8(1);
@@ -392,7 +400,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
           p.qg[(size_t)b * D + c] = v;
           if (prb) prb[(size_t)b * 2 * D + c] = v;
         } else {
-          const size_t base = (((size_t)l * p.nseq + b) * p.maxpos + (s_plen[b] + k)) * D;
+          const size_t base = (((size_t)l * p.nseq + b) * p.maxpos + (s_plen[b] + row_k(b, k))) * D;
           const __nv_bfloat16 kvb = __float2bfloat16_rn(v);
           if (c < 2 * D) p.kc[base + (c - D)] = kvb;
           else p.vc[base + (c - 2 * D)] = kvb;
@@ -406,7 +414,7 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
       if (cta < B * (H / 2)) {
         const int b = cta / (H / 2), h = 2 * (cta % (H / 2)) + (warp >> 2);
         const int w4 = warp & 3;
-        const int ctx = s_plen[b] + k + 1;
+        const int ctx = s_plen[b] + row_k(b, k) + 1;
         const int g4 = lane >> 3, sub = lane & 7;
         const size_t cbase = ((size_t)l * p.nseq + b) * p.maxpos;
         const size_t coff = (size_t)h * HD + sub * 8;
@@ -645,22 +653,24 @@ __global__ void __launch_bounds__(NCT, 1) gpt_decode8_kernel(const GptParams p) 
       while (j + 1 < sc.nth && cl >= split_begin(nh, sc.nth, j + 1)) ++j;
       const float lg = rnd(red8_sum(sm.red, j, cl - split_begin(nh, sc.nth, j), b) + sm.bias_s[L * bstride + cl], rr);
       p.logits[(size_t)b * V + h0 + cl] = lg;
-      if (p.logits_dump) p.logits_dump[((size_t)b * p.max_new + k) * V + h0 + cl] = lg;
+      if (p.logits_dump) p.logits_dump[((size_t)b * p.max_new + row_k(b, k)) * V + h0 + cl] = lg;
     }
     gsync();
 
     // ---------------- sampling: CTA b decides for sequence b ----------------
     if (cta < B) {
-      const int b = cta;
-      const int tk = pick_token(sample_args(p, s_fin[b]), sm.red, sm.seen_s, p.logits + (size_t)b * V, k, b);
+      const int b = cta, kb = row_k(b, k);
+      SampleArgs sa = sample_args(p, s_fin[b]);
+      sa.seq_base = 0;                          // the Philox counter is (kb, row_seqidx[b])
+      const int tk = pick_token(sa, sm.red, sm.seen_s, p.logits + (size_t)b * V, kb, s_seq[b]);
       if (tid == 0 && !s_fin[b]) {
-        p.codes[(size_t)b * p.max_new + k] = tk;
-        p.nout[b] = k + 1;
+        p.codes[(size_t)b * p.max_new + kb] = tk;
+        p.nout[b] = kb + 1;
         int feed = tk;
         int fin = 0;
-        if (p.forced) feed = p.forced[(size_t)b * p.max_new + k];
+        if (p.forced) feed = p.forced[(size_t)b * p.max_new + kb];
         else if (tk == p.stop_tok) fin = 1;
-        if (k + 1 >= p.max_new) fin = 1;
+        if (kb + 1 >= p.max_new) fin = 1;
         p.tok[b] = feed;
         if (fin) p.finished[b] = 1;
         sm.seen_s[feed >> 5] |= 1u << (feed & 31);

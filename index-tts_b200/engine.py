@@ -267,6 +267,11 @@ def load_library(path: str = None):
                                               C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     lib.idx_gpt_stream_beam_state_batch.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.POINTER(C.c_int32)]
     lib.idx_stream_vocode_batch.argtypes = [C.c_void_p, C.POINTER(StreamWindow), C.c_int, C.c_int, C.c_float]
+    lib.idx_gpt_serve_begin.argtypes = [C.c_void_p, C.POINTER(Sampling), C.c_int32]
+    lib.idx_gpt_serve_admit.argtypes = [C.c_void_p, C.c_int32, C.POINTER(GptRequest), C.c_int32]
+    lib.idx_gpt_serve_next.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_void_p), C.POINTER(C.c_int32),
+                                       C.POINTER(C.c_int32)]
+    lib.idx_gpt_serve_release.argtypes = [C.c_void_p, C.c_int32]
     _lib = lib
     return lib
 
@@ -357,6 +362,63 @@ class GptStreamBatch:
                                                            _ptr(nd), C.byref(steps)), "idx_gpt_stream_beam_state")
         return dict(hist=hist, hyp_tok=htok, hyp_len=hlen, hyp_order=horder, nhyp=int(nd[0]), done=bool(nd[1]),
                     steps=int(steps.value))
+
+    def close(self):
+        if self._open:
+            self._open = False
+            self._eng._check(self._eng.lib.idx_gpt_stream_end(self._eng.h), "idx_gpt_stream_end")
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+        return False
+
+
+class GptServe:
+    """An open serving group (Engine.gpt_serve): `slots` decode rows that requests join (`admit`) and leave (`release`)
+    while the group runs.  For an occupied slot, `codes[s]` holds every code of its request committed so far and
+    `n_committed[s]` / `finished[s]` are its count and flag; `occupied[s]` says whether the slot holds a request."""
+
+    def __init__(self, eng, slots, max_new_tokens):
+        self._eng, self.slots, self._max_new = eng, slots, max_new_tokens
+        self._bufs = [np.zeros(0, dtype=np.int32) for _ in range(slots)]
+        self.occupied, self.n_committed, self.finished = [False] * slots, [0] * slots, [False] * slots
+        self._open = True
+
+    @property
+    def codes(self):
+        return [b[:n] if o else None for b, n, o in zip(self._bufs, self.n_committed, self.occupied)]
+
+    def admit(self, slot, prompt, seq_index):
+        """Run the prefill of `prompt` ([S, D] rows of gpt_prepare_inputs) into `slot` and start its decode at the group's
+        current step, sampling as request `seq_index` of a gpt_generate call with the group's arguments."""
+        eng, pr = self._eng, _as_f32(prompt)
+        req = GptRequest()
+        req.prompt_emb, req.prompt_len = _ptr(pr), int(pr.shape[0])
+        eng._check(eng.lib.idx_gpt_serve_admit(eng.h, int(slot), C.byref(req), int(seq_index)), "idx_gpt_serve_admit")
+        self._bufs[slot] = np.zeros(self._max_new, dtype=np.int32)    # a fresh array: the last occupant's codes stay valid
+        self.occupied[slot], self.n_committed[slot], self.finished[slot] = True, 0, False
+
+    def release(self, slot):
+        """Free `slot`: after its finished request's codes have been read, or as a cancel of a live request."""
+        eng = self._eng
+        eng._check(eng.lib.idx_gpt_serve_release(eng.h, int(slot)), "idx_gpt_serve_release")
+        self.occupied[slot], self.n_committed[slot], self.finished[slot] = False, 0, False
+
+    def next(self, until):
+        """Decode until some live slot s has at least until[s] committed codes, some slot finishes, or no slot is live;
+        returns (the newly committed codes of each slot, None for an empty one; the finished flags).  until[s] of an empty
+        slot is not read."""
+        eng, old, k = self._eng, list(self.n_committed), self.slots
+        u = (C.c_int32 * k)(*[int(x) if o else 1 for x, o in zip(until, self.occupied)])
+        outs = (C.c_void_p * k)(*[b.ctypes.data if o else None for b, o in zip(self._bufs, self.occupied)])
+        n, fin = (C.c_int32 * k)(), (C.c_int32 * k)()
+        eng._check(eng.lib.idx_gpt_serve_next(eng.h, u, outs, n, fin), "idx_gpt_serve_next")
+        self.n_committed, self.finished = [int(x) for x in n], [bool(x) for x in fin]
+        new = [b[o:c].copy() if occ else None for b, o, c, occ in zip(self._bufs, old, self.n_committed, self.occupied)]
+        return new, list(self.finished)
 
     def close(self):
         if self._open:
@@ -563,6 +625,19 @@ class Engine:
                       int(seed), int(forbid_stop_before), int(mel_pos_mode))
         self._check(self.lib.idx_gpt_stream_begin_batch(self.h, reqs, n, C.byref(sp)), "idx_gpt_stream_begin")
         return GptStreamBatch(self, n, int(max_new_tokens), int(num_beams))
+
+    def gpt_serve(self, slots, max_new_tokens, repetition_penalty=10.0, do_sample=False, num_beams=1, top_k=0, top_p=1.0,
+                  temperature=1.0, length_penalty=0.0, seed=0, forbid_stop_before=0, mel_pos_mode=0):
+        """A serving group of `slots` rows (include/idxtts.h idx_gpt_serve_*) with the sampling arguments of gpt_generate:
+        requests are admitted into free slots and released while the group runs.  A request admitted with seq_index i
+        decodes the codes gpt_generate returns for request i of a call with the same arguments, provided that call decodes
+        it in a group of at least 2 requests.  Returns a GptServe; close it with `.close()` or a `with` block: GPT calls are
+        refused while it is open."""
+        sp = Sampling(int(do_sample), int(num_beams), int(top_k), float(top_p), float(temperature),
+                      float(repetition_penalty), float(length_penalty), int(max_new_tokens),
+                      int(seed), int(forbid_stop_before), int(mel_pos_mode))
+        self._check(self.lib.idx_gpt_serve_begin(self.h, C.byref(sp), int(slots)), "idx_gpt_serve_begin")
+        return GptServe(self, int(slots), int(max_new_tokens))
 
     # ------------------------------------------------------- v1 / v1.5 GPT side (row a13) --
     def v1_cond_init(self, c: dict, n_latents=32):

@@ -159,6 +159,151 @@ def stream_segments(engine, prompts, prompt_condition, ref_mel, style, *, chunk_
                 yield [None] * n_req, silent
 
 
+class StreamServer:
+    """Chunked streaming for a caller that serves clients: requests are submitted at any time and join a running decode
+    group (Engine.gpt_serve) as its slots free up, instead of waiting for a whole stream_segments group to drain.
+
+    submit() queues a request and returns its id; before each decode call the waiting requests are admitted in
+    submission order, each into the lowest free slot, which is also its join slot of Engine.stream_vocode_batch.  round()
+    runs one round and returns its events (rid, pcm or None, done).  A request's windows, noise draws, first / last
+    flags, flush and silent-end rules are those of stream_segments for that request alone: its window schedule cut
+    before the stop token, one torch.randn(80, P + F) per window on the device of its ref_mel (within a round in slot
+    order), its first window with first=True, done exactly once.  A round runs a decode call only when no window is
+    waiting, then at most one window per slot in one stream_vocode_batch call.  A slot is released when its request is
+    done or cancelled.
+
+    The sequence index of a request is its id (the submission counter) and the sampling seed is drawn once per server
+    from torch's generator unless `seed` is passed, so request i decodes the codes gpt_generate returns for request i of
+    all submitted prompts with that seed (when that call decodes it in a group of at least 2 requests).  The slots stay
+    in one gpt_decode8_kernel group even when a single request is live."""
+
+    def __init__(self, engine, slots=8, chunk_codes=100, overlap_codes=20, duration_factor=1.0, n_steps=25, cfg_rate=0.7,
+                 **generation_kwargs):
+        self._ovlp = overlap_samples(overlap_codes, duration_factor)
+        WindowSchedule(chunk_codes, overlap_codes)        # refuses overlap_codes >= chunk_codes
+        if window_frames(chunk_codes, duration_factor) * HOP < 2 * self._ovlp:
+            raise ValueError("a full window must hold at least twice the overlap: chunk_codes too small for overlap_codes")
+        generation_kwargs.setdefault("max_new_tokens", 1500)
+        if "seed" not in generation_kwargs:
+            generation_kwargs["seed"] = int(torch.randint(0, 2 ** 62, (1,)).item())
+        self._eng, self._chunk, self._overlap, self._df = engine, chunk_codes, overlap_codes, duration_factor
+        self._n_steps, self._cfg_rate = n_steps, cfg_rate
+        self._stop = engine.gpt_cfg.stop_mel_token
+        self._gen = engine.gpt_serve(slots, **generation_kwargs)
+        self._waiting = []                  # rids in submission order
+        self._req = {}                      # rid -> request state, from submit until done or cancel
+        self._slot = [None] * slots         # rid in each slot
+        self._count = 0
+
+    def submit(self, prompt_emb, prompt_condition, ref_mel, style):
+        """Queue one request (the arguments of stream_segment); returns its id."""
+        rid = self._count
+        self._count += 1
+        self._req[rid] = dict(prompt=prompt_emb, pc=prompt_condition, mel=ref_mel, style=style, slot=None,
+                              sched=WindowSchedule(self._chunk, self._overlap), pending=[], started=False, ended=False)
+        self._waiting.append(rid)
+        return rid
+
+    def cancel(self, rid):
+        """Drop a waiting or running request: no event of it follows.  Returns False when it is unknown or done."""
+        r = self._req.pop(rid, None)
+        if r is None:
+            return False
+        if r["slot"] is None:
+            self._waiting.remove(rid)
+        else:
+            self._free(r["slot"])
+        return True
+
+    @property
+    def busy(self):
+        """Whether a request is waiting or running."""
+        return bool(self._req)
+
+    def _free(self, slot):
+        self._gen.release(slot)
+        self._slot[slot] = None
+
+    def _decode(self):
+        events = []
+        for s in range(len(self._slot)):
+            if self._slot[s] is None and self._waiting:
+                rid = self._waiting.pop(0)
+                self._gen.admit(s, self._req[rid]["prompt"], rid)
+                self._req[rid]["slot"], self._slot[s] = s, rid
+        live = [s for s, rid in enumerate(self._slot) if rid is not None and not self._req[rid]["ended"]]
+        if not live:
+            return events
+        self._gen.next([self._req[rid]["sched"].next_end if rid is not None else 1 for rid in self._slot])
+        for s in live:
+            r = self._req[self._slot[s]]
+            codes = self._gen.codes[s]
+            hit = np.flatnonzero(codes == self._stop)
+            n = int(hit[0]) if hit.size else len(codes)
+            r["codes"] = codes
+            r["pending"] += [(a, b, False) for a, b in r["sched"].ready(n)]
+            if self._gen.finished[s] or hit.size:
+                r["ended"] = True
+                fin = r["sched"].final(n)
+                if fin is not None:
+                    r["pending"].append((fin[0], fin[1], True))
+                elif r["started"] or r["pending"]:
+                    r["pending"].append(None)
+                else:                       # ended without a single code: done, silent
+                    events.append((self._slot[s], None, True))
+                    del self._req[self._slot[s]]
+                    self._free(s)
+        return events
+
+    def round(self):
+        """One round: a decode call when no window is waiting (after admitting waiting requests), then every slot's next
+        due window in one stream_vocode_batch call.  Returns the round's events (rid, pcm int16 array or None, done)."""
+        events = []
+        if not any(self._req[rid]["pending"] for rid in self._slot if rid is not None):
+            events += self._decode()
+        calls, who = [], []
+        for s, rid in enumerate(self._slot):
+            if rid is None or not self._req[rid]["pending"]:
+                continue
+            r = self._req[rid]
+            w = r["pending"].pop(0)
+            if w is None:
+                calls.append(dict(slot=s, codes=None, last=True))
+            else:
+                a, b, last = w
+                F = window_frames(b - a, self._df)
+                dev = r["mel"].device if (torch is not None and isinstance(r["mel"], torch.Tensor)) else "cpu"
+                z = torch.randn(80, int(r["mel"].shape[-1]) + F, device=dev)
+                calls.append(dict(slot=s, codes=np.ascontiguousarray(r["codes"][a:b]), prompt_condition=r["pc"],
+                                  ref_mel=r["mel"], style=r["style"], z=z.numpy() if dev == "cpu" else z, F=F,
+                                  overlap_samples=self._ovlp, first=not r["started"], last=last))
+                r["started"] = True
+            who.append(s)
+        if calls:
+            outs = self._eng.stream_vocode_batch(calls, self._n_steps, self._cfg_rate)
+            for s, o in zip(who, outs):
+                rid = self._slot[s]
+                done = self._req[rid]["ended"] and not self._req[rid]["pending"]
+                events.append((rid, o["pcm"], done))
+                if done:
+                    del self._req[rid]
+                    self._free(s)
+        return events
+
+    def close(self):
+        """End the serving group; requests still waiting or running are dropped."""
+        self._gen.close()
+        self._req.clear()
+        self._waiting.clear()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+        return False
+
+
 def stream_segment(engine, prompt_emb, prompt_condition, ref_mel, style, **kwargs):
     """Decode one segment and yield its audio as int16 arrays, window by window: the one-request case of
     stream_segments.
