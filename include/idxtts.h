@@ -346,10 +346,11 @@ int idx_gpt_profile(idx_engine* e, int enable, int64_t* stamps_out, int n);
  * layer of the last decode step: stamps_out [num_SMs][64] (0 where a slot is unused).                          */
 int idx_gpt_profile_fine(idx_engine* e, int64_t* stamps_out, int n);
 /* Diagnostic (tests): arm an attention probe for the NEXT idx_gpt_generate call (bf16 path, one decode group).  It
- * records the decode kernel of that call: with num_beams = 1 the batch-1 kernel or the 2..8-sequence kernel, with
- * num_beams > 1 the beam rows of gpt_fused_kernel (nreq * num_beams <= max_seqs, max_batch; row u * num_beams + j is
- * beam j of request u).  For every decode step k, probed layer l and row b the kernel records q as its attention reads
- * it (fp32) and the normalised attention output before its bf16 rounding:
+ * records the decode kernel of that call: with num_beams = 1 the batch-1 kernel or the 2..8-sequence kernel (or, where
+ * idx_gpt_init left it out, the rows of gpt_fused_kernel), with num_beams > 1 the beam rows of gpt_fused_kernel
+ * (nreq * num_beams <= max_seqs, max_batch; row u * num_beams + j is beam j of request u).  For every decode step k,
+ * probed layer l and row b the kernel records q as its attention reads it (fp32) and the normalised attention output
+ * before its bf16 rounding:
  *   qo_out     [max_steps][nl][max_seqs][2][model_dim] f32, [..][0] = q, [..][1] = attention output;
  *              nl = 1 (layer >= 0: that layer only) or layers (layer = -1); only the first max_new_tokens steps and
  *              the first nreq * num_beams rows are written (beam search: every step the call ran, pad steps included)

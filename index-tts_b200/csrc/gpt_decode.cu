@@ -2785,10 +2785,7 @@ extern "C" int idx_gpt_generate(idx_engine* e, const idx_gpt_request* reqs, int 
   g->probe_armed = g->pprobe_armed = 0;
   const int rows = nreq * sp->num_beams;      // decode rows of one group
   if (probe_on) {
-    const bool dec1 = nreq == 1 && g->v2, dec8 = nreq > 1 && g->v8;
-    IDX_CHECK(!g->strict && (sp->num_beams > 1 || dec1 || dec8) && rows <= c.max_batch, IDX_ERR_ARG,
-              "the attention probe records one decode group of gpt_decode1 / gpt_decode8 (num_beams = 1) or of gpt_fused_kernel "
-              "(num_beams > 1), bf16 path");
+    IDX_CHECK(!g->strict && rows <= c.max_batch, IDX_ERR_ARG, "the attention probe records one decode group of the bf16 path");
     IDX_CHECK(rows <= g->probe_seqs && sp->max_new_tokens <= g->probe_steps, IDX_ERR_ARG, "attention probe buffer too small");
   }
   if (pprobe_on) {

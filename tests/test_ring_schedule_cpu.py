@@ -149,7 +149,11 @@ def check_stream(r, rows, nsteps):
     assert r.fill == 0 and r.tix == r.cons_tile == nsteps * len(rows)
 
 
-GEOMS = [  # (D, V, G, L, R of the 1-row kernel, R of the 8-row kernel) — R as idx_gpt_init computes them on a 227 KB SM
+# (D, V, G SMs, L, R of the 1-row kernel, R of the 8-row kernel).  For D = 1280 the R are those idx_gpt_init computes
+# from a 227 KB shared-memory budget at that SM count: on the 132-SM H100 SXM the 8-row ring is exactly its largest phase
+# (the 63-row mel head), with no spare row; at 148 SMs that phase is 56 rows.  The D = 256 rings are deep ones.
+GEOMS = [
+    (1280, 8194, 132, 24, 71, 63),
     (1280, 8194, 148, 24, 72, 63),
     (256, 8194, 148, 3, 400, 380),
 ]
